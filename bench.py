@@ -12,9 +12,9 @@ One "step" = one pass of the hot path over one 4096-ray batch of synthetic lego-
     893 190 144 FLOP/ray roofline of SURVEY 8d; with N GPUs also `train_dp`: data parallel on a FIXED global 4096-ray batch
     (strong scaling, one all-reduce of the flat 4.77 MB gradient per step) and `frame`: an 800x800 frame ray-sharded over the
     ranks with the [rays,5] all-gather (BASELINE configs[3], [4]).
-  * `torch_gpu` (N = 1): the UNMODIFIED reference (baseline/_ref/run_nerf.py: its own render(), autograd and Adam) on the
+  * `torch_gpu` (N = 1): the UNMODIFIED reference (oracle/_ref/run_nerf.py: its own render(), autograd and Adam) on the
     same GPU, fp32 and TF32 matmuls, forward and train -- what the north star's ">= 10x" is relative to.
-  * `cpu_baseline` / `--impl reference`: the reference on the host cores (the unmodified script when baseline/_ref is
+  * `cpu_baseline` / `--impl reference`: the reference on the host cores (the unmodified script when oracle/_ref is
     present -- kind "reference" --, else the op-chain port oracle/torch_ref.py -- kind "port").
 JSON keys: see the build spec (value, e2e, roofline, cpu_baseline, clocks, gpu_launches ...).
 """
@@ -32,7 +32,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 N_RAYS, N_SAMPLES, N_IMPORTANCE = 4096, 64, 128
 FLOP_PER_RAY_FWD = 303_824_896          # SURVEY 8d / Appendix B: 593 408 MAC x 2 x 256 evaluations
@@ -48,15 +48,15 @@ def load_peaks():
         with open(path) as f:
             pk = json.load(f)
         return float(pk["bf16_tflops"]), "measured (MEASURED_PEAKS.json bf16_tflops, burst; fp16 == bf16 rate)", pk.get("bf16_tflops_sustained"), pk.get("hbm_gbs")
-    return 1590.0, "fallback (B200_PROFILING.md 1.59 PFLOP/s)", None, 6650.0
+    return 989.0, "fallback (H100 SXM data sheet: 989 dense fp16 TFLOP/s at up to 700 W; not reached)", None, 3350.0
 
 
 # --------------------------------------------------------------------------------------------
-# the unmodified reference (baseline/_ref), importable on CPU or GPU
+# the unmodified reference (oracle/_ref), importable on CPU or GPU
 # --------------------------------------------------------------------------------------------
 
 def import_reference():
-    """run_nerf from baseline/_ref with stand-ins for the two packages this image lacks (neither is on the path)."""
+    """run_nerf from oracle/_ref with stand-ins for the two packages this image lacks (neither is on the path)."""
     if not os.path.isfile(os.path.join(REF, "run_nerf.py")):
         return None
     for name in ("imageio", "matplotlib", "matplotlib.pyplot", "configargparse"):
@@ -102,7 +102,7 @@ def _cpu_limit():
 
 
 def cpu_rays_per_s(n_rays, reps, warmup, budget_s=45.0, train_step=False):
-    """The reference's forward render of `n_rays` rays on the host cores: the unmodified script when baseline/_ref exists
+    """The reference's forward render of `n_rays` rays on the host cores: the unmodified script when oracle/_ref exists
     (kind "reference"), else the restated op chain (kind "port").  The thread count is calibrated ON THE REAL SAMPLE SIZE
     (more threads than the container owns slows torch's CPU ops down badly); time-bounded; returns the MEDIAN."""
     import tempfile
@@ -166,7 +166,7 @@ def cpu_rays_per_s(n_rays, reps, warmup, budget_s=45.0, train_step=False):
 
 def reference_arm(args, rank):
     """`--impl reference`: the reference's own CPU implementation of the path on the host cores, all the threads it can use,
-    each step the FULL 4096-ray batch when baseline/_ref is present (bounded by time: fewer steps, never a smaller batch)."""
+    each step the FULL 4096-ray batch when oracle/_ref is present (bounded by time: fewer steps, never a smaller batch)."""
     if rank != 0:
         return
     os.environ["CUDA_VISIBLE_DEVICES"] = ""                      # the reference picks cuda when it sees one (run_nerf.py:21)
@@ -180,7 +180,7 @@ def reference_arm(args, rank):
             "config": {"workload": WORKLOAD, "steps_requested": steps, "note": "time-bounded: runs fewer steps than requested rather than a smaller batch"},
             "cpu_baseline": {"value": rps, "unit": "rays/s", "cores": threads, "kind": kind,
                              "sample": f"{N_RAYS} rays x (64+128) samples per step (the full batch), median of {done} step(s), "
-                                       f"{'the unmodified run_nerf.render from baseline/_ref' if kind == 'reference' else 'torch fp32 CPU ops, the op chain of the reference (oracle/torch_ref.py)'}, "
+                                       f"{'the unmodified run_nerf.render from oracle/_ref' if kind == 'reference' else 'torch fp32 CPU ops, the op chain of the reference (oracle/torch_ref.py)'}, "
                                        f"{threads} torch threads (calibrated on this batch; {os.cpu_count()} logical CPUs visible)",
                              "train": None if train_sec is None else {"value": N_RAYS / train_sec, "unit": "rays/s", "ms_per_step": train_sec * 1e3, "steps": 1,
                                                                        "what": "one step of the reference's loop body on the same threads: render(retraw=True), two img2mse, backward, Adam"}},
@@ -197,9 +197,9 @@ def torch_gpu_arm(args):
     import torch
     from oracle import synth
     mod = import_reference()
-    res = {"impl": "torch_gpu", "what": "the unmodified reference (baseline/_ref/run_nerf.py: render(), autograd, torch.optim.Adam) on cuda:0"}
+    res = {"impl": "torch_gpu", "what": "the unmodified reference (oracle/_ref/run_nerf.py: render(), autograd, torch.optim.Adam) on cuda:0"}
     if mod is None or not torch.cuda.is_available():
-        res["unavailable"] = "baseline/_ref or CUDA missing"
+        res["unavailable"] = "oracle/_ref or CUDA missing"
         print(json.dumps(res), flush=True)
         return
     torch.set_default_tensor_type("torch.cuda.FloatTensor")
@@ -318,6 +318,12 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-torch-gpu", action="store_true")
     ap.add_argument("--no-train", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy: the forward step's "
+                         "rgb/disp/acc maps of both passes and z_std (float32) and, unless --no-train, the train step's loss (float64) "
+                         "and a fixed seeded sample of 65536 of its updated parameters (float32).  The forward maps are bit-identical "
+                         "from run to run; the train outputs agree to float-atomic summation order (the backward's bias and weight "
+                         "gradient sums), which Adam amplifies for near-zero gradients")
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
@@ -368,7 +374,7 @@ def main():
               N_samples=N_SAMPLES, N_importance=N_IMPORTANCE, perturb=0., white_bkgd=True, raw_noise_std=0.)
     rays_host = torch.from_numpy(sb["rays"]).pin_memory()
     rays_dev = rays_host.to(dev)
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)            # > 126 MB L2
+    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)            # >> the 50 MB L2
 
     def timed(fn, steps, warmup, use_events=True):
         """-> (median ms per step, max over ranks).  L2 flushed between timed iterations, outside the timed region."""
@@ -410,9 +416,12 @@ def main():
     sampler.start()
 
     # ---------------- forward ----------------
+    last = {}
+
     def step_resident():
         with torch.no_grad():
-            return nb.render(sb["H"], sb["W"], sb["K"], chunk=32768, rays=rays_dev, **kw)
+            last["fwd"] = nb.render(sb["H"], sb["W"], sb["K"], chunk=32768, rays=rays_dev, **kw)
+            return last["fwd"]
 
     def step_eager_e2e():
         with torch.no_grad():
@@ -428,23 +437,24 @@ def main():
     ms_res, ms_res_mean = timed(step_resident, args.steps, args.warmup)
     kms, kn, kfl, _ = read_timing()                 # accumulators hold warm-up + timed launches: per-launch averages are reported
     lib.nerf_b200_timing_enable(0)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        rgb, disp, acc, ex = last["fwd"]
+        outs = {"rgb_map": rgb, "disp_map": disp, "acc_map": acc, "rgb0": ex["rgb0"], "disp0": ex["disp0"], "acc0": ex["acc0"], "z_std": ex["z_std"]}
+        for name, v in outs.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), v.detach().float().cpu().numpy())
     ms_e2e, _ = timed(lambda: graphed(rays_host), args.steps, args.warmup, use_events=False)
     ms_e2e_eager, _ = timed(step_eager_e2e, max(5, args.steps // 3), 3, use_events=False)
     value = N_RAYS * world / (ms_res * 1e-3)
     achieved = (kfl / (kms * 1e-3)) / 1e12 if kms > 0 else 0.0
-    traffic = None
-    tfile = os.path.join(ROOT, "profiles", "march_tc_traffic.json")
-    if os.path.isfile(tfile):
-        with open(tfile) as f:
-            traffic = json.load(f).get("dram_bytes_per_launch")
     fwd = {"value": value, "ms_per_step": ms_res, "ms_per_step_mean": ms_res_mean,
            "e2e": {"value": N_RAYS * world / (ms_e2e * 1e-3), "unit": "rays/s", "h2d_bytes_per_step": int(rays_host.numel() * 4),
                    "d2h_bytes_per_step": int(N_RAYS * 5 * 4), "ms_per_step": ms_e2e,
                    "api": "nerf_pytorch_b200.GraphedRender(...)(rays_host): H2D copy, CUDA-graph replay of render(), D2H copy of rgb/disp/acc, stream sync",
                    "eager_render": {"value": N_RAYS * world / (ms_e2e_eager * 1e-3), "ms_per_step": ms_e2e_eager,
                                     "api": "nerf_pytorch_b200.render(rays=host.to(device)) + .to('cpu'): the drop-in call itself"}},
-           "roofline": {"bound": "tensor", "kernel": "march_tc2_kernel (cta_group::2 pair; coarse + fine launches)", "achieved": achieved, "peak": peak,
-                        "unit": "TFLOP/s", "frac": achieved / peak if peak else None, "traffic": traffic, "peak_source": peak_src,
+           "roofline": {"bound": "tensor", "kernel": "march_wg_kernel (wgmma; coarse + fine launches)", "achieved": achieved, "peak": peak,
+                        "unit": "TFLOP/s", "frac": achieved / peak if peak else None, "peak_source": peak_src,
                         "peak_sustained": peak_sus, "frac_sustained": (achieved / peak_sus) if peak_sus else None,
                         "kernel_ms_per_step": kms / max(1, kn) * 2, "launches_timed": int(kn)},
            "gpu_launches": int(fwd_launches * args.steps)}
@@ -458,6 +468,7 @@ def main():
         tgt_host = torch.rand(N_RAYS, 3, generator=torch.Generator().manual_seed(1)).pin_memory()
 
         def run_train(n_local, group_world):
+            torch.manual_seed(rank)                     # perturb draws (t_rand, u_rand): the same inputs from run to run
             tnets = make_nets()
             k2 = dict(tkw); k2.update(network_fn=tnets[0], network_fine=tnets[1])
             tr = FusedTrainStep(sb["H"], sb["W"], sb["K"], n_local, k2, lrate=5e-4, lrate_decay=250)
@@ -469,6 +480,10 @@ def main():
             torch.cuda.synchronize()
             lib.nerf_b200_timing_enable(0)
             ms_dev, ms_dev_mean = timed(tr.step_device, args.steps, args.warmup)
+            if args.dump_outputs and rank == 0 and not group_world:
+                np.save(os.path.join(args.dump_outputs, "train_loss.npy"), tr.state[:1].double().cpu().numpy())
+                idx = np.random.default_rng(0).choice(tr.flat_p.numel(), size=65536, replace=False)
+                np.save(os.path.join(args.dump_outputs, "train_params_sample.npy"), tr.flat_p.detach()[torch.from_numpy(idx).to(dev)].float().cpu().numpy())
             ms_host, _ = timed(lambda: tr(r_h, t_h), args.steps, args.warmup, use_events=False)
             # kernel split of the step: an eager (un-graphed) pass with the library's event bracketing on
             lib.nerf_b200_timing_enable(1)
@@ -573,7 +588,7 @@ def main():
         "ms_per_step": fwd["ms_per_step"] if headline is not None else train["ms_per_step"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "f16", "data": "synthetic",
         "config": {"workload": WORKLOAD if headline is not None else WORKLOAD_TRAIN, "rays_per_gpu_per_step": N_RAYS,
-                   "operands": "fp16 x fp16 -> fp32 accumulate (tcgen05 kind::f16); backward: loss-scaled fp16 activation gradients",
+                   "operands": "fp16 x fp16 -> fp32 accumulate (wgmma); backward: loss-scaled fp16 activation gradients",
                    "l2": "flushed between timed iterations (512 MiB memset, outside the timed events)",
                    "statistic": "median over the timed steps (mean reported beside it)",
                    "parallelism": f"ray-parallel x{world}, no data-path collective"},

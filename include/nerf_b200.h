@@ -1,5 +1,5 @@
 /*
- * nerf_b200.h -- C ABI of the B200-native NeRF ray-marching hot path.
+ * nerf_b200.h -- C ABI of the H100-native NeRF ray-marching hot path.
  *
  * Drop-in boundary for yenchenlin/nerf-pytorch's  render_rays -> run_network/batchify ->
  * NeRF.forward -> raw2outputs  (+ sample_pdf, Embedder).  The reference has no FFI of its own
@@ -13,7 +13,7 @@
  *   - return value 0 = OK, negative = error; nerf_b200_last_error() gives the message
  *     (thread-local).  The Python host turns a non-zero return into RuntimeError, which is the
  *     reference's only error convention (Python exceptions);
- *   - no CPU fallback exists: every entry point launches sm_100a kernels.
+ *   - no CPU fallback exists: every entry point launches sm_90a kernels.
  */
 #ifndef NERF_B200_H_
 #define NERF_B200_H_
@@ -62,7 +62,7 @@ typedef struct NerfRenderCfg {
   int32_t reserved[3];
 } NerfRenderCfg;
 
-#define NERF_B200_PREC_TC_FP16 0   /* tcgen05 kind::f16, fp16 operands, fp32 accumulate (fast path) */
+#define NERF_B200_PREC_TC_FP16 0   /* wgmma f16, fp16 operands, fp32 accumulate (fast path)        */
 #define NERF_B200_PREC_FP32    1   /* CUDA-core fp32 FMA chain (exact mode, validation)             */
 
 /* Outputs of one network pass over N rays x S samples.  NULL pointers are skipped. */
@@ -151,7 +151,7 @@ int nerf_b200_fine_z(const float* z_vals, const float* weights, const float* u, 
                      int64_t N, int S, int n_imp, float* z_fine, float* z_samples /*[N,n_imp]|NULL*/,
                      float* z_std, void* stream);
 
-/* ---- one fused network pass: pts = o + d*z  -> encode -> MLP (tcgen05) -> raw2outputs ----------
+/* ---- one fused network pass: pts = o + d*z  -> encode -> MLP (wgmma) -> raw2outputs ----------
  *      replaces run_nerf.py:381-386 (coarse) / :397-403 (fine).  rays [N,ray_stride], z_vals [N,S],
  *      noise [N,S]|NULL.  sigma/rgb stay on chip unless out->raw is requested. -------------------- */
 int nerf_b200_march(const float* rays, const float* z_vals, const float* noise, int64_t N, int S,
@@ -220,8 +220,8 @@ typedef struct NerfNetGrads {
   float* views_w;   float* views_b;   float* rgb_w;   float* rgb_b;
   float* output_w;  float* output_b;
 } NerfNetGrads;
-/* tensor-core backward (csrc/bwd_tc2.cuh): compositing adjoint, tcgen05 dgrad chain with loss-scaled fp16
- * activation gradients, layer-major tcgen05 weight gradient; consumes the records of the training-mode pass
+/* tensor-core backward (csrc/bwd_wg.cuh): compositing adjoint, wgmma dgrad chain with loss-scaled fp16
+ * activation gradients, layer-major wgmma weight gradient; consumes the records of the training-mode pass
  * and its raw [N,S,4]. */
 int nerf_b200_march_bwd_tc(const float* rays, const float* z_vals, const float* noise, int64_t N, int S,
                            const NerfNetParams* net, const void* packed, const NerfRenderCfg* cfg,
@@ -234,9 +234,8 @@ size_t nerf_b200_march_bwd_tc_workspace_bytes(int64_t N, int S, const NerfNetPar
 int nerf_b200_march_bwd_tc_layout(int64_t N, int S, const NerfNetParams* net, int64_t* out);
 /* Backward of BOTH passes of one render_rays call -- what loss.backward() triggers for loss = img2mse(rgb) + img2mse(rgb0)
  * (run_nerf.py:765-772; z_samples is detached at :394, so the two passes are independent).  Same kernels as
- * nerf_b200_march_bwd_tc per pass, but scheduled together: the data-gradient chain of one pass (HBM-write-bound) runs on
- * part of the SMs next to the weight gradient of the other pass / previous chunk (HBM-read-bound) on a side stream that forks
- * from and joins `stream` (CUDA-graph capturable).  `fine` may be NULL (N_importance == 0). */
+ * nerf_b200_march_bwd_tc per pass, one pass after the other on `stream` (CUDA-graph capturable).  `fine` may be NULL
+ * (N_importance == 0). */
 typedef struct {
   const float* z_vals;      /* [N,S] */
   const float* noise;       /* [N,S] or NULL */
@@ -270,11 +269,7 @@ int nerf_b200_mse_seed(const float* rgb, const float* target, int64_t N, float g
 int nerf_b200_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, float* state,
                         float lr0, float decay_rate, float decay_steps, float beta1, float beta2, float eps, float grad_mul, void* stream);
 
-/* ---- debug hook (NERF_B200_TRACE builds only; a no-op otherwise): clock64 trace of CTA 0 into a device
- *      buffer of 4096 int64 (NULL disables) ---------------------------------------------------------------- */
-int nerf_b200_debug_set_trace(void* dev_buf_4096_i64);
-
-/* ---- device-time accounting of the dominant kernels (march_tc2 / dgrad_tc2 / wgrad_tc) for bench.py's roofline:
+/* ---- device-time accounting of the dominant kernels (march_wg / dgrad_wg / wgrad_wg) for bench.py's roofline:
  *      when enabled, every launch is bracketed by CUDA events on its own stream; read() synchronises
  *      those events, returns the summed kernel time [ms], the launch count and the algorithmic
  *      FLOPs those launches performed (SURVEY 8d: 2 x MACs of the reference layers x rows), and

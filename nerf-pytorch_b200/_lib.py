@@ -8,9 +8,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# NERF_B200_EXPERIMENTS=1 selects the build with the NERF_B200_DBG_* switches compiled in (libnerf_b200_exp.so: same sources,
-# -DNERF_B200_EXPERIMENTS; tools only)
-LIB_PATH = os.path.join(_HERE, "libnerf_b200_exp.so" if os.environ.get("NERF_B200_EXPERIMENTS") == "1" else "libnerf_b200.so")
+LIB_PATH = os.path.join(_HERE, "libnerf_b200.so")
 MAX_D = 16
 PREC_TC_FP16, PREC_FP32 = 0, 1
 
@@ -123,17 +121,11 @@ SIGNATURES = {
     "nerf_b200_timing_enable": (C.c_int, [C.c_int]),
     "nerf_b200_timing_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int64), C.POINTER(C.c_double)]),
     "nerf_b200_timing_read_kinds": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int64), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
-    "nerf_b200_debug_set_trace": (C.c_int, [c_fp]),
 }
 
 # bring-up self-tests and micro-benchmarks: libnerf_b200_dev.so (include/nerf_b200_dev.h), never used by the product path
 DEV_SIGNATURES = {
     "nerf_b200_dev_last_error": (C.c_char_p, []),
-    "nerf_b200_debug_mma_rate": (C.c_int, [C.c_int, C.c_int, C.c_int, c_fp, c_fp]),
-    "nerf_b200_debug_epi_rate": (C.c_int, [C.c_int, C.c_int, C.c_int, c_fp, c_fp]),
-    "nerf_b200_debug_ldtm_rate": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, c_fp, c_fp]),
-    "nerf_b200_debug_issue_probe": (C.c_int, [C.c_int, C.c_int, C.c_int, c_fp, c_fp]),
-    "nerf_b200_debug_l2_stream": (C.c_int, [c_fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_fp, c_fp]),
     "nerf_b200_debug_dram_stream": (C.c_int, [c_fp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_fp, c_fp]),
     "nerf_b200_debug_hbm_stream": (C.c_int, [c_fp, c_fp, C.c_size_t, C.c_int, C.c_int, c_fp]),
     "nerf_b200_selftest_gemm": (C.c_int, [c_fp, c_fp, C.c_int, C.c_int, c_fp, c_fp, C.c_size_t, c_fp]),

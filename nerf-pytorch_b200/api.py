@@ -3,7 +3,7 @@
 Same names, argument meaning and return structure as yenchenlin/nerf-pytorch, so that these
 functions can be rebound onto the reference's `run_nerf` module (see dropin.py) and `train()`
 runs unchanged -- but every tensor-op chain of the hot path is one call into the hand-written
-sm_100a library behind include/nerf_b200.h.  PyTorch is used for memory, streams and autograd
+sm_90a library behind include/nerf_b200.h.  PyTorch is used for memory, streams and autograd
 plumbing only.  There is no CPU fallback: tensors must live on a CUDA device.
 
 Reference sites: render run_nerf.py:69-134, batchify_rays :54-66, render_rays :308-418,
@@ -40,7 +40,7 @@ to8b = lambda x: (255 * np.clip(x, 0, 1)).astype(np.uint8)                      
 
 
 def set_precision(mode: str):
-    """'tc_fp16' (tcgen05 fp16 operands / fp32 accumulate, default) or 'fp32' (CUDA-core exact mode)."""
+    """'tc_fp16' (wgmma fp16 operands / fp32 accumulate, default) or 'fp32' (CUDA-core exact mode)."""
     _PRECISION["mode"] = {"tc_fp16": PREC_TC_FP16, "fp32": PREC_FP32}[mode]
 
 
@@ -49,7 +49,7 @@ def get_precision() -> str:
 
 
 def set_backward(mode: str):
-    """'tc' (default in tc_fp16 precision: tcgen05 backward from the forward's saved tile records) or 'exact'
+    """'tc' (default in tc_fp16 precision: wgmma backward from the forward's saved tile records) or 'exact'
     (fp32 CUDA-core recompute backward; always used in fp32 precision and for networks without view directions)."""
     if mode not in ("tc", "exact"):
         raise ValueError(mode)
@@ -496,7 +496,7 @@ def _flush_deferred_pack():
 class _RenderRays(torch.autograd.Function):
     """Forward: nerf_b200_render_rays_fwd (coarse z -> fused pass -> resample -> fused pass); when a parameter needs a
     gradient and the tensor-core backward is selected, the training-mode variant that also leaves the per-tile
-    activation records.  Backward: per pass nerf_b200_march_bwd_tc (tcgen05 dgrad chain + layer-major wgrad from
+    activation records.  Backward: per pass nerf_b200_march_bwd_tc (wgmma dgrad chain + layer-major wgrad from
     those records) or, in exact mode, nerf_b200_march_bwd (fp32 recompute + GEMM backprop).  Gradients w.r.t. rgb_map
     and rgb0 only -- exactly the terms of the reference's loss (run_nerf.py:765-772); z_samples is detached in the
     reference (:394) so nothing flows through the resampling."""

@@ -5,7 +5,7 @@
 // (SURVEY App. E) gives dL/draw, and the MLP is walked backwards with two generic fp32 GEMMs
 // (dgrad: C = A B, wgrad: C += A^T B reduced over all sample rows), a ReLU-mask and a column-sum
 // kernel.  No gradient flows to rays / z (run_nerf.py:394, SURVEY 3.5).
-// This is the first correct backward (round 1); the tcgen05 dgrad/wgrad kernels replace it in round 2.
+// The tensor-core path (bwd_wg.cuh) is the default; this one serves exact mode and networks without view directions.
 #pragma once
 #include "common.cuh"
 

@@ -5,8 +5,8 @@
 #include "bwd_simt.cuh"
 #include "mlp_simt.cuh"
 #include "fused_tc.cuh"
-#include "fused_tc2.cuh"
-#include "bwd_tc2.cuh"
+#include "fused_wg.cuh"
+#include "bwd_wg.cuh"
 #include "train_step.cuh"
 #include <stdlib.h>
 
@@ -21,7 +21,7 @@ int set_error(int code, const char* fmt, ...) {
   return code;
 }
 
-// ---- optional device-time accounting of march_tc_kernel launches (bench.py roofline) ----
+// ---- optional device-time accounting of the tensor-core kernel launches (bench.py roofline) ----
 struct TimedLaunch { cudaEvent_t a, b; double flops; int kind; };   // kind 0: forward pass, 1: dgrad chain, 2: wgrad
 static bool g_timing = false;
 static TimedLaunch g_timed[4096];
@@ -35,8 +35,6 @@ static double net_macs_per_row(const NerfNetParams& n) {
   else m += (double)n.W * n.output_ch;
   return m;
 }
-
-static long long* g_trace = nullptr;      // debug: device buffer of 4096 int64 clock stamps (NERF_B200_TRACE builds)
 
 static int check_tc_net(const NerfNetParams* net) {
   NB_CHECK_ARG(net != nullptr, "net is NULL");
@@ -55,9 +53,7 @@ static int smem_optin(const void* fn, size_t bytes) {
 
 // per-device facts (SM count; which kernels already have their > 48 KB shared-memory opt-in): the library may be used
 // on several devices of one process, and cudaFuncSetAttribute is per device
-static const char* exp_env(const char* name) { return kExp ? getenv(name) : nullptr; }      // experiment switches: product build ignores them
-static int dbg_emit() { static int v = -1; if (v < 0) { const char* e = exp_env("NERF_B200_DBG_EMIT"); v = e ? atoi(e) : 0; } return v; }
-struct DeviceState { int sms; bool optin_fwd, optin_bwd; cudaStream_t side; cudaEvent_t ev[10]; };
+struct DeviceState { int sms; bool optin_fwd, optin_bwd; };
 static DeviceState* device_state() {
   static DeviceState st[64];
   static bool init[64] = {false};
@@ -67,17 +63,8 @@ static DeviceState* device_state() {
   if (!init[dev]) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    st[dev].sms = n > 0 ? n : 148;
+    st[dev].sms = n > 0 ? n : 132;
     st[dev].optin_fwd = st[dev].optin_bwd = false;
-    // side stream + events of the two-pass backward: created with the device state (the first library call on a device), not
-    // lazily inside a call that may be running under stream capture
-    st[dev].side = nullptr;
-    if (cudaStreamCreateWithFlags(&st[dev].side, cudaStreamNonBlocking) == cudaSuccess) {
-      for (int i = 0; i < 10; ++i)
-        if (cudaEventCreateWithFlags(&st[dev].ev[i], cudaEventDisableTiming) != cudaSuccess) { cudaStreamDestroy(st[dev].side); st[dev].side = nullptr; break; }
-    } else {
-      st[dev].side = nullptr;
-    }
     cudaGetLastError();
     init[dev] = true;
   }
@@ -85,31 +72,7 @@ static DeviceState* device_state() {
 }
 static int num_sms() { return device_state()->sms; }
 
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-// 2-D tensor map over a byte buffer viewed as [rows][256] uint16 (512-byte rows); box = `box_rows` rows (box_rows * 512 bytes)
-static int make_row_map(CUtensorMap* map, const void* base, size_t bytes, int box_rows) {
-  static EncodeFn encode = nullptr;
-  if (!encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    NB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-    NB_CHECK_ARG(fn != nullptr && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available");
-    encode = reinterpret_cast<EncodeFn>(fn);
-  }
-  NB_CHECK_ARG(bytes % 512 == 0 && (reinterpret_cast<uintptr_t>(base) & 15) == 0, "tensor map: buffer must be 16-byte aligned, a multiple of 512 bytes");
-  const cuuint64_t gdim[2] = {256, (cuuint64_t)(bytes / 512)};
-  const cuuint64_t gstr[1] = {512};
-  const cuuint32_t box[2] = {256, (cuuint32_t)box_rows}, estr[2] = {1, 1};
-  CUresult cr = encode(map, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(base), gdim, gstr, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  NB_CHECK_ARG(cr == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
-  return 0;
-}
-
-// shared launcher of the fused tcgen05 pass; `save` != NULL selects the training-mode kernel (EMIT)
+// shared launcher of the fused tensor-core pass; `save` != NULL selects the training-mode kernel (EMIT)
 static int launch_march(const float* rays, int ray_stride, const float* z_vals, const float* pts,
                         const float* dirs, int dir_stride, const float* noise, long long N, int S,
                         const NerfNetParams* net, const void* packed, int L, int Lv, int white_bkgd, int do_composite,
@@ -128,7 +91,6 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
   p.N = N; p.S = S;
   p.bias = reinterpret_cast<const float*>(pk + PL.off_bias);
   p.heads = reinterpret_cast<const float*>(pk + PL.off_heads);
-  p.biasb = pk + PL.off_biasb;
   p.D = net->D; p.skip = net->skip; p.use_viewdirs = net->use_viewdirs; p.L = L; p.IC = net->input_ch;
   p.white_bkgd = white_bkgd; p.do_composite = do_composite;
   if (out) p.out = *out;
@@ -144,17 +106,16 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
     NB_LAUNCH_OK("view_bias_kernel");
     p.vb = vb;
   }
-  // persistent grid: whole rays per CTA, balanced over the SMs, whole CTA pairs (a padding CTA owns no rays)
+  // persistent grid: whole rays per CTA, balanced over the SMs (the tile plan)
   DeviceState* ds = device_state();
   const TilePlan plan = make_tile_plan(N, S, ds->sms);
   p.rays_per_cta = plan.rays_per_cta;
   NB_CHECK_ARG((long long)p.rays_per_cta * S < (1ll << 30), "rays_per_cta * S overflows");
   if (!ds->optin_fwd) {
-    if (int rc = smem_optin((const void*)march_tc2_kernel<false>, SM_ALLOC)) return rc;
-    if (int rc = smem_optin((const void*)march_tc2_kernel<true>, SM_ALLOC)) return rc;
+    if (int rc = smem_optin((const void*)march_wg_kernel<false>, SM_ALLOC)) return rc;
+    if (int rc = smem_optin((const void*)march_wg_kernel<true>, SM_ALLOC)) return rc;
     ds->optin_fwd = true;
   }
-  p.trace = g_trace;
   TrainSaveDev sv;
   memset(&sv, 0, sizeof(sv));
   if (save) {
@@ -165,7 +126,6 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
     NB_CHECK_ARG((reinterpret_cast<uintptr_t>(save->act) & 15) == 0 && (reinterpret_cast<uintptr_t>(save->mask) & 15) == 0, "save buffers must be 16-byte aligned");
     sv.act = static_cast<uint8_t*>(save->act); sv.mask = static_cast<uint8_t*>(save->mask);
     sv.nst_plan = plan.nst; sv.rec_act = rec_act_bytes(net->D); sv.rec_mask = rec_mask_bytes(net->D);
-    sv.dbg = dbg_emit();
   }
   TimedLaunch* tl = nullptr;
   if (g_timing && g_ntimed < 4096) {
@@ -175,16 +135,11 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
     tl->kind = 0;
     cudaEventRecord(tl->a, st);
   }
-  // tensor map over the rank-split chunk stream (512-byte rows); box = 16 rows = 8 KB = one ring stage
-  CUtensorMap wmap;
-  const uint8_t* pair_stream = pk + PL.off_pair;
-  p.chunks = pair_stream;
-  p.pair_half_bytes = PL.chunk_bytes / 2;
-  if (int rc = make_row_map(&wmap, pair_stream, PL.chunk_bytes, 16)) return rc;
-  if (save) march_tc2_kernel<true><<<plan.grid, TC_THREADS, SM_ALLOC, st>>>(p, wmap, sv);
-  else march_tc2_kernel<false><<<plan.grid, TC_THREADS, SM_ALLOC, st>>>(p, wmap, sv);
+  p.chunks = pk + PL.off_chunks;
+  if (save) march_wg_kernel<true><<<plan.grid, TC_THREADS, SM_ALLOC, st>>>(p, sv);
+  else march_wg_kernel<false><<<plan.grid, TC_THREADS, SM_ALLOC, st>>>(p, sv);
   if (tl) cudaEventRecord(tl->b, st);
-  NB_LAUNCH_OK("march_tc2_kernel");
+  NB_LAUNCH_OK("march_wg_kernel");
   return 0;
 }
 
@@ -250,10 +205,7 @@ int nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t packed
     c.src = src; c.sn = ld; c.sk = 1; c.k0 = k0; c.kvalid = kvalid < 0 ? 0 : (kvalid > 32 ? 32 : kvalid); c.nrows = nrows; c.dst_off = off;
     off += (unsigned)nrows * 64;
   };
-  PackBiasJob bj;
-  bj.n = 0;
   for (int l = 0; l < PL.NL; ++l) {
-    if (tc_layer_has_bias(l, net->D)) bj.src[bj.n++] = (l < net->D) ? net->pts_b[l] : net->feature_b;
     if (l == 0) { add(net->pts_w[0], IC, 0, IC, 256); add(net->pts_w[0], IC, 32, IC - 32, 256); }
     else if (l < net->D) {
       const bool sk = (net->skip >= 0 && l == net->skip + 1);
@@ -264,27 +216,11 @@ int nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t packed
     else { for (int c = 0; c < 8; ++c) add(net->views_w, W + net->input_ch_views, 32 * c, 32, 128); }
   }
   NB_CHECK_ARG(job.n == PL.n_chunks && off == PL.off_chunks + PL.chunk_bytes, "internal: chunk table mismatch");
-  bj.dst_off = (unsigned)PL.off_biasb;
-  pack_bias_kernel<<<1, 256, 0, st>>>(bj, static_cast<uint8_t*>(packed));
-  NB_LAUNCH_OK("pack_bias_kernel");
   dim3 grid(4, job.n);
   pack_chunks_kernel<<<grid, 256, 0, st>>>(job, static_cast<uint8_t*>(packed));
   NB_LAUNCH_OK("pack_chunks_kernel");
-  {
-    // rank-split copy for the CTA-pair kernel: [rank 0: every chunk's rows 0..N/2-1][rank 1: rows N/2..N-1], so that
-    // two consecutive chunk halves of one CTA are contiguous (one 16 KB TMA box)
-    uint8_t* base = static_cast<uint8_t*>(packed);
-    const size_t views_bytes = net->use_viewdirs ? (size_t)8 * (TC_STAGE_BYTES / 2) : 0;
-    const size_t reg_bytes = PL.chunk_bytes - views_bytes;
-    for (int r = 0; r < 2; ++r) {
-      uint8_t* dst = base + PL.off_pair + (size_t)r * (PL.chunk_bytes / 2);
-      NB_CUDA(cudaMemcpy2DAsync(dst, 8192, base + PL.off_chunks + (size_t)r * 8192, 16384, 8192, reg_bytes / 16384, cudaMemcpyDeviceToDevice, st));
-      if (views_bytes)
-        NB_CUDA(cudaMemcpy2DAsync(dst + reg_bytes / 2, 4096, base + PL.off_chunks + reg_bytes + (size_t)r * 4096, 8192, 4096, 8, cudaMemcpyDeviceToDevice, st));
-    }
-  }
   if (PL.bwd_bytes) {
-    // backward (dgrad) stream, bwd_tc2.cuh: chunk [n][k] = W[k0 + k][col0 + n] -- the transposed weights, so that the
+    // backward (dgrad) stream, bwd_wg.cuh: chunk [n][k] = W[k0 + k][col0 + n] -- the transposed weights, so that the
     // chain dA_{l-1} = dA_l W_l runs through the forward's operand layouts.  Step 0: views_linears[0].weight[:, :W]
     // (K = W/2), step 1: feature_linear, then pts_linears[D-1] ... [1] restricted to their h columns.
     PackJob bj2;
@@ -305,10 +241,6 @@ int nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t packed
     dim3 g2(4, bj2.n);
     pack_chunks_kernel<<<g2, 256, 0, st>>>(bj2, static_cast<uint8_t*>(packed));
     NB_LAUNCH_OK("pack_chunks_kernel (backward stream)");
-    uint8_t* base = static_cast<uint8_t*>(packed);
-    for (int r = 0; r < 2; ++r)
-      NB_CUDA(cudaMemcpy2DAsync(base + PL.off_bwd_pair + (size_t)r * (PL.bwd_bytes / 2), 8192, base + PL.off_bwd + (size_t)r * 8192, 16384, 8192,
-                                PL.bwd_bytes / 16384, cudaMemcpyDeviceToDevice, st));
   }
   PackTables t;
   t.net = *net; t.off_bias = PL.off_bias; t.off_heads = PL.off_heads; t.off_vdir = PL.off_vdir;
@@ -733,25 +665,29 @@ int nerf_b200_march_bwd(const float* rays, const float* z_vals, const float* noi
   return 0;
 }
 
-// ---- tensor-core backward of one pass (bwd_tc2.cuh) ------------------------------------------------
+// ---- tensor-core backward of one pass (bwd_wg.cuh) ------------------------------------------------
 namespace {
 struct BwdTcLayout { size_t off_amax, off_draw, off_encv, off_dsum, off_gv, off_partial, off_grad, total; long long part_floats; };
-struct BwdTcJobs { int n; WgradJob w[WG2_MAX_JOBS]; ReduceJob r[WG2_MAX_JOBS]; int total_ctas; long long part_floats; };
+struct BwdTcJobs { int n; bool overflow; WgradJob w[WG2_MAX_JOBS]; ReduceJob r[WG2_MAX_JOBS]; int total_ctas; long long part_floats; };
 
-// jobs of the weight gradient and their CTA ranges (proportional to the bytes each job streams per tile)
+// jobs of the weight gradient (128-row blocks of dW) and their CTA ranges (proportional to the bytes each job streams per tile).
+// Every job gets at least one CTA: the caller rejects `sms` < J.n (and J.overflow: more jobs than WG2_MAX_JOBS).
 BwdTcJobs make_bwd_jobs(const NerfNetParams& n, const NerfNetGrads* g, int sms) {
   BwdTcJobs J;
   memset(&J, 0, sizeof(J));
   const int D = n.D, W = n.W, IC = n.input_ch;
   auto add = [&](uint32_t a_off, int Mc, uint32_t b_off, int Nc, float* dst, int ldw, int n_valid, float* db) {
-    WgradJob& w = J.w[J.n];
-    ReduceJob& r = J.r[J.n];
-    w.a_off = a_off; w.b_off = b_off; w.Mc = Mc; w.Nc = Nc; w.db = db; w.aux = 0; w.aux_dst = nullptr; w.aux_b = nullptr;
-    r.Mc = Mc; r.Nc = Nc; r.n_valid = n_valid; r.ldw = ldw; r.dst = dst;
-    ++J.n;
+    for (int m0 = 0; m0 < Mc; m0 += 128) {
+      if (J.n == WG2_MAX_JOBS) { J.overflow = true; return; }
+      WgradJob& w = J.w[J.n];
+      ReduceJob& r = J.r[J.n];
+      w.a_off = a_off; w.a_cols = Mc; w.m0 = m0; w.b_off = b_off; w.Nc = Nc; w.db = db; w.aux = 0; w.aux_dst = nullptr; w.aux_b = nullptr;
+      r.Mc = 128; r.Nc = Nc; r.n_valid = n_valid; r.ldw = ldw; r.dst = dst ? dst + (size_t)m0 * ldw : nullptr;
+      ++J.n;
+    }
   };
   // job 0: G = d_hv^T h_{D-1} (-> views_linears[0].weight[:, :W] through views_feat_wgrad_kernel; its reduce target is a scratch
-  // block set by the caller);  job 1: feature_linear = d_feat^T h_{D-1}
+  // block set by the caller);  jobs 1, 2: feature_linear = d_feat^T h_{D-1} (job 1 also forms alpha_linear's gradient)
   add(0, 128, rec_act_h(D - 1), 256, nullptr, 256, 256, g ? g->views_b : nullptr);
   add(rec_grad_step(0), 256, rec_act_h(D - 1), 256, g ? g->feature_w : nullptr, W, W, g ? g->feature_b : nullptr);
   for (int l = D - 1; l >= 1; --l) {
@@ -760,16 +696,9 @@ BwdTcJobs make_bwd_jobs(const NerfNetParams& n, const NerfNetGrads* g, int sms) 
     if (sk) add(rec_grad_dA(l, D), 256, 0, 64, g ? g->pts_w[l] : nullptr, W + IC, IC, nullptr);        // the [input_pts] columns
   }
   add(rec_grad_dA(0, D), 256, 0, 64, g ? g->pts_w[0] : nullptr, IC, IC, g ? g->pts_b[0] : nullptr);
-  // CTAs per job ~ its measured cost (profiles/r02_backward_experiments.txt: per-job finish times of a byte-proportional split):
-  // bytes streamed per tile (Mc + Nc columns), x 1.27 for the feature job (its spare warps also sweep B for alpha_linear),
-  // x 1.06 for the views job (per-ray atomics), x 1.16 for a 64-wide B with a bias gradient (short stages, same column sums)
-  auto cost = [&](int i) {
-    double c = (double)(J.w[i].Mc + J.w[i].Nc);
-    if (i == 0) c *= 1.06;
-    if (i == 1) c *= 1.27;
-    if (J.w[i].Nc == 64 && J.w[i].db) c *= 1.16;
-    return c;
-  };
+  // CTAs per job ~ the bytes it streams per tile (128 + Nc columns)
+  auto cost = [&](int i) { return (double)(128 + J.w[i].Nc); };
+  if (J.overflow || J.n > sms) return J;
   double tot = 0;
   for (int i = 0; i < J.n; ++i) tot += cost(i);
   int used = 0;
@@ -787,7 +716,7 @@ BwdTcJobs make_bwd_jobs(const NerfNetParams& n, const NerfNetGrads* g, int sms) 
     for (int i = 1; i < J.n; ++i) if (frac[i] > frac[b]) b = i;
     ++J.w[b].ncta; ++used; frac[b] -= 1.0;
   }
-  while (used > sms) {                               // (tiny launches: more jobs than CTAs is rejected by the caller's minimum)
+  while (used > sms) {                               // (rounding up to one CTA per job overshot: take from the largest)
     int b = 0;
     for (int i = 1; i < J.n; ++i) if (J.w[i].ncta > J.w[b].ncta) b = i;
     --J.w[b].ncta; --used;
@@ -797,7 +726,7 @@ BwdTcJobs make_bwd_jobs(const NerfNetParams& n, const NerfNetGrads* g, int sms) 
   for (int i = 0; i < J.n; ++i) {
     J.w[i].cta0 = cta; cta += J.w[i].ncta;
     J.w[i].part_off = pf; J.r[i].part_off = pf; J.r[i].ncta = J.w[i].ncta;
-    pf += (long long)J.w[i].ncta * J.w[i].Mc * J.w[i].Nc;
+    pf += (long long)J.w[i].ncta * 128 * J.w[i].Nc;
   }
   J.total_ctas = cta; J.part_floats = pf;
   return J;
@@ -846,9 +775,8 @@ int nerf_b200_march_bwd_tc_layout(int64_t N, int S, const NerfNetParams* net, in
 }
 
 namespace {
-// One pass of the tensor-core backward, split into its phases so that the two passes of render_rays can interleave: the data-
-// gradient chain is bound by HBM WRITES (3.9 TB/s ceiling), the weight gradient by HBM READS; side by side on disjoint SMs they
-// share a bus that carries 6.6 TB/s of mixed traffic (profiles/r02_hbm_probe.json).
+// One pass of the tensor-core backward, in its phases: prologue (loss scale, compositing adjoint, seed tiles), dgrad chain,
+// weight gradients, view-column gradients.
 struct BwdTcPass {
   const float* rays; const float* z; const float* noise; int64_t N; int S; const NerfNetParams* net; const void* packed;
   const NerfRenderCfg* cfg; const float* raw; const NerfTrainSave* save; const float* g_rgb; const NerfNetGrads* grads;
@@ -875,8 +803,8 @@ struct BwdTcPass {
     act = static_cast<const uint8_t*>(save->act);
     mask = static_cast<const uint8_t*>(save->mask);
     if (!ds->optin_bwd) {
-      NB_TRY(smem_optin((const void*)dgrad_tc2_kernel, SM_ALLOC));
-      NB_TRY(smem_optin((const void*)wgrad_tc_kernel, WG2_TOTAL));
+      NB_TRY(smem_optin((const void*)dgrad_wg_kernel, SM_ALLOC));
+      NB_TRY(smem_optin((const void*)wgrad_wg_kernel, WG2_TOTAL));
       ds->optin_bwd = true;
     }
     return 0;
@@ -901,23 +829,18 @@ struct BwdTcPass {
     return 0;
   }
 
-  // 3. dgrad chain of the forward's CTAs [vc0, vc1) on at most `ctas` CTAs (CTA pairs, the forward's tile order)
-  int dgrad(cudaStream_t st, int ctas, int vc0, int vc1) {
+  // 3. dgrad chain, one CTA per forward CTA (the forward's tile order)
+  int dgrad(cudaStream_t st) {
+    const int vc0 = 0, vc1 = plan.grid;
     const int D = net->D;
     const uint8_t* pk = static_cast<const uint8_t*>(packed);
     DgradParams dp;
     dp.mask = mask; dp.grad = grec; dp.d_raw = d_raw; dp.amax = amax; dp.alpha_w = net->alpha_w;
+    dp.chunks = pk + PL.off_bwd;
     dp.N = N; dp.S = S; dp.rays_per_cta = plan.rays_per_cta; dp.nst_plan = plan.nst; dp.D = D;
     dp.rec_mask = rec_mask_bytes(D); dp.rec_grad = rec_grad_bytes(D);
-    dp.pair_half_bytes = PL.bwd_bytes / 2;
-    dp.vc0 = vc0; dp.vc1 = vc1; dp.dbg = dbg_emit();
-    int grid = vc1 - vc0;
-    if (grid > ctas) grid = ctas;
-    grid &= ~1;
-    if (grid < 2) grid = 2;
-    CUtensorMap wmap, gmap;
-    NB_TRY(make_row_map(&wmap, pk + PL.off_bwd_pair, PL.bwd_bytes, 16));
-    NB_TRY(make_row_map(&gmap, grec, (size_t)plan.n_tiles * rec_grad_bytes(D), 16));      // 8 KB boxes: the pieces of the d_hv image
+    dp.vc0 = vc0; dp.vc1 = vc1;
+    const int grid = plan.grid;
     TimedLaunch* tl = nullptr;
     if (g_timing && g_ntimed < 4096) {
       tl = &g_timed[g_ntimed++];
@@ -926,46 +849,27 @@ struct BwdTcPass {
       tl->kind = 1;
       cudaEventRecord(tl->a, st);
     }
-    static const char* prof_path = exp_env("NERF_B200_DBG_DGRAD_PROF");     // experiments: where the epilogue warps wait
-    static unsigned long long* prof_dev = nullptr;
-    dp.prof = nullptr;
-    if (prof_path) { if (!prof_dev) NB_CUDA(cudaMalloc(&prof_dev, 512 * 16 * 3 * 8)); dp.prof = prof_dev; }
-    dgrad_tc2_kernel<<<grid, TC_THREADS, SM_ALLOC, st>>>(dp, wmap, gmap);
+    dgrad_wg_kernel<<<grid, TC_THREADS, SM_ALLOC, st>>>(dp);
     if (tl) cudaEventRecord(tl->b, st);
-    NB_LAUNCH_OK("dgrad_tc2_kernel");
-    if (prof_path) {
-      static unsigned long long h[512 * 16 * 3];
-      NB_CUDA(cudaStreamSynchronize(st));
-      NB_CUDA(cudaMemcpy(h, prof_dev, (size_t)grid * 16 * 3 * 8, cudaMemcpyDeviceToHost));
-      if (FILE* f = fopen(prof_path, "a")) {
-        double tot = 0, df = 0, gt = 0;
-        for (int i = 0; i < grid * 16; ++i) { tot += (double)h[3 * i]; df += (double)h[3 * i + 1]; gt += (double)h[3 * i + 2]; }
-        fprintf(f, "dgrad S=%d grid=%d: epilogue warps, mean cycles: total %.0f, waiting for d_full %.0f (%.1f %%), at the copy gates %.0f (%.1f %%)\n", S, grid,
-                tot / (grid * 16), df / (grid * 16), 100.0 * df / tot, gt / (grid * 16), 100.0 * gt / tot);
-        fclose(f);
-      }
-    }
+    NB_LAUNCH_OK("dgrad_wg_kernel");
     return 0;
   }
 
-  // 4. weight gradients (layer-major) + bias gradients of the forward's CTAs [vc0, vc1) on `ctas` CTAs, then the reduction of
-  // the per-CTA partial blocks (adds into the gradient tensors, so a pass may be covered by several launches)
-  int wgrad(cudaStream_t st, int ctas, int vc0, int vc1) {
+  // 4. weight gradients (layer-major) + bias gradients on all SMs, then the reduction of the per-CTA partial blocks (adds into
+  // the gradient tensors)
+  int wgrad(cudaStream_t st) {
+    const int ctas = ds->sms, vc0 = 0, vc1 = plan.grid;
     const int D = net->D;
-    BwdTcJobs J = make_bwd_jobs(*net, grads, ctas & ~1);           // whole CTA pairs: the kernel launches as 2-CTA clusters
+    BwdTcJobs J = make_bwd_jobs(*net, grads, ctas);
+    NB_CHECK_ARG(!J.overflow && J.n <= ctas, "weight gradient: %d jobs need at least as many CTAs (have %d; at most %d jobs)", J.n, ctas, WG2_MAX_JOBS);
     J.w[0].aux = 1; J.w[0].aux_dst = dsum;            // views job: per-ray row sums of d_hv
-    J.w[1].aux = 2; J.w[1].aux_dst = grads->alpha_w; J.w[1].aux_b = grads->alpha_b;   // feature job: alpha_linear gradients
-    { static int noaux = -1; if (noaux < 0) { const char* e = exp_env("NERF_B200_DBG_NOAUX"); noaux = e ? atoi(e) : 0; }
-      if (noaux & 1) J.w[0].aux = 0;
-      if (noaux & 2) J.w[1].aux = 0;
-      if (noaux & 4) for (int i = 0; i < J.n; ++i) J.w[i].db = nullptr; }
+    J.w[1].aux = 2; J.w[1].aux_dst = grads->alpha_w; J.w[1].aux_b = grads->alpha_b;   // feature job, first block: alpha_linear gradients
     WgradParams wp;
     memset(&wp, 0, sizeof(wp));
     wp.act = act; wp.grad = grec; wp.rec_act = rec_act_bytes(D); wp.rec_grad = rec_grad_bytes(D);
     wp.N = N; wp.S = S; wp.rays_per_cta = plan.rays_per_cta; wp.nst_plan = plan.nst; wp.n_tiles = plan.n_tiles;
     wp.t0 = (long long)vc0 * plan.nst * 2; wp.t1 = (long long)vc1 * plan.nst * 2;
     wp.amax = amax; wp.partial = partial; wp.d_raw = d_raw; wp.njobs = J.n;
-    { static int wd = -1; if (wd < 0) { const char* e = exp_env("NERF_B200_DBG_WGRAD"); wd = e ? atoi(e) : 0; } wp.dbg = wd; }
     for (int i = 0; i < J.n; ++i) wp.jobs[i] = J.w[i];
     TimedLaunch* tl = nullptr;
     if (g_timing && g_ntimed < 4096) {
@@ -975,34 +879,15 @@ struct BwdTcPass {
       tl->kind = 2;
       cudaEventRecord(tl->a, st);
     }
-    static const char* prof_path = exp_env("NERF_B200_DBG_WGRAD_PROF");     // experiments: per-CTA start / end times appended to a file
-    static unsigned long long* prof_dev = nullptr;
-    if (prof_path) { if (!prof_dev) NB_CUDA(cudaMalloc(&prof_dev, 1024 * 16)); wp.prof = prof_dev; }
-    wgrad_tc_kernel<<<J.total_ctas, WG2_THREADS, WG2_TOTAL, st>>>(wp);
+    wgrad_wg_kernel<<<J.total_ctas, WG2_THREADS, WG2_TOTAL, st>>>(wp);
     if (tl) cudaEventRecord(tl->b, st);
-    NB_LAUNCH_OK("wgrad_tc_kernel");
-    if (prof_path) {
-      unsigned long long h[2048];
-      NB_CUDA(cudaStreamSynchronize(st));
-      NB_CUDA(cudaMemcpy(h, prof_dev, (size_t)J.total_ctas * 16, cudaMemcpyDeviceToHost));
-      if (FILE* f = fopen(prof_path, "a")) {
-        unsigned long long t0 = ~0ull;
-        for (int i = 0; i < J.total_ctas; ++i) if (h[2 * i] < t0) t0 = h[2 * i];
-        fprintf(f, "launch S=%d ctas=%d\n", S, J.total_ctas);
-        for (int j = 0; j < J.n; ++j) {
-          unsigned long long lo = ~0ull, hi = 0;
-          for (int i = J.w[j].cta0; i < J.w[j].cta0 + J.w[j].ncta; ++i) { if (h[2 * i + 1] - t0 < lo) lo = h[2 * i + 1] - t0; if (h[2 * i + 1] - t0 > hi) hi = h[2 * i + 1] - t0; }
-          fprintf(f, "  job %2d Mc=%3d Nc=%3d aux=%d db=%d ctas=%2d end_us min %.1f max %.1f\n", j, J.w[j].Mc, J.w[j].Nc, J.w[j].aux, J.w[j].db != nullptr, J.w[j].ncta, lo * 1e-3, hi * 1e-3);
-        }
-        fclose(f);
-      }
-    }
+    NB_LAUNCH_OK("wgrad_wg_kernel");
     ReduceParams rp;
     memset(&rp, 0, sizeof(rp));
     rp.partial = partial; rp.amax = amax; rp.njobs = J.n;
     J.r[0].dst = gv;                                  // job 0 reduces into the scratch block G
     for (int i = 0; i < J.n; ++i) rp.jobs[i] = J.r[i];
-    dim3 rg(256, J.n);
+    dim3 rg(128, J.n);
     wgrad_reduce_kernel<<<rg, 256, 0, st>>>(rp);
     NB_LAUNCH_OK("wgrad_reduce_kernel");
     return 0;
@@ -1050,8 +935,8 @@ int nerf_b200_march_bwd_tc(const float* rays, const float* z_vals, const float* 
   BwdTcPass b = bind_pass(rays, N, cfg, &q);
   NB_TRY(b.init(workspace, workspace_bytes));
   NB_TRY(b.prologue(st));
-  NB_TRY(b.dgrad(st, b.plan.grid, 0, b.plan.grid));
-  NB_TRY(b.wgrad(st, b.ds->sms, 0, b.plan.grid));
+  NB_TRY(b.dgrad(st));
+  NB_TRY(b.wgrad(st));
   NB_TRY(b.heads(st));
   return 0;
 }
@@ -1067,13 +952,8 @@ size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, con
 }
 
 // Backward of both passes of render_rays (run_nerf.py:765-772: loss = img2mse(rgb) + img2mse(rgb0); z_samples is detached, :394,
-// so the passes are independent).  Two streams (graph-capturable: the side stream forks from and joins `stream`).  Default schedule:
-//   main: prologue(c) dgrad(c) | wgrad(c)      | dgrad(f) | wgrad(f) heads(f) |
-//   side:                      | prologue(f)   |          | heads(c)          | join
-// the small memory-bound kernels of one pass (compositing adjoint, seed tiles + rgb_linear, view-column gradients) run on the SM
-// resources the weight-gradient kernel leaves free (it holds one 192-thread CTA per SM) instead of between the big kernels.
-// NERF_B200_BWD_OVERLAP = "0": one stream, one pass after the other;  "w[,chunks]" (w >= 16): split the SMs -- the fine pass's chain
-// on sms - w of them next to a weight gradient on w (measured slower in every split: profiles/r02_bwd_overlap_sweep.jsonl).
+// so the passes are independent): one pass after the other on `stream`.  The weight-gradient kernel holds a whole SM (384 threads
+// x 168 registers), so nothing of the other pass could run beside it.
 int nerf_b200_render_rays_bwd_tc(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse, const NerfBwdPass* fine,
                                  void* workspace, size_t workspace_bytes, void* stream) {
   if (int rc = check_bwd_pass(rays, coarse, cfg)) return rc;
@@ -1084,86 +964,11 @@ int nerf_b200_render_rays_bwd_tc(const float* rays, int64_t N, const NerfRenderC
   const size_t cb = bwd_pass_bytes(N, coarse->S, coarse->net);
   NB_CHECK_ARG(workspace && workspace_bytes >= cb, "render_rays_bwd_tc workspace too small");
   NB_TRY(c.init(workspace, cb));
-  DeviceState* ds = c.ds;
-  const int sms = ds->sms;
-  static int env_w = -2, env_chunks = 1;                // -1: default schedule
-  if (env_w == -2) {
-    const char* e = getenv("NERF_B200_BWD_OVERLAP");
-    env_w = -1;
-    if (e) { int a = -1, k = 1; const int n = sscanf(e, "%d,%d", &a, &k); if (n >= 1) env_w = a; if (n >= 2 && k > 0) env_chunks = k; }
-  }
-  if (!fine) {
-    NB_TRY(c.prologue(st)); NB_TRY(c.dgrad(st, c.plan.grid, 0, c.plan.grid)); NB_TRY(c.wgrad(st, sms, 0, c.plan.grid)); NB_TRY(c.heads(st));
-    return 0;
-  }
+  NB_TRY(c.prologue(st)); NB_TRY(c.dgrad(st)); NB_TRY(c.wgrad(st)); NB_TRY(c.heads(st));
+  if (!fine) return 0;
   BwdTcPass f = bind_pass(rays, N, cfg, fine);
   NB_TRY(f.init(static_cast<uint8_t*>(workspace) + cb, workspace_bytes - cb));
-  const bool shared_grads = (coarse->grads->pts_w[0] == fine->grads->pts_w[0]);       // one network serving both passes: += races
-  int w = env_w;
-  if (w > sms - 16) w = sms - 16;
-  if (w > 0) w &= ~1;
-  if (w == 0 || (w > 0 && w < 16) || shared_grads || f.plan.grid < 4) {
-    static int dc = -1, wc = -1;                       // NERF_B200_DBG_BWD_CTAS="d,w": CTA caps of the two kernels (scaling experiments)
-    if (dc < 0) { dc = 1 << 20; wc = sms; const char* e = exp_env("NERF_B200_DBG_BWD_CTAS"); if (e) { int a = 0, b = 0; if (sscanf(e, "%d,%d", &a, &b) == 2 && a >= 2 && b >= 16 && b <= sms) { dc = a; wc = b; } } }
-    NB_TRY(c.prologue(st)); NB_TRY(c.dgrad(st, dc, 0, c.plan.grid)); NB_TRY(c.wgrad(st, wc, 0, c.plan.grid)); NB_TRY(c.heads(st));
-    NB_TRY(f.prologue(st)); NB_TRY(f.dgrad(st, dc, 0, f.plan.grid)); NB_TRY(f.wgrad(st, wc, 0, f.plan.grid)); NB_TRY(f.heads(st));
-    return 0;
-  }
-  if (!ds->side) {                                   // (creation failed at start-up: one stream, one pass after the other)
-    NB_TRY(c.prologue(st)); NB_TRY(c.dgrad(st, c.plan.grid, 0, c.plan.grid)); NB_TRY(c.wgrad(st, sms, 0, c.plan.grid)); NB_TRY(c.heads(st));
-    NB_TRY(f.prologue(st)); NB_TRY(f.dgrad(st, f.plan.grid, 0, f.plan.grid)); NB_TRY(f.wgrad(st, sms, 0, f.plan.grid)); NB_TRY(f.heads(st));
-    return 0;
-  }
-  cudaStream_t sd = ds->side;
-  if (w < 0) {
-    // ---- default: the small kernels ride next to the weight-gradient kernels ----
-    NB_TRY(c.prologue(st));
-    NB_TRY(c.dgrad(st, c.plan.grid, 0, c.plan.grid));
-    NB_CUDA(cudaEventRecord(ds->ev[0], st));
-    NB_CUDA(cudaStreamWaitEvent(sd, ds->ev[0], 0));
-    NB_TRY(f.prologue(sd));
-    NB_CUDA(cudaEventRecord(ds->ev[1], sd));
-    NB_TRY(c.wgrad(st, sms, 0, c.plan.grid));
-    NB_CUDA(cudaStreamWaitEvent(st, ds->ev[1], 0));
-    NB_TRY(f.dgrad(st, f.plan.grid, 0, f.plan.grid));
-    NB_CUDA(cudaEventRecord(ds->ev[2], st));
-    NB_CUDA(cudaStreamWaitEvent(sd, ds->ev[2], 0));
-    NB_TRY(c.heads(sd));
-    NB_CUDA(cudaEventRecord(ds->ev[3], sd));
-    NB_TRY(f.wgrad(st, sms, 0, f.plan.grid));
-    NB_TRY(f.heads(st));
-    NB_CUDA(cudaStreamWaitEvent(st, ds->ev[3], 0));
-    return 0;
-  }
-  // ---- SM split (experiment) ----
-  int chunks = env_chunks;
-  if (chunks > 8) chunks = 8;
-  if (chunks > f.plan.grid / 2) chunks = f.plan.grid / 2;
-  if (chunks < 1) chunks = 1;
-  NB_TRY(c.prologue(st));
-  NB_TRY(f.prologue(st));
-  NB_TRY(c.dgrad(st, c.plan.grid, 0, c.plan.grid));
-  NB_CUDA(cudaEventRecord(ds->ev[0], st));
-  NB_CUDA(cudaStreamWaitEvent(sd, ds->ev[0], 0));
-  NB_TRY(c.wgrad(sd, w, 0, c.plan.grid));
-  NB_TRY(c.heads(sd));
-  // fine pass: `chunks` ranges of the forward's CTA pairs; chunk k's weight gradient runs on the side stream next to chunk
-  // k + 1's chain, the last chunk's on the main stream with all SMs
-  const int pairs = f.plan.grid / 2;
-  int v0 = 0, v1 = 0;
-  for (int k = 0; k < chunks; ++k) {
-    v0 = 2 * (int)((long long)pairs * k / chunks); v1 = 2 * (int)((long long)pairs * (k + 1) / chunks);
-    NB_TRY(f.dgrad(st, sms - w, v0, v1));
-    if (k + 1 < chunks) {
-      NB_CUDA(cudaEventRecord(ds->ev[k + 1], st));
-      NB_CUDA(cudaStreamWaitEvent(sd, ds->ev[k + 1], 0));
-      NB_TRY(f.wgrad(sd, w, v0, v1));
-    }
-  }
-  NB_CUDA(cudaEventRecord(ds->ev[9], sd));
-  NB_CUDA(cudaStreamWaitEvent(st, ds->ev[9], 0));
-  NB_TRY(f.wgrad(st, sms, v0, v1));
-  NB_TRY(f.heads(st));
+  NB_TRY(f.prologue(st)); NB_TRY(f.dgrad(st)); NB_TRY(f.wgrad(st)); NB_TRY(f.heads(st));
   return 0;
 }
 
@@ -1189,7 +994,5 @@ int nerf_b200_adam_step(float* params, const float* grads, float* exp_avg, float
   NB_LAUNCH_OK("adam_advance_kernel");
   return 0;
 }
-
-int nerf_b200_debug_set_trace(void* dev_buf_4096_i64) { g_trace = static_cast<long long*>(dev_buf_4096_i64); return 0; }
 
 }  // extern "C"

@@ -28,51 +28,11 @@ extern "C" {
 
 const char* nerf_b200_dev_last_error(void) { return g_err; }
 
-int nerf_b200_debug_mma_rate(int reps, int N, int b_sw64, void* out_2_i64, void* stream) {
-  const size_t sm = 65536 + 32768 + 256 + 1024;
-  if (int rc = smem_optin((const void*)mma_rate_kernel, sm)) return rc;
-  mma_rate_kernel<<<1, 128, sm, (cudaStream_t)stream>>>(reps, N, b_sw64, static_cast<long long*>(out_2_i64));
-  NB_LAUNCH_OK("mma_rate_kernel");
-  return 0;
-}
-
-int nerf_b200_debug_epi_rate(int reps, int mode, int mma, void* out_2_i64, void* stream) {
-  const size_t sm = 65536 + 49152 + 1024 + 256 + 1024;
-  if (int rc = smem_optin((const void*)epi_rate_kernel, sm)) return rc;
-  epi_rate_kernel<<<1, 384, sm, (cudaStream_t)stream>>>(reps, mode, mma, static_cast<long long*>(out_2_i64));
-  NB_LAUNCH_OK("epi_rate_kernel");
-  return 0;
-}
-
-int nerf_b200_debug_ldtm_rate(int reps, int shape, int nwarps, int mma, void* out_2_i64, void* stream) {
-  const size_t sm = 49152 + 256 + 1024;
-  if (int rc = smem_optin((const void*)ldtm_rate_kernel, sm)) return rc;
-  ldtm_rate_kernel<<<1, 384, sm, (cudaStream_t)stream>>>(reps, shape, nwarps, mma, static_cast<long long*>(out_2_i64));
-  NB_LAUNCH_OK("ldtm_rate_kernel");
-  return 0;
-}
-
-int nerf_b200_debug_issue_probe(int reps, int nmma, int flags, void* out_2_i64, void* stream) {
-  const size_t sm = 65536 + 32768 + 256 + 1024;
-  if (int rc = smem_optin((const void*)issue_probe_kernel, sm)) return rc;
-  issue_probe_kernel<<<1, 128, sm, (cudaStream_t)stream>>>(reps, nmma, flags, static_cast<long long*>(out_2_i64));
-  NB_LAUNCH_OK("issue_probe_kernel");
-  return 0;
-}
-
-int nerf_b200_debug_l2_stream(const void* buf, int buf_bytes, int chunk, int stages, int passes, int nblocks, void* out_i64, void* stream) {
-  const size_t sm = (size_t)stages * chunk + 512 + 1024;
-  if (int rc = smem_optin((const void*)l2_stream_probe_kernel, sm)) return rc;
-  l2_stream_probe_kernel<<<nblocks, 64, sm, (cudaStream_t)stream>>>(static_cast<const uint8_t*>(buf), buf_bytes, chunk, stages, passes, static_cast<long long*>(out_i64));
-  NB_LAUNCH_OK("l2_stream_probe_kernel");
-  return 0;
-}
-
 int nerf_b200_selftest_gemm_tn(const float* X, const float* Y, float* out, int lbo_bytes, int sbo_bytes, void* stream) {
   NB_CHECK_ARG(X && Y && out, "null pointer");
   NB_CHECK_ARG(lbo_bytes >= 0 && sbo_bytes >= 0 && lbo_bytes % 16 == 0 && sbo_bytes % 16 == 0, "lbo / sbo must be multiples of 16 bytes");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int sm = 131072 + 256 + 1024;
+  const int sm = 131072;
   if (int rc = smem_optin((const void*)selftest_gemm_tn_kernel, sm)) return rc;
   selftest_gemm_tn_kernel<<<1, 128, sm, st>>>(X, Y, out, (uint32_t)lbo_bytes, (uint32_t)sbo_bytes);
   NB_LAUNCH_OK("selftest_gemm_tn_kernel");
@@ -90,9 +50,9 @@ int nerf_b200_selftest_gemm(const float* A, const float* W, int K, int N, float*
   dim3 grid(4, job.n);
   pack_chunks_kernel<<<grid, 256, 0, st>>>(job, static_cast<uint8_t*>(scratch));
   NB_LAUNCH_OK("pack_chunks_kernel");
-  const size_t sm = 65536 + 16384 + 256 + 1024;
+  const size_t sm = 65536 + 131072 + 64;
   if (int rc = smem_optin((const void*)selftest_gemm_kernel, sm)) return rc;
-  selftest_gemm_kernel<<<1, 128, sm, st>>>(A, static_cast<const uint8_t*>(scratch), K, N, out);
+  selftest_gemm_kernel<<<1, 256, sm, st>>>(A, static_cast<const uint8_t*>(scratch), K, N, out);
   NB_LAUNCH_OK("selftest_gemm_kernel");
   return 0;
 }

@@ -1,462 +1,106 @@
-// dev_kernels.cuh -- bring-up and measurement kernels, NOT part of the product library: tcgen05 self-test GEMMs (K-major
-// and MN-major operand encodings) and the issue / epilogue / TMEM-load / L2-stream micro-benchmarks behind
-// profiles/r01_summary.md.  Compiled only into libnerf_b200_dev.so (capi_dev.cu).  The single-CTA fused pass that the
-// CTA-pair kernel superseded (3.1 M rays/s, round 1) was removed from the tree in round 2 (git: fused_tc.cuh @ be69ba1).
+// dev_kernels.cuh -- bring-up and measurement kernels, NOT part of the product library: wgmma self-test GEMMs (K-major
+// and MN-major operand encodings of the fused pass and of the weight gradient) and the HBM stream probes.  Compiled only
+// into libnerf_b200_dev.so (capi_dev.cu).
 #pragma once
 #include "fused_tc.cuh"
+#include "fused_wg.cuh"
 
 namespace nb {
 
 // ---------------------------------------------------------------------------------------------
-// self-test GEMM: out[128,N] = A[128,K] * W[N,K]^T through exactly the operand layouts, descriptors,
-// bulk copies and TMEM loads the march kernel uses (fp16 operands, fp32 accumulate).  1 CTA.
+// self-test GEMM: out[128,N] = A[128,K] * W[N,K]^T through exactly the operand layouts and descriptors the fused pass uses
+// (A: 64-row K-blocks of 8 KB, SWIZZLE_128B, written by threads; W: packed [N x 32] SWIZZLE_64B chunks by bulk copy; fp16
+// operands, fp32 accumulation).  1 CTA = 2 warpgroups, each on 64 rows.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) selftest_gemm_kernel(const float* __restrict__ A, const uint8_t* __restrict__ chunks,
-                                                             int K, int N, float* __restrict__ out) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t sb = ptx::smem_u32(smem);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, r = threadIdx.x;
-  const uint32_t ACT = 0, WST = 65536, BAR = 65536 + 16384, TPTR = BAR + 64;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + TPTR);
-  if (threadIdx.x == 0) { ptx::mbar_init(sb + BAR, 1); ptx::mbar_init(sb + BAR + 8, 1); ptx::fence_mbar_init(); }
-  if (warp == 0) { ptx::tmem_alloc(ptx::smem_u32(s_tmem), 256); ptx::tmem_relinquish(); }
-  // A -> fp16, 128B-swizzled K-major (thread r owns row r), K padded to a multiple of 32 by the caller
-  for (int c0 = 0; c0 < K; c0 += 32) {
-    float x[32];
-    for (int j = 0; j < 32; ++j) x[j] = A[(size_t)r * K + c0 + j];
-    store_act32<false>(x, sb + ACT, r, c0);
+template <int N>
+__device__ __forceinline__ void selftest_gemm_body(const float* A, const uint8_t* chunks, int K, float* out, uint32_t sb) {
+  constexpr uint32_t WST = 65536, BAR = WST + 131072;
+  const int w = threadIdx.x >> 7, t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
+  const uint32_t act = sb + (uint32_t)w * 32768u;
+  // rows 64 w .. of A as fp16 into the warpgroup's K-blocks
+  for (int i = t; i < 64 * (K / 2); i += 128) {
+    const int r = i / (K / 2), c = 2 * (i % (K / 2));
+    const float* a = A + (size_t)(64 * w + r) * K + c;
+    ptx::st_shared_b32(act + half_off(r, c), ptx::cvt_f16x2(a[0], a[1]));
+  }
+  const uint32_t cb = (uint32_t)N * 64u * (uint32_t)(K / 32);
+  if (threadIdx.x == 0) {
+    ptx::mbar_init(sb + BAR, 1);
+    ptx::fence_mbar_init();
   }
   ptx::fence_proxy_async_smem();
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *s_tmem;
   if (threadIdx.x == 0) {
-    const uint32_t cb = (uint32_t)N * 64;
-    const uint32_t idesc = ptx::umma_idesc_f16(128, N);
-    for (int c = 0; c < K / 32; ++c) {
-      ptx::mbar_arrive_expect_tx(sb + BAR, cb);
-      ptx::bulk_g2s(sb + WST, chunks + (size_t)c * cb, cb, sb + BAR);
-      ptx::mbar_wait(sb + BAR, c & 1);
-      ptx::tc_fence_after();
-      const uint32_t a_base = sb + ACT + (c >> 1) * 16384 + (c & 1) * 64;
-      for (int j = 0; j < 2; ++j)
-        ptx::mma_f16_ss(tmem, ptx::umma_desc(a_base + j * 32, 1024, ptx::UMMA_SW128),
-                        ptx::umma_desc(sb + WST + j * 32, 512, ptx::UMMA_SW64), idesc, (c > 0 || j > 0) ? 1u : 0u);
-      ptx::mma_commit(sb + BAR + 8);
-      ptx::mbar_wait(sb + BAR + 8, c & 1);       // serialise: the single weight stage is reused
-    }
-  }
-  __syncthreads();
-  ptx::tc_fence_after();
-  for (int col0 = 0; col0 < N; col0 += 32) {
-    uint32_t v[32];
-    ptx::tmem_ld_x32(tmem + ((uint32_t)(32 * warp) << 16) + col0, v);
-    ptx::tmem_ld_wait();
-    for (int j = 0; j < 32; ++j) out[(size_t)r * N + col0 + j] = __uint_as_float(v[j]);
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc(tmem, 256);
-}
-
-// ---------------------------------------------------------------------------------------------
-// "TN" self-test for the weight-gradient GEMM of the backward (round 2): out[256,256] = X^T Y with
-// X, Y [128 rows, 256] given as the forward's activation tiles (row = sample, K-blocks of 64 columns,
-// SWIZZLE_128B) and read by the MMA as MN-MAJOR operands: A = X viewed [M = column, K = row],
-// B = Y viewed [N = column, K = row].  The canonical MN-major SWIZZLE_128B atom is 64 contiguous
-// MN elements x 8 K rows = the same physical 1 KB atom as the K-major one, so no re-layout is needed:
-// LBO = stride between 64-column groups (16 KB: the K-block stride), SBO = stride between 8-row groups
-// (1 KB).  lbo / sbo are arguments so that one GPU run can confirm the encoding.  1 CTA, 128 threads.
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) selftest_gemm_tn_kernel(const float* __restrict__ X, const float* __restrict__ Y,
-                                                                float* __restrict__ out, uint32_t lbo, uint32_t sbo) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t sb = ptx::smem_u32(smem);
-  const int warp = threadIdx.x >> 5, r = threadIdx.x;
-  const uint32_t XT = 0, YT = 65536, BAR = 131072, TPTR = BAR + 64;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + TPTR);
-  if (threadIdx.x == 0) { ptx::mbar_init(sb + BAR, 1); ptx::fence_mbar_init(); }
-  if (warp == 0) { ptx::tmem_alloc(ptx::smem_u32(s_tmem), 512); ptx::tmem_relinquish(); }
-  for (int c0 = 0; c0 < 256; c0 += 32) {
-    float x[32], y[32];
-    for (int j = 0; j < 32; ++j) { x[j] = X[(size_t)r * 256 + c0 + j]; y[j] = Y[(size_t)r * 256 + c0 + j]; }
-    store_act32<false>(x, sb + XT, r, c0);
-    store_act32<false>(y, sb + YT, r, c0);
-  }
-  ptx::fence_proxy_async_smem();
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *s_tmem;
-  if (threadIdx.x == 0) {
-    const uint32_t idesc = ptx::umma_idesc_f16_major(128, 256, 1, 1);
-    for (int mh = 0; mh < 2; ++mh)                      // output rows (X columns) 0-127, 128-255
-      for (int k = 0; k < 8; ++k) {                     // 16 sample rows per MMA: two 8-row groups = 2 KB
-        const uint64_t ad = ptx::umma_desc_full(sb + XT + mh * 2 * 16384 + k * 2048, lbo, sbo, ptx::UMMA_SW128);
-        const uint64_t bd = ptx::umma_desc_full(sb + YT + k * 2048, lbo, sbo, ptx::UMMA_SW128);
-        ptx::mma_f16_ss(tmem + mh * 256, ad, bd, idesc, k > 0 ? 1u : 0u);
-      }
-    ptx::mma_commit(sb + BAR);
+    ptx::mbar_arrive_expect_tx(sb + BAR, cb);
+    ptx::bulk_g2s(sb + WST, chunks, cb, sb + BAR);
   }
   ptx::mbar_wait(sb + BAR, 0);
-  ptx::tc_fence_after();
-  for (int mh = 0; mh < 2; ++mh)
-    for (int col0 = 0; col0 < 256; col0 += 32) {
-      uint32_t v[32];
-      ptx::tmem_ld_x32(tmem + ((uint32_t)(32 * warp) << 16) + mh * 256 + col0, v);
-      ptx::tmem_ld_wait();
-      for (int j = 0; j < 32; ++j) out[(size_t)(mh * 128 + r) * 256 + col0 + j] = __uint_as_float(v[j]);
-    }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc(tmem, 512);
+  float acc[N / 2];
+  ptx::wgmma_fence();
+  for (int c = 0; c < K / 32; ++c) {
+    const uint64_t ad = desc_act(act + (uint32_t)(c >> 1) * 8192u + (uint32_t)(c & 1) * 64u);
+    const uint64_t bd = desc_w(sb + WST + (uint32_t)c * N * 64u);
+    mma_chunk(acc, ad, bd, c > 0 ? 1u : 0u);
+  }
+  ptx::wgmma_commit();
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(acc);
+  const int r0 = 64 * w + 16 * wq + (lane >> 2), q4 = lane & 3;
+  for (int j = 0; j < N / 8; ++j) {
+    const int c = 8 * j + 2 * q4;
+    out[(size_t)r0 * N + c] = acc[4 * j]; out[(size_t)r0 * N + c + 1] = acc[4 * j + 1];
+    out[(size_t)(r0 + 8) * N + c] = acc[4 * j + 2]; out[(size_t)(r0 + 8) * N + c + 1] = acc[4 * j + 3];
+  }
+}
+__global__ void __launch_bounds__(256, 1) selftest_gemm_kernel(const float* __restrict__ A, const uint8_t* __restrict__ chunks,
+                                                               int K, int N, float* __restrict__ out) {
+  const uint32_t sb = ptx::smem_u32(tc_smem);
+  if ((sb & 1023u) != 0) __trap();
+  if (N == 256) selftest_gemm_body<256>(A, chunks, K, out, sb);
+  else selftest_gemm_body<128>(A, chunks, K, out, sb);
 }
 
-// MMA issue-rate microbenchmark: `reps` x (M=128, N, K=16) tcgen05.mma on resident (garbage) operands,
-// alternating between two accumulators; out[0] = cycles from first issue to completion of the last.
-__global__ void __launch_bounds__(128, 1) mma_rate_kernel(int reps, int N, int b_sw64, long long* out) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t sb = ptx::smem_u32(smem);
-  const int warp = threadIdx.x >> 5;
-  const uint32_t BAR = 65536 + 32768, TPTR = BAR + 64;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + TPTR);
-  for (int i = threadIdx.x; i < (65536 + 32768) / 4; i += 128) reinterpret_cast<uint32_t*>(smem)[i] = 0x3c003c00u;   // fp16 1.0
-  if (threadIdx.x == 0) { ptx::mbar_init(sb + BAR, 1); ptx::fence_mbar_init(); }
-  if (warp == 0) { ptx::tmem_alloc(ptx::smem_u32(s_tmem), 512); ptx::tmem_relinquish(); }
+// ---------------------------------------------------------------------------------------------
+// "TN" self-test for the weight-gradient GEMM of the backward: out[256,256] = X^T Y with X, Y [128 rows, 256] given as
+// activation tiles (row = sample, K-blocks of 64 columns x 128 rows, SWIZZLE_128B) and read by the MMA as MN-MAJOR operands:
+// A = X viewed [M = column, K = row], B = Y viewed [N = column, K = row].  The canonical MN-major SWIZZLE_128B atom is 64
+// contiguous MN elements x 8 K rows = the same physical 1 KB atom as the K-major one, so no re-layout is needed:
+// LBO = stride between 64-column groups (16 KB: the K-block stride), SBO = stride between 8-row groups (1 KB).  lbo / sbo
+// are arguments so that one GPU run can confirm the encoding.  1 CTA = 1 warpgroup, one 64-row block of out at a time.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128, 1) selftest_gemm_tn_kernel(const float* __restrict__ X, const float* __restrict__ Y,
+                                                                  float* __restrict__ out, uint32_t lbo, uint32_t sbo) {
+  const uint32_t sb = ptx::smem_u32(tc_smem);
+  if ((sb & 1023u) != 0) __trap();
+  constexpr uint32_t XT = 0, YT = 65536;
+  const int t = threadIdx.x, wq = t >> 5, lane = t & 31;
+  for (int i = t; i < 128 * 128; i += 128) {
+    const int r = i >> 7, c = 2 * (i & 127);
+    const uint32_t o = (uint32_t)(c >> 6) * 16384u + (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2);
+    ptx::st_shared_b32(sb + XT + o, ptx::cvt_f16x2(X[r * 256 + c], X[r * 256 + c + 1]));
+    ptx::st_shared_b32(sb + YT + o, ptx::cvt_f16x2(Y[r * 256 + c], Y[r * 256 + c + 1]));
+  }
   ptx::fence_proxy_async_smem();
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *s_tmem;
-  if (threadIdx.x == 0) {
-    const uint32_t idesc = ptx::umma_idesc_f16(128, N);
-    const long long t0 = clock64();
-    for (int i = 0; i < reps; ++i) {
-      const uint32_t a = sb + ((i >> 1) & 3) * 16384 + (i & 1) * 32;
-      const uint64_t bd = b_sw64 ? ptx::umma_desc(sb + 65536 + (i & 1) * 32, 512, ptx::UMMA_SW64)
-                                 : ptx::umma_desc(sb + 65536 + (i & 3) * 32, 1024, ptx::UMMA_SW128);
-      ptx::mma_f16_ss(tmem + (i & 1) * 256, ptx::umma_desc(a, 1024, ptx::UMMA_SW128), bd, idesc, 1u);
+  float acc[128];
+  for (int mb = 0; mb < 4; ++mb) {
+    ptx::wgmma_fence();
+    for (int k = 0; k < 8; ++k) {
+      const uint64_t ad = ptx::gmma_desc(sb + XT + mb * 16384 + k * 2048, lbo, sbo, ptx::GMMA_SW128);
+      const uint64_t bd = ptx::gmma_desc(sb + YT + k * 2048, lbo, sbo, ptx::GMMA_SW128);
+      ptx::wgmma_m64n256k16<1, 1>(acc, ad, bd, k > 0 ? 1u : 0u);
     }
-    const long long t1 = clock64();
-    ptx::mma_commit(sb + BAR);
-    ptx::mbar_wait(sb + BAR, 0);
-    const long long t2 = clock64();
-    out[0] = t2 - t0; out[1] = t1 - t0;
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc(tmem, 512);
-}
-
-// Epilogue-rate microbenchmark: 8 warps drain a 128x256 fp32 accumulator `reps` times the way the
-// march kernel does (mode 0: tcgen05.ld only; 1: + bias/ReLU/convert; 2: + st.shared of the A tile),
-// optionally while another warp keeps the tensor pipe busy on the other accumulator (mma != 0).
-// out[0] = cycles for `reps` tile-layer epilogues (warp 4 lane 0).
-__global__ void __launch_bounds__(384, 1) epi_rate_kernel(int reps, int mode, int mma, long long* out) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t sb = ptx::smem_u32(smem);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t ACT = 0, OPS = 65536, BIAS = 65536 + 49152, BAR = BIAS + 1024, TPTR = BAR + 64;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + TPTR);
-  float* s_bias = reinterpret_cast<float*>(smem + BIAS);
-  volatile int* s_stop = reinterpret_cast<volatile int*>(smem + TPTR + 16);
-  for (int i = threadIdx.x; i < (65536 + 49152) / 4; i += 384) reinterpret_cast<uint32_t*>(smem)[i] = 0x3c003c00u;
-  if (threadIdx.x < 256) s_bias[threadIdx.x] = 0.5f;
-  if (threadIdx.x == 0) { ptx::mbar_init(sb + BAR, 1); ptx::fence_mbar_init(); *s_stop = 0; }
-  if (warp == 0) { ptx::tmem_alloc(ptx::smem_u32(s_tmem), 512); ptx::tmem_relinquish(); }
-  ptx::fence_proxy_async_smem();
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *s_tmem;
-  if (warp == 1) {
-    if (lane == 0 && mma) {
-      const uint32_t idesc = ptx::umma_idesc_f16(128, 256);
-      int i = 0;
-      while (!*s_stop) {
-        for (int j = 0; j < 8; ++j, ++i)
-          ptx::mma_f16_ss(tmem + 256, ptx::umma_desc(sb + OPS + (i & 1) * 32, 1024, ptx::UMMA_SW128),
-                          ptx::umma_desc(sb + OPS + 16384 + (i & 1) * 32, 512, ptx::UMMA_SW64), idesc, 1u);
-        ptx::mma_commit(sb + BAR);
-        ptx::mbar_wait(sb + BAR, (i / 8 - 1) & 1);
-      }
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_regs(acc);
+    const int r0 = 64 * mb + 16 * wq + (lane >> 2), q4 = lane & 3;
+    for (int j = 0; j < 32; ++j) {
+      const int c = 8 * j + 2 * q4;
+      out[r0 * 256 + c] = acc[4 * j]; out[r0 * 256 + c + 1] = acc[4 * j + 1];
+      out[(r0 + 8) * 256 + c] = acc[4 * j + 2]; out[(r0 + 8) * 256 + c + 1] = acc[4 * j + 3];
     }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int e = warp - 4, q = e & 3, ch = e >> 2, r = 32 * q + lane;
-    const uint32_t t_lane = tmem + ((uint32_t)(32 * q) << 16);
-    float sink = 0.f;
-    const int math = mode & 3;
-    const bool no_pfence = mode & 4, no_tfence = mode & 8, no_bar = mode & 16, dual = mode & 32;
-    long long ldw = 0;
-    ptx::named_bar_sync(1, 256);
-    const long long t0 = clock64();
-    for (int it = 0; it < reps; ++it) {
-      if (dual) {
-#pragma unroll 1
-        for (int b = 0; b < 2; ++b) {
-          const int col0 = ch * 128 + b * 64;
-          uint32_t v[32], w[32];
-          const long long c0 = clock64();
-          ptx::tmem_ld_x32(t_lane + col0, v);
-          ptx::tmem_ld_x32(t_lane + col0 + 32, w);
-          ptx::tmem_ld_wait();
-          ldw += clock64() - c0;
-          sink += __uint_as_float(v[it & 31]) + __uint_as_float(w[it & 31]);
-        }
-      } else {
-#pragma unroll 1
-        for (int b = 0; b < 4; ++b) {
-          const int col0 = ch * 128 + b * 32;
-          uint32_t v[32];
-          const long long c0 = clock64();
-          ptx::tmem_ld_x32(t_lane + col0, v);
-          ptx::tmem_ld_wait();
-          ldw += clock64() - c0;
-          if (math == 0) { sink += __uint_as_float(v[it & 31]); continue; }
-          float x[32];
-          const float4* b4 = reinterpret_cast<const float4*>(s_bias + col0);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 bb = b4[j];
-            x[4 * j + 0] = __uint_as_float(v[4 * j + 0]) + bb.x; x[4 * j + 1] = __uint_as_float(v[4 * j + 1]) + bb.y;
-            x[4 * j + 2] = __uint_as_float(v[4 * j + 2]) + bb.z; x[4 * j + 3] = __uint_as_float(v[4 * j + 3]) + bb.w;
-          }
-          if (math == 1) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) sink += __uint_as_float(ptx::cvt_relu_f16x2(x[j], x[j + 1]));
-          } else store_act32<true>(x, sb + ACT, r, col0);
-        }
-      }
-      if (!no_tfence) ptx::tc_fence_before();
-      if (!no_pfence) ptx::fence_proxy_async_smem();
-      if (!no_bar) ptx::named_bar_sync(1, 256);
-    }
-    const long long t1 = clock64();
-    if (e == 0 && lane == 0) { out[0] = t1 - t0; out[1] = ldw; *s_stop = 1; }
-    if (sink == 123.456f) out[1] = 1;
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc(tmem, 512);
-}
-
-// L2 -> shared-memory streaming probe: every CTA streams the same `buf_bytes` buffer `passes` times through a ring of
-// `stages` x `chunk` bytes with cp.async.bulk (a consumer warp frees a stage as soon as it lands).
-// out[blockIdx.x*2] = cycles, out[blockIdx.x*2+1] = summed issue->landed latency of warp 0's copies.
-__global__ void __launch_bounds__(64, 1) l2_stream_probe_kernel(const uint8_t* __restrict__ buf, int buf_bytes, int chunk, int stages,
-                                                              int passes, long long* out) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t sb = ptx::smem_u32(smem);
-  const uint32_t BAR = (uint32_t)stages * (uint32_t)chunk;
-  const int warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) { for (int i = 0; i < stages; ++i) { ptx::mbar_init(sb + BAR + 8 * i, 1); ptx::mbar_init(sb + BAR + 128 + 8 * i, 1); } ptx::fence_mbar_init(); }
-  __syncthreads();
-  const int n = (buf_bytes / chunk) * passes;
-  const long long t0 = clock64();
-  if (warp == 0) {
-    uint32_t stage = 0, ph = 0;
-    int off = 0;
-    for (int i = 0; i < n; ++i) {
-      ptx::mbar_wait(sb + BAR + 128 + 8 * stage, ph ^ 1);
-      if (ptx::elect_one()) {
-        ptx::mbar_arrive_expect_tx(sb + BAR + 8 * stage, chunk);
-        ptx::bulk_g2s(sb + stage * chunk, buf + off, chunk, sb + BAR + 8 * stage);
-      }
-      __syncwarp();
-      off += chunk; if (off + chunk > buf_bytes) off = 0;
-      if (++stage == (uint32_t)stages) { stage = 0; ph ^= 1; }
-    }
-  } else {
-    uint32_t stage = 0, ph = 0;
-    for (int i = 0; i < n; ++i) {
-      ptx::mbar_wait(sb + BAR + 8 * stage, ph);
-      if (ptx::elect_one()) ptx::mbar_arrive(sb + BAR + 128 + 8 * stage);
-      __syncwarp();
-      if (++stage == (uint32_t)stages) { stage = 0; ph ^= 1; }
-    }
-    if (threadIdx.x == 32) out[blockIdx.x] = clock64() - t0;
   }
 }
-
-// Issue-overhead probe: one thread runs `reps` iterations of {optional mbarrier try_wait on a completed
-// barrier; `nmma` x tcgen05.mma (N=256, K=16); optional tcgen05.commit to a scratch barrier} and reports the
-// cycles per iteration (out[0] = to completion of everything, out[1] = issue loop only).
-//   flags bit0: try_wait per iteration   bit1: one commit per iteration   bit2: two commits   bit3: tcgen05.fence::after
-__global__ void __launch_bounds__(128, 1) issue_probe_kernel(int reps, int nmma, int flags, long long* out) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t sb = ptx::smem_u32(smem);
-  const int warp = threadIdx.x >> 5;
-  const uint32_t BAR = 65536 + 32768, TPTR = BAR + 64;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + TPTR);
-  for (int i = threadIdx.x; i < (65536 + 32768) / 4; i += 128) reinterpret_cast<uint32_t*>(smem)[i] = 0x3c003c00u;
-  if (threadIdx.x == 0) { ptx::mbar_init(sb + BAR, 1); ptx::mbar_init(sb + BAR + 8, 1); ptx::mbar_init(sb + BAR + 16, 1); ptx::fence_mbar_init(); }
-  if (warp == 0) { ptx::tmem_alloc(ptx::smem_u32(s_tmem), 512); ptx::tmem_relinquish(); }
-  ptx::fence_proxy_async_smem();
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *s_tmem;
-  if (warp == 0 && (flags & 128)) {
-    // warp-uniform control flow, only the tcgen05 instructions are issued by one elected lane
-    const uint32_t idesc = ptx::umma_idesc_f16(128, 256);
-    const uint32_t tm = __shfl_sync(0xffffffffu, tmem, 0);
-    if (threadIdx.x == 0) ptx::mbar_arrive(sb + BAR + 16);
-    __syncwarp();
-    const uint64_t ad = ptx::umma_desc(sb, 1024, ptx::UMMA_SW128), bd = ptx::umma_desc(sb + 65536, 512, ptx::UMMA_SW64);
-    const long long t0 = clock64();
-    for (int i = 0; i < reps; ++i) {
-      if (flags & 1) ptx::mbar_wait(sb + BAR + 16, 0);
-      if (flags & 8) ptx::tc_fence_after();
-      if (ptx::elect_one()) {
-        for (int j = 0; j < nmma; ++j) {
-          const uint32_t dsel = (flags & 16) ? 0u : ((flags & 32) ? (uint32_t)(j & 1) : (uint32_t)(i & 1));
-          const uint32_t ks = (flags & 64) ? (uint32_t)((i + j) & 3) : (uint32_t)(j & 1);
-          ptx::mma_f16_ss(tm + dsel * 256, ad + 2 * ks, bd + 2 * (ks & 1), idesc, 1u);
-        }
-        if (flags & 2) ptx::mma_commit(sb + BAR + 8);
-        if (flags & 4) ptx::mma_commit(sb + BAR + 8);
-      }
-      __syncwarp();
-    }
-    const long long t1 = clock64();
-    if (ptx::elect_one()) ptx::mma_commit(sb + BAR);
-    __syncwarp();
-    ptx::mbar_wait(sb + BAR, 0);
-    const long long t2 = clock64();
-    if (threadIdx.x == 0) { out[0] = t2 - t0; out[1] = t1 - t0; }
-  } else if (threadIdx.x == 0 && !(flags & 128)) {
-    const uint32_t idesc = ptx::umma_idesc_f16(128, 256);
-    ptx::mbar_arrive(sb + BAR + 16);                    // complete phase 0 of the "always ready" barrier
-    const uint64_t ad = ptx::umma_desc(sb, 1024, ptx::UMMA_SW128), bd = ptx::umma_desc(sb + 65536, 512, ptx::UMMA_SW64);
-    const long long t0 = clock64();
-    for (int i = 0; i < reps; ++i) {
-      if (flags & 1) ptx::mbar_wait(sb + BAR + 16, 0);
-      if (flags & 8) ptx::tc_fence_after();
-      // flags bit4: keep ONE accumulator (no alternation)   bit5: alternate the accumulator every MMA   bit6: vary operand k-step per iteration
-      for (int j = 0; j < nmma; ++j) {
-        const uint32_t dsel = (flags & 16) ? 0u : ((flags & 32) ? (uint32_t)(j & 1) : (uint32_t)(i & 1));
-        const uint32_t ks = (flags & 64) ? (uint32_t)((i + j) & 3) : (uint32_t)(j & 1);
-        ptx::mma_f16_ss(tmem + dsel * 256, ad + 2 * ks, bd + 2 * (ks & 1), idesc, 1u);
-      }
-      if (flags & 2) ptx::mma_commit(sb + BAR + 8);
-      if (flags & 4) ptx::mma_commit(sb + BAR + 8);
-    }
-    const long long t1 = clock64();
-    ptx::mma_commit(sb + BAR);
-    ptx::mbar_wait(sb + BAR, 0);
-    const long long t2 = clock64();
-    out[0] = t2 - t0; out[1] = t1 - t0;
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc(tmem, 512);
-}
-
-// TMEM -> register load-rate probe.  `nwarps` warps (4 or 8) each drain their share of a 128-lane x 256-column
-// fp32 accumulator `reps` times with the given tcgen05.ld shape; values are xor-folded so nothing spills.
-//   shape 0: 32x32b.x32 (one load in flight)   1: 32x32b.x32, two loads per wait   2: 32x32b.x64
-//   shape 3: 16x256b.x8 (two per 32-lane group) 4: 16x128b.x16                     5: 32x32b.x16, 4 per wait
-#define NB_LDTM(SHAPE, NREG, ...) asm volatile("tcgen05.ld.sync.aligned." SHAPE ".b32 {" __VA_ARGS__ "}, [%" #NREG "];"
-__device__ __forceinline__ uint32_t fold32(const uint32_t (&v)[32]) { uint32_t a = 0;
-#pragma unroll
-  for (int i = 0; i < 32; ++i) a ^= v[i]; return a; }
-__device__ __forceinline__ void ldtm_16x256b_x8(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile("tcgen05.ld.sync.aligned.16x256b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void ldtm_16x128b_x16(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile("tcgen05.ld.sync.aligned.16x128b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void ldtm_32x32b_x16(uint32_t taddr, uint32_t (&v)[32], int o) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[o + 0]), "=r"(v[o + 1]), "=r"(v[o + 2]), "=r"(v[o + 3]), "=r"(v[o + 4]), "=r"(v[o + 5]), "=r"(v[o + 6]), "=r"(v[o + 7]),
-        "=r"(v[o + 8]), "=r"(v[o + 9]), "=r"(v[o + 10]), "=r"(v[o + 11]), "=r"(v[o + 12]), "=r"(v[o + 13]), "=r"(v[o + 14]), "=r"(v[o + 15])
-      : "r"(taddr) : "memory");
-}
-
-__global__ void __launch_bounds__(384, 1) ldtm_rate_kernel(int reps, int shape, int nwarps, int mma, long long* out) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t sb = ptx::smem_u32(smem);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t OPS = 0, BAR = 49152, TPTR = BAR + 64;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + TPTR);
-  volatile int* s_stop = reinterpret_cast<volatile int*>(smem + TPTR + 16);
-  for (int i = threadIdx.x; i < 49152 / 4; i += 384) reinterpret_cast<uint32_t*>(smem)[i] = 0x3c003c00u;
-  if (threadIdx.x == 0) { ptx::mbar_init(sb + BAR, 1); ptx::fence_mbar_init(); *s_stop = 0; }
-  if (warp == 0) { ptx::tmem_alloc(ptx::smem_u32(s_tmem), 512); ptx::tmem_relinquish(); }
-  ptx::fence_proxy_async_smem();
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *s_tmem;
-  if (warp == 1) {
-    if (lane == 0 && mma) {
-      const uint32_t idesc = ptx::umma_idesc_f16(128, 256);
-      int i = 0;
-      while (!*s_stop) {
-        for (int j = 0; j < 8; ++j, ++i)
-          ptx::mma_f16_ss(tmem + 256, ptx::umma_desc(sb + OPS + (i & 1) * 32, 1024, ptx::UMMA_SW128),
-                          ptx::umma_desc(sb + OPS + 16384 + (i & 1) * 32, 512, ptx::UMMA_SW64), idesc, 1u);
-        ptx::mma_commit(sb + BAR);
-        ptx::mbar_wait(sb + BAR, (i / 8 - 1) & 1);
-      }
-    }
-    __syncwarp();
-  } else if (warp >= 4 && warp < 4 + nwarps) {
-    const int e = warp - 4, q = warp & 3, ch = e >> 2;
-    const int ncol = (nwarps == 8) ? 128 : 256, col_base = (nwarps == 8) ? ch * 128 : 0;
-    const uint32_t t_lane = tmem + ((uint32_t)(32 * q) << 16) + col_base;
-    uint32_t acc = 0;
-    ptx::named_bar_sync(1, nwarps * 32);
-    const long long t0 = clock64();
-    for (int it = 0; it < reps; ++it) {
-      if (shape == 0) {
-#pragma unroll 1
-        for (int c = 0; c < ncol; c += 32) { uint32_t v[32]; ptx::tmem_ld_x32(t_lane + c, v); ptx::tmem_ld_wait(); acc ^= fold32(v); }
-      } else if (shape == 1) {
-#pragma unroll 1
-        for (int c = 0; c < ncol; c += 64) { uint32_t v[32], w[32]; ptx::tmem_ld_x32(t_lane + c, v); ptx::tmem_ld_x32(t_lane + c + 32, w); ptx::tmem_ld_wait(); acc ^= fold32(v) ^ fold32(w); }
-      } else if (shape == 3) {
-#pragma unroll 1
-        for (int c = 0; c < ncol; c += 64) { uint32_t v[32], w[32]; ldtm_16x256b_x8(t_lane + c, v); ldtm_16x256b_x8(t_lane + (16u << 16) + c, w); ptx::tmem_ld_wait(); acc ^= fold32(v) ^ fold32(w); }
-      } else if (shape == 4) {
-#pragma unroll 1
-        for (int c = 0; c < ncol; c += 64) { uint32_t v[32], w[32]; ldtm_16x128b_x16(t_lane + c, v); ldtm_16x128b_x16(t_lane + (16u << 16) + c, w); ptx::tmem_ld_wait(); acc ^= fold32(v) ^ fold32(w); }
-      } else if (shape == 5) {
-#pragma unroll 1
-        for (int c = 0; c < ncol; c += 64) { uint32_t v[32], w[32]; ldtm_32x32b_x16(t_lane + c, v, 0); ldtm_32x32b_x16(t_lane + c + 16, v, 16); ldtm_32x32b_x16(t_lane + c + 32, w, 0); ldtm_32x32b_x16(t_lane + c + 48, w, 16); ptx::tmem_ld_wait(); acc ^= fold32(v) ^ fold32(w); }
-      }
-    }
-    const long long t1 = clock64();
-    ptx::named_bar_sync(1, nwarps * 32);
-    if (e == 0 && lane == 0) { out[0] = t1 - t0; *s_stop = 1; }
-    if (acc == 0x12345u) out[1] = acc;
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc(tmem, 512);
-}
-
 
 // ---- HBM stream probes: what a pure read / pure write / mixed stream reaches on this GPU (context for the training kernels,
 // which are bound by record writes (forward, dgrad) or record reads (wgrad)) -----------------------------------------------

@@ -1,11 +1,10 @@
-// fused_tc.cuh -- shared pieces of the fused tcgen05 network pass: shared-memory map, packed-weight layout and the
-// packing kernels, the per-ray view-bias kernel, and the device helpers of the epilogue (swizzled A-tile stores,
-// in-register positional encoding, segmented warp scans, the compositing of raw2outputs with its warp-to-warp carry).
+// fused_tc.cuh -- shared pieces of the fused tensor-core network pass: shared-memory map, packed-weight layout and the
+// packing kernels, the per-ray view-bias kernel, and the device helpers of the epilogue (in-register positional
+// encoding, segmented warp scans, the compositing of raw2outputs with its warp-to-warp carry).
 //
 // The pass itself -- pts = o + d*z -> positional encoding -> 8x256 MLP (+ heads) -> alpha compositing, replacing
 // run_nerf.py:381-386 / :397-403 (run_network :37-51, batchify :27-34, Embedder.embed run_nerf_helpers.py:36-45,
-// NeRF.forward :96-119, raw2outputs run_nerf.py:262-305) -- is march_tc2_kernel in fused_tc2.cuh (CTA pair,
-// cta_group::2).  The single-CTA kernel it superseded lives in dev_kernels.cuh (libnerf_b200_dev.so only).
+// NeRF.forward :96-119, raw2outputs run_nerf.py:262-305) -- is march_wg_kernel in fused_wg.cuh (wgmma).
 #pragma once
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -13,41 +12,29 @@
 
 namespace nb {
 
-constexpr int TC_THREADS = 640;              // producer + issuer + spare + sampler warps, 16 epilogue warps
-constexpr int TC_SAMPLER_THREADS = 32;       // (register allocation is per 4 warps: 20 warps x 96 regs fit)
 constexpr int TC_W = 256;                 // hidden width supported by the tensor-core path
 constexpr int TC_MAXD = 8;                // pts layers supported (bias table lives in smem)
-constexpr int TC_TILE = 128;              // rows per MMA tile
-constexpr int TC_ST = 256;                // rows per super-tile (two tile slots)
-constexpr int TC_NST = 3;                 // weight ring stages
+constexpr int TC_TILE = 128;              // rows per tile (one record); each of the two MMA warpgroups owns 64 of them
+constexpr int TC_ST = 256;                // rows per super-tile (two tiles: the record order of the tile plan)
 constexpr int TC_CHUNK_K = 32;            // K per weight chunk
-constexpr uint32_t TC_STAGE_BYTES = 256 * TC_CHUNK_K * 2;   // 16 KB
+constexpr uint32_t TC_STAGE_BYTES = 256 * TC_CHUNK_K * 2;   // 16 KB: one [N = 256 x K = 32] weight chunk
 
-// shared-memory map (bytes, relative to a 1024-aligned base)
-constexpr uint32_t SM_ACT = 0;                                  // 2 x 64 KB  A operand (4 K-blocks x 16 KB)
-constexpr uint32_t SM_ENC = 131072;                             // 2 x 16 KB  encoded inputs (1 K-block)
-constexpr uint32_t SM_WRING = 163840;                           // 3 x 16 KB  weight ring
-constexpr uint32_t SM_ONES = 212992;                            // 256 B: ONE 8-row atom of the bias-selector A slab (K=16, SWIZZLE_32B,
-                                                                //        SBO = 0: all 128 rows read the same atom)
-constexpr uint32_t SM_BIASB = SM_ONES + 512;                    // 213504: 8 KB resident B operand [256 x K=16]: all layers' biases
-                                                                //        (one 256-byte selector atom per tile slot before it)
-constexpr uint32_t SM_HEADS = SM_BIASB + 8192;                  // 221440: head weights, 4128 B
-constexpr uint32_t SM_PART = SM_HEADS + 4128;                   // 225568: 2 x 128 x float4 partials
-constexpr uint32_t SM_BARS = SM_PART + 4096;                    // mbarriers
-constexpr uint32_t SM_MISC = SM_BARS + 256;                     // 229920: tmem ptr, compositing carry
-constexpr uint32_t SM_TOTAL = SM_MISC + 128;                    // 230048
-constexpr uint32_t SM_ALLOC = 230400 > SM_TOTAL ? 230400 : SM_TOTAL;                           // >= SM_TOTAL and the pair kernel's P2_TOTAL; dynamic smem base is 1024-aligned (checked at run time)
-static_assert(SM_TOTAL <= SM_ALLOC, "shared-memory map exceeds the allocation");
-constexpr uint32_t TC_BIAS_CHUNK_BYTES = 256 * 32;              // [256 rows x K=16] fp16: column pair (2l, 2l+1) = (hi, lo) of layer l's bias
-
-// K columns of the resident bias operand used by bias layer `li` of `nb`: (hi, lo) pairs while 16 columns
-// suffice, hi only for the last 2*nb-16 layers.  Returns hi column; *lo = lo column or -1.
-__host__ __device__ inline int tc_bias_cols(int li, int nb, int* lo) {
-  const int n_single = (2 * nb > 16) ? 2 * nb - 16 : 0, n_pair = nb - n_single;
-  if (li < n_pair) { *lo = 2 * li + 1; return 2 * li; }
-  *lo = -1;
-  return 2 * n_pair + (li - n_pair);
-}
+// Kernels of the chain (march_wg_kernel, dgrad_wg_kernel): warpgroup 0 = producer (one thread issues the weight-ring bulk
+// copies), warpgroups 1 and 2 = MMA + epilogue, each on its own 64 rows of the 128-row tile.
+constexpr int TC_THREADS = 384;
+constexpr int TC_NST = 6;                 // weight ring stages (16 KB each)
+// shared-memory map (bytes, relative to a 1024-aligned base).  A warpgroup's A operand is its 64 rows of the tile as K-blocks
+// of 64 columns x 64 rows (8 KB, SWIZZLE_128B): byte for byte the warpgroup's half image of the tile record (train_common.cuh).
+constexpr uint32_t SM_ACT = 0;                                  // 2 x 32 KB  A operand (4 K-blocks x 8 KB), one per warpgroup
+constexpr uint32_t SM_ENC = 65536;                              // 2 x 16 KB  encoded inputs (1 K-block) | dgrad: the seed tile (2 K-blocks)
+constexpr uint32_t SM_WRING = 98304;                            // 6 x 16 KB  weight ring
+constexpr uint32_t SM_HEADS = SM_WRING + TC_NST * TC_STAGE_BYTES;   // 196608: head weights, 4128 B | dgrad: alpha_linear.weight
+constexpr uint32_t SM_BIAS = SM_HEADS + 4128;                   // 200736: fp32 biases [TC_MAXD + 1][256]
+constexpr uint32_t SM_RAW = SM_BIAS + (TC_MAXD + 1) * 1024;     // 209952: 128 x float4 raw rows of the tile
+constexpr uint32_t SM_BARS = SM_RAW + 2048;                     // 212000: mbarriers
+constexpr uint32_t SM_MISC = SM_BARS + 256;                     // 212256: compositing carry
+constexpr uint32_t SM_ALLOC = SM_MISC + 128;                    // 212384 (dynamic smem base is 1024-aligned: checked at run time)
+static_assert(SM_ALLOC <= 227 * 1024, "shared-memory map exceeds the per-block limit");
 
 // heads region (floats): viewdirs: alpha_w[256] rgb_w[3][128] alpha_b rgb_b[3]; else output_w[4][256] output_b[4]
 constexpr int HEADS_FLOATS = 1032;
@@ -58,10 +45,10 @@ constexpr int HEADS_FLOATS = 1032;
 struct PackLayout {
   int D, skip, use_viewdirs, IC, ICV, NL;
   int n_chunks;
-  size_t off_chunks, chunk_bytes, off_bias, off_heads, off_vdir, off_biasb, off_pair, total;
-  // backward (dgrad) stream: transposed weight chunks, linear image and its rank-split copy (bwd_tc2.cuh); 0 bytes when
-  // the net has no view head (the tensor-core backward serves use_viewdirs nets)
-  size_t off_bwd, bwd_bytes, off_bwd_pair;
+  size_t off_chunks, chunk_bytes, off_bias, off_heads, off_vdir, total;
+  // backward (dgrad) stream: transposed weight chunks (bwd_wg.cuh); 0 bytes when the net has no view head (the tensor-core
+  // backward serves use_viewdirs nets)
+  size_t off_bwd, bwd_bytes;
 };
 
 __host__ __device__ inline int tc_layer_chunks(int l, int D, int skip) {
@@ -70,8 +57,7 @@ __host__ __device__ inline int tc_layer_chunks(int l, int D, int skip) {
   return 8;
 }
 __host__ __device__ inline uint32_t tc_layer_chunk_bytes(int l, int D) { return (l == D + 1) ? TC_STAGE_BYTES / 2 : TC_STAGE_BYTES; }
-// every layer but the view layer (whose bias is per ray) starts with a bias chunk: one K=16 MMA of a
-// constant-one A slab against [bias_hi, bias_lo, 0...] initialises the accumulator with the bias
+// every layer but the view layer (whose bias is per ray) starts its accumulator at the fp32 bias
 __host__ __device__ inline bool tc_layer_has_bias(int l, int D) { return l != D + 1; }
 
 static inline PackLayout make_pack_layout(const NerfNetParams& n) {
@@ -88,13 +74,10 @@ static inline PackLayout make_pack_layout(const NerfNetParams& n) {
   L.off_bias = L.off_chunks + L.chunk_bytes;
   L.off_heads = L.off_bias + (size_t)(TC_MAXD + 1) * 1024;
   L.off_vdir = L.off_heads + HEADS_FLOATS * 4;
-  L.off_biasb = L.off_vdir + (size_t)(128 * (n.input_ch_views > 0 ? n.input_ch_views : 1) + 128) * 4;
-  L.off_biasb = (L.off_biasb + 255) & ~(size_t)255;
-  L.off_pair = L.off_biasb + TC_BIAS_CHUNK_BYTES;          // rank-split copy of the chunk stream for the CTA-pair kernel
-  L.off_bwd = L.off_pair + L.chunk_bytes;
+  L.off_bwd = L.off_vdir + (size_t)(128 * (n.input_ch_views > 0 ? n.input_ch_views : 1) + 128) * 4;
+  L.off_bwd = (L.off_bwd + 1023) & ~(size_t)1023;
   L.bwd_bytes = n.use_viewdirs ? (size_t)(4 + 8 * n.D) * TC_STAGE_BYTES : 0;
-  L.off_bwd_pair = L.off_bwd + L.bwd_bytes;
-  L.total = L.off_bwd_pair + L.bwd_bytes;
+  L.total = L.off_bwd + L.bwd_bytes;
   return L;
 }
 
@@ -124,32 +107,6 @@ __global__ void pack_chunks_kernel(PackJob job, uint8_t* __restrict__ dst) {
   // SWIZZLE_64B K-major: 8-row atoms of 512 B, 16B-chunk index ^= (row%8)>>1
   unsigned off = c.dst_off + (row >> 3) * 512 + (row & 7) * 64 + ((c16 ^ ((row & 7) >> 1)) << 4);
   *reinterpret_cast<uint4*>(dst + off) = o;
-}
-
-// resident bias operand: [256 rows x 16 K] fp16, K-major SWIZZLE_32B (rows of 32 B, 8-row atoms of 256 B)
-struct PackBiasJob { const float* src[TC_MAXD + 2]; int n; unsigned dst_off; };
-__global__ void pack_bias_kernel(PackBiasJob job, uint8_t* __restrict__ dst) {
-  const int row = threadIdx.x;                         // 256 threads = 256 output rows
-  __half h[16];
-#pragma unroll
-  for (int k = 0; k < 16; ++k) h[k] = __float2half_rn(0.0f);
-  for (int li = 0; li < job.n; ++li) {
-    const float b = job.src[li][row];
-    int lo;
-    const int hi = tc_bias_cols(li, job.n, &lo);
-    const __half bh = __float2half_rn(b);
-    h[hi] = bh;
-    if (lo >= 0) h[lo] = __float2half_rn(b - __half2float(bh));
-  }
-  uint8_t* base = dst + job.dst_off + (row >> 3) * 256 + (row & 7) * 32;
-  const int sw = ((row & 7) >> 2) & 1;                 // Swizzle<1,4,3>: 16-byte chunk index ^= bit 7 of the byte address
-  uint4 c[2];
-  for (int q = 0; q < 2; ++q) {
-    const unsigned short* u = reinterpret_cast<const unsigned short*>(h + 8 * q);
-    c[q] = make_uint4(u[0] | (u[1] << 16), u[2] | (u[3] << 16), u[4] | (u[5] << 16), u[6] | (u[7] << 16));
-  }
-  *reinterpret_cast<uint4*>(base + ((0 ^ sw) << 4)) = c[0];
-  *reinterpret_cast<uint4*>(base + ((1 ^ sw) << 4)) = c[1];
 }
 
 struct PackTables { NerfNetParams net; size_t off_bias, off_heads, off_vdir; };
@@ -296,13 +253,10 @@ struct MarchParams {
   const float* noise;                     // [N,S] or NULL
   const float* vb;                        // [N,128] view bias (use_viewdirs)
   long long N; int S; int rays_per_cta;
-  const uint8_t* chunks; const float* bias; const float* heads; const uint8_t* biasb;
+  const uint8_t* chunks; const float* bias; const float* heads;
   int D, skip, use_viewdirs, L, IC;
   int white_bkgd, do_composite;
   NerfPassOut out;
-  unsigned long long pair_half_bytes;     // pair kernel: bytes of one rank's half of the chunk stream
-  long long* trace;                       // debug: clock64 timestamps of CTA 0, super-tile 1 (or NULL)
-  int dbg;                                // debug: NERF_B200_DBG bit flags for A/B experiments (0 in production)
 };
 
 // compositing carry of the ray that is still open at a warp boundary (shared memory, 32 B)
@@ -326,53 +280,6 @@ __device__ __forceinline__ uint32_t ld_acquire_shared(uint32_t addr) {
 __device__ __forceinline__ void st_release_shared(uint32_t addr, uint32_t v) {
   asm volatile("st.release.cta.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
-// (a, b) += (c, d) as one packed FADD2
-__device__ __forceinline__ void add2(float& a, float& b, float c, float d) {
-  asm("{\n\t.reg .b64 ra, rb, rc;\n\tmov.b64 ra, {%0, %1};\n\tmov.b64 rb, {%2, %3};\n\tadd.rn.f32x2 rc, ra, rb;\n\tmov.b64 {%0, %1}, rc;\n\t}"
-      : "+f"(a), "+f"(b) : "f"(c), "f"(d));
-}
-
-// v[32] (fp32 accumulators of one row, bias already added) -> (ReLU) -> fp16 -> 4 x 16-byte stores
-// into the 128B-swizzled K-major A tile.
-template <bool RELU>
-__device__ __forceinline__ void store_act32(const float (&x)[32], uint32_t act_base, int r, int col0) {
-  const uint32_t kb = (uint32_t)(col0 >> 6) * 16384u;
-  const int c16_0 = (col0 & 63) >> 3;
-  const uint32_t row = act_base + kb + act_row_off(r);
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    uint32_t h0, h1, h2, h3;
-    if (RELU) {
-      h0 = ptx::cvt_relu_f16x2(x[g * 8 + 0], x[g * 8 + 1]); h1 = ptx::cvt_relu_f16x2(x[g * 8 + 2], x[g * 8 + 3]);
-      h2 = ptx::cvt_relu_f16x2(x[g * 8 + 4], x[g * 8 + 5]); h3 = ptx::cvt_relu_f16x2(x[g * 8 + 6], x[g * 8 + 7]);
-    } else {
-      h0 = ptx::cvt_f16x2(x[g * 8 + 0], x[g * 8 + 1]); h1 = ptx::cvt_f16x2(x[g * 8 + 2], x[g * 8 + 3]);
-      h2 = ptx::cvt_f16x2(x[g * 8 + 4], x[g * 8 + 5]); h3 = ptx::cvt_f16x2(x[g * 8 + 6], x[g * 8 + 7]);
-    }
-    ptx::st_shared_v4(row + (uint32_t)(((c16_0 + g) ^ (r & 7)) << 4), h0, h1, h2, h3);
-  }
-}
-
-// Same, with the 8 swizzled 16-byte-chunk addresses of this thread's row precomputed once
-// (sw[c] = tile base + row offset + ((c ^ (r & 7)) << 4)): every store is [register + immediate].
-template <bool RELU, int COL0>
-__device__ __forceinline__ void store_act32_pre(const float (&x)[32], const uint32_t (&sw)[8]) {
-  constexpr uint32_t kb = (uint32_t)(COL0 >> 6) * 16384u;
-  constexpr int c16_0 = (COL0 & 63) >> 3;
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    uint32_t h0, h1, h2, h3;
-    if (RELU) {
-      h0 = ptx::cvt_relu_f16x2(x[g * 8 + 0], x[g * 8 + 1]); h1 = ptx::cvt_relu_f16x2(x[g * 8 + 2], x[g * 8 + 3]);
-      h2 = ptx::cvt_relu_f16x2(x[g * 8 + 4], x[g * 8 + 5]); h3 = ptx::cvt_relu_f16x2(x[g * 8 + 6], x[g * 8 + 7]);
-    } else {
-      h0 = ptx::cvt_f16x2(x[g * 8 + 0], x[g * 8 + 1]); h1 = ptx::cvt_f16x2(x[g * 8 + 2], x[g * 8 + 3]);
-      h2 = ptx::cvt_f16x2(x[g * 8 + 4], x[g * 8 + 5]); h3 = ptx::cvt_f16x2(x[g * 8 + 6], x[g * 8 + 7]);
-    }
-    ptx::st_shared_v4(sw[c16_0 + g] + kb, h0, h1, h2, h3);
-  }
-}
-
 // segmented (per-ray) inclusive scans over one warp; `s` = lane of the segment start at or before
 // this lane inside the warp, or -1 when the segment began in an earlier warp.
 __device__ __forceinline__ float seg_scan_mul(float v, int lane, int s) {
@@ -386,25 +293,6 @@ __device__ __forceinline__ float seg_scan_add(float v, int lane, int s) {
   return v;
 }
 
-// One 32-column batch of a hidden-layer epilogue: the bias is already in the accumulator (bias chunk)
-__device__ __forceinline__ void as_float32(const uint32_t (&v)[32], float (&x)[32]) {
-#pragma unroll
-  for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
-}
-
-// Row `r` (0..7) of the 8-row bias-selector A atom for bias layer `li`: 1.0 in that layer's K columns.
-__device__ __forceinline__ void write_bias_selector(uint32_t slab, int r, int li, int nb) {
-  int lo;
-  const int hi = tc_bias_cols(li, nb, &lo);
-  uint32_t w[8] = {0, 0, 0, 0, 0, 0, 0, 0};            // 16 halves as 8 words
-  w[hi >> 1] |= (hi & 1) ? 0x3c000000u : 0x00003c00u;
-  if (lo >= 0) w[lo >> 1] |= (lo & 1) ? 0x3c000000u : 0x00003c00u;
-  const int sw = (r >> 2) & 1;
-  const uint32_t a = slab + (uint32_t)(r * 32);
-  ptx::st_shared_v4(a + ((0 ^ sw) << 4), w[0], w[1], w[2], w[3]);
-  ptx::st_shared_v4(a + ((1 ^ sw) << 4), w[4], w[5], w[6], w[7]);
-}
-
 // Positional encoding of one point into its 128-byte K-block row of the A operand (64 fp16 channels:
 // x y z, then per frequency sin(2^f xyz), cos(2^f xyz); channel 63 is zero padding), written as eight
 // 16-byte swizzled chunks.  run_nerf_helpers.py:36-45 evaluates sin/cos of 2^f x for every f; here only
@@ -412,8 +300,7 @@ __device__ __forceinline__ void write_bias_selector(uint32_t slab, int r, int li
 // sin 2a = 2 sin a cos a, cos 2a = (cos a - sin a)(cos a + sin a).  Four doublings amplify the fp32
 // rounding of the anchor to <= 1.6e-6 absolute (numpy model over [-6, 6]: 0.07 % of the fp16 operand
 // values move by one fp16 ulp), far below the fp16 quantisation of the operand itself, and cut the
-// sampler warp's work ~4x: with 30 sincosf per row it took longer than the MMAs of half a super-tile and
-// the issuers idled on enc_full (profiles/r01_summary.md, "sampler").
+// encoding work ~4x against 30 sincosf per row.
 __device__ __forceinline__ void encode_row_store(uint32_t row, int tr_, float px, float py, float pz, int L) {
   uint32_t h[32];
   float s[3], c[3];

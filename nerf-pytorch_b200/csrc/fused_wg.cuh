@@ -1,0 +1,343 @@
+// fused_wg.cuh -- the fused network pass on Hopper warpgroup MMA (wgmma): pts = o + d*z -> positional encoding ->
+// 8x256 MLP (+ heads) -> alpha compositing, run_nerf.py:381-386 / :397-403 (run_network :37-51, Embedder.embed
+// run_nerf_helpers.py:36-45, NeRF.forward :96-119, raw2outputs run_nerf.py:262-305).
+//
+// One CTA per SM walks its whole rays in 128-row tiles (the tile plan of train_common.cuh).  Warpgroup 0 is the producer: one
+// thread streams the packed weight chunks ([N = 256 x K = 32] fp16, 16 KB, SWIZZLE_64B K-major) through a ring of TC_NST
+// stages with cp.async.bulk.  Warpgroups 1 and 2 each own 64 rows of the tile: they encode their rows into the layer-0 A
+// operand, issue the layer's wgmma.m64n256k16 chain (A = their activation K-blocks, B = the ring stage; the accumulator
+// starts at the fp32 bias) and run the epilogue in registers -- ReLU, fp16, stored in place as the next layer's A operand,
+// the heads as fp32 FMA chains on the pre-rounding activations, the per-ray view bias in the view layer -- then composite
+// the tile's rows with segmented warp scans and a carry handed warp to warp.  A ring stage is released when both MMA
+// warpgroups' wgmma groups that read it have completed (every consumer thread arrives on the stage's empty barrier).
+//
+// Training mode (EMIT): each warpgroup's A operand is byte for byte its half of the tile image in the record, so after a layer's
+// epilogue one thread copies the 32 KB (encodings 8 KB, view layer 16 KB) to the record with cp.async.bulk shared -> global,
+// and waits for the copy to finish reading before the next epilogue overwrites the operand.  The sign bits of the
+// pre-activations go out as 8-byte stores (mask record, train_common.cuh).
+#pragma once
+#include "fused_tc.cuh"
+#include "train_common.cuh"
+
+namespace nb {
+
+// training-mode save buffers of one pass (train_common.cuh)
+struct TrainSaveDev { uint8_t* act; uint8_t* mask; int nst_plan; uint32_t rec_act, rec_mask; };
+
+// byte offset of (row r < 64, even column c) in a warpgroup's A operand: K-blocks of 64 columns x 64 rows, SWIZZLE_128B
+__device__ __forceinline__ uint32_t half_off(int r, int c) {
+  return (uint32_t)((c >> 6) * 8192 + (r >> 3) * 1024 + (r & 7) * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2);
+}
+
+// K-major operand descriptors: activations (SWIZZLE_128B, 8-row groups of 1 KB) and weight chunks (SWIZZLE_64B, 512 B)
+__device__ __forceinline__ uint64_t desc_act(uint32_t addr) { return ptx::gmma_desc(addr, 16, 1024, ptx::GMMA_SW128); }
+__device__ __forceinline__ uint64_t desc_w(uint32_t addr) { return ptx::gmma_desc(addr, 16, 512, ptx::GMMA_SW64); }
+
+// Weight ring shared by the producer and both MMA warpgroups: every party walks the same chunk sequence.
+struct Ring {
+  uint32_t full, empty, stage, phase;
+  __device__ __forceinline__ void advance() { if (++stage == TC_NST) { stage = 0; phase ^= 1; } }
+};
+
+// One K = 32 chunk into a 64 x N accumulator (two K = 16 instructions); `acc0` = 0 overwrites the accumulator
+template <int R>
+__device__ __forceinline__ void mma_chunk(float (&acc)[R], uint64_t ad, uint64_t bd, uint32_t acc0) {
+  if constexpr (R == 128) {
+    ptx::wgmma_m64n256k16<0, 0>(acc, ad, bd, acc0);
+    ptx::wgmma_m64n256k16<0, 0>(acc, ad + 2, bd + 2, 1u);
+  } else {
+    ptx::wgmma_m64n128k16<0, 0>(acc, ad, bd, acc0);
+    ptx::wgmma_m64n128k16<0, 0>(acc, ad + 2, bd + 2, 1u);
+  }
+}
+
+// All chunks of one layer: `a_of(c)` gives chunk c's A descriptor.  The previous chunk's stage is released as soon as the
+// wgmma group of the next one is in flight; on return the accumulator is complete.
+template <int R, typename AOf>
+__device__ __forceinline__ void mma_layer(float (&acc)[R], Ring& rg, uint32_t ring_base, int nch, bool from_zero, AOf a_of) {
+  ptx::wgmma_fence();
+  int pending = -1;
+  for (int c = 0; c < nch; ++c) {
+    const uint32_t s = rg.stage;
+    ptx::mbar_wait(rg.full + 8 * s, rg.phase);
+    mma_chunk(acc, a_of(c), desc_w(ring_base + s * TC_STAGE_BYTES), (from_zero && c == 0) ? 0u : 1u);
+    ptx::wgmma_commit();
+    if (pending >= 0) { ptx::wgmma_wait<1>(); ptx::mbar_arrive(rg.empty + 8 * pending); }
+    pending = (int)s;
+    rg.advance();
+  }
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(acc);
+  if (pending >= 0) ptx::mbar_arrive(rg.empty + 8 * pending);
+}
+
+// OR of a value over the four lanes that share an accumulator row
+__device__ __forceinline__ uint32_t quad_or(uint32_t v) {
+  v |= __shfl_xor_sync(0xffffffffu, v, 1);
+  return v | __shfl_xor_sync(0xffffffffu, v, 2);
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+template <bool EMIT>
+__global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchParams p, const TrainSaveDev sv) {
+  uint8_t* smem = tc_smem;
+  const uint32_t sb = ptx::smem_u32(smem);
+  if ((sb & 1023u) != 0) __trap();
+  float* s_heads = reinterpret_cast<float*>(smem + SM_HEADS);
+  float* s_bias = reinterpret_cast<float*>(smem + SM_BIAS);
+  const uint32_t a_heads = sb + SM_HEADS, a_carry = sb + SM_MISC;
+  const int D = p.D, NL = p.D + (p.use_viewdirs ? 2 : 0);
+
+  // this CTA's rays / rows; the number of super-tiles is the tile plan's (train_common.cuh: plan_cta_nst)
+  const long long ray0 = (long long)blockIdx.x * p.rays_per_cta;
+  const int nrows = plan_cta_rows(p.N, p.S, p.rays_per_cta, blockIdx.x);
+  const int nst = plan_cta_nst(p.N, p.S, p.rays_per_cta, blockIdx.x);
+  const long long row_begin = ray0 * p.S;
+
+  for (int i = threadIdx.x; i < HEADS_FLOATS; i += TC_THREADS) s_heads[i] = p.heads[i];
+  for (int i = threadIdx.x; i < (TC_MAXD + 1) * 256; i += TC_THREADS) s_bias[i] = p.bias[i];
+  Ring rg{sb + SM_BARS, sb + SM_BARS + 8 * TC_NST, 0, 0};
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < TC_NST; ++i) { ptx::mbar_init(rg.full + 8 * i, 1); ptx::mbar_init(rg.empty + 8 * i, 256); }
+    sts32(a_carry + CARRY_T, 1.0f); sts32(a_carry + CARRY_R, 0.f); sts32(a_carry + CARRY_G, 0.f); sts32(a_carry + CARRY_B, 0.f);
+    sts32(a_carry + CARRY_D, 0.f); sts32(a_carry + CARRY_A, 0.f); st_release_shared(a_carry + CARRY_TURN, 0u);
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (threadIdx.x < 128) {
+    // =========================== producer: the chunk stream, once per tile ===========================
+    ptx::setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      for (int tile = 0; tile < 2 * nst; ++tile) {
+        const uint8_t* src = p.chunks;
+        for (int l = 0; l < NL; ++l) {
+          const int nch = tc_layer_chunks(l, D, p.skip);
+          const uint32_t bytes = tc_layer_chunk_bytes(l, D);
+          for (int c = 0; c < nch; ++c) {
+            ptx::mbar_wait(rg.empty + 8 * rg.stage, rg.phase ^ 1);
+            ptx::mbar_arrive_expect_tx(rg.full + 8 * rg.stage, bytes);
+            ptx::bulk_g2s(sb + SM_WRING + rg.stage * TC_STAGE_BYTES, src, bytes, rg.full + 8 * rg.stage);
+            src += bytes;
+            rg.advance();
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // =========================== MMA warpgroups ===========================
+  ptx::setmaxnreg_inc<232>();
+  const int w = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
+  const int q4 = lane & 3;
+  const int r0 = 16 * wq + (lane >> 2), r1 = r0 + 8;              // this thread's two accumulator rows (of the warpgroup's 64)
+  const uint32_t act = sb + SM_ACT + (uint32_t)w * 32768u, enc = sb + SM_ENC + (uint32_t)w * 16384u;
+  const uint32_t ring = sb + SM_WRING;
+  const uint64_t l2_first = EMIT ? ptx::l2_policy_evict_first() : 0ull;
+  auto wg_sync = [&]() { ptx::named_bar_sync(1 + w, 128); };
+  // row-dependent parts of the swizzled addresses of this thread's pairs: column pair (8 j + 2 q4) of row r sits at
+  // rowoff(r) + (j >> 3) * 8192 + (((j & 7) ^ (r & 7)) << 4) + 4 q4
+  const uint32_t ro0 = (uint32_t)((r0 >> 3) * 1024 + (r0 & 7) * 128 + 4 * q4), ro1 = (uint32_t)((r1 >> 3) * 1024 + (r1 & 7) * 128 + 4 * q4);
+  auto pair_addr = [&](uint32_t base, uint32_t ro, int r, int j) { return base + ro + (uint32_t)(j >> 3) * 8192u + (uint32_t)(((j & 7) ^ (r & 7)) << 4); };
+
+  float acc[128];
+  for (int tile = 0; tile < 2 * nst; ++tile) {
+    const int st = tile >> 1, X = tile & 1;
+    uint8_t* const arec = EMIT ? sv.act + (size_t)((blockIdx.x * sv.nst_plan + st) * 2 + X) * sv.rec_act : nullptr;
+    uint8_t* const mrec = EMIT ? sv.mask + (size_t)((blockIdx.x * sv.nst_plan + st) * 2 + X) * sv.rec_mask : nullptr;
+    const int lrb = st * TC_ST + X * TC_TILE + 64 * w;            // row (inside the CTA's range) of the warpgroup's row 0
+    long long nray[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int lr = lrb + (h ? r1 : r0);
+      const int rl = (lr < nrows ? lr : nrows - 1) / p.S;
+      long long n = ray0 + rl;
+      nray[h] = n > p.N - 1 ? p.N - 1 : (n < 0 ? 0 : n);
+    }
+
+    // ---- sampler: pts = o + d z (run_nerf.py:381) and the positional encoding of the warpgroup's 64 rows ----
+    if (EMIT && t == 0) ptx::bulk_wait_read0();                  // the previous tile's copies have read the operands
+    wg_sync();
+    if (t < 64) {
+      const int lr = lrb + t;
+      float px = 0.f, py = 0.f, pz = 0.f;
+      if (lr < nrows) {
+        const long long m = row_begin + lr;
+        if (p.pts) { px = p.pts[m * 3]; py = p.pts[m * 3 + 1]; pz = p.pts[m * 3 + 2]; }
+        else {
+          const float* ry = p.rays + (ray0 + lr / p.S) * p.ray_stride;
+          const float z = p.z_vals[m];
+          px = __fadd_rn(ry[0], __fmul_rn(ry[3], z));
+          py = __fadd_rn(ry[1], __fmul_rn(ry[4], z));
+          pz = __fadd_rn(ry[2], __fmul_rn(ry[5], z));
+        }
+      }
+      encode_row_store(enc + act_row_off(t), t, px, py, pz, p.L);
+    }
+    ptx::fence_proxy_async_smem();
+    wg_sync();
+    if (EMIT && t == 0) { ptx::bulk_s2g_hint(arec + (uint32_t)w * 8192u, enc, 8192u, l2_first); ptx::bulk_commit(); }
+
+    float hp[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};   // head partial sums of this thread's columns, per row
+    for (int l = 0; l < NL; ++l) {
+      const int nch = tc_layer_chunks(l, D, p.skip);
+      const bool skip_layer = (l < D && p.skip >= 0 && l == p.skip + 1);
+      auto a_of = [&](int c) -> uint64_t {
+        if (l == 0 || (skip_layer && c < 2)) return desc_act(enc + (uint32_t)c * 64u);
+        const int k = skip_layer ? c - 2 : c;
+        return desc_act(act + (uint32_t)(k >> 1) * 8192u + (uint32_t)(k & 1) * 64u);
+      };
+      if (l <= D) {
+        // ---- pts_linears[l] (ReLU) or feature_linear (no activation): 64 x 256 ----
+        const float* bias = s_bias + 256 * l;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
+          acc[4 * j] = b.x; acc[4 * j + 1] = b.y; acc[4 * j + 2] = b.x; acc[4 * j + 3] = b.y;
+        }
+        mma_layer(acc, rg, ring, nch, false, a_of);
+        if (EMIT && t == 0) ptx::bulk_wait_read0();
+        wg_sync();                                                // the whole warpgroup's MMAs and copies are done with the operand
+        const bool last_pts = (l == D - 1);
+        if (EMIT && l < D) {
+          uint32_t m0[8], m1[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) { m0[i] = 0u; m1[i] = 0u; }
+#pragma unroll
+          for (int j = 0; j < 32; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int bit = 31 - (8 * (j & 3) + 2 * q4 + e);
+              m0[j >> 2] |= (__float_as_uint(acc[4 * j + e]) >> 31) << bit;
+              m1[j >> 2] |= (__float_as_uint(acc[4 * j + 2 + e]) >> 31) << bit;
+            }
+          uint2 v0 = make_uint2(0u, 0u), v1 = make_uint2(0u, 0u);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            m0[i] = quad_or(m0[i]); m1[i] = quad_or(m1[i]);
+          }
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (q4 == k) { v0 = make_uint2(m0[2 * k], m0[2 * k + 1]); v1 = make_uint2(m1[2 * k], m1[2 * k + 1]); }
+          const uint32_t mo = (uint32_t)l * 4096u + (uint32_t)(q4 >> 1) * 2048u + (uint32_t)(q4 & 1) * 8u;
+          *reinterpret_cast<uint2*>(mrec + mo + (uint32_t)(64 * w + r0) * 16u) = v0;
+          *reinterpret_cast<uint2*>(mrec + mo + (uint32_t)(64 * w + r1) * 16u) = v1;
+        }
+        if (last_pts) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const int c = 8 * j + 2 * q4;
+            const float a0 = fmaxf(acc[4 * j], 0.f), a1 = fmaxf(acc[4 * j + 1], 0.f), b0 = fmaxf(acc[4 * j + 2], 0.f), b1 = fmaxf(acc[4 * j + 3], 0.f);
+            if (p.use_viewdirs) {                                 // alpha_linear (run_nerf_helpers.py:106)
+              const float2 wa = *reinterpret_cast<const float2*>(s_heads + c);
+              hp[0][3] = fmaf(a1, wa.y, fmaf(a0, wa.x, hp[0][3]));
+              hp[1][3] = fmaf(b1, wa.y, fmaf(b0, wa.x, hp[1][3]));
+            } else {                                              // output_linear (:117)
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const float2 wk = *reinterpret_cast<const float2*>(s_heads + 256 * k + c);
+                hp[0][k] = fmaf(a1, wk.y, fmaf(a0, wk.x, hp[0][k]));
+                hp[1][k] = fmaf(b1, wk.y, fmaf(b0, wk.x, hp[1][k]));
+              }
+            }
+          }
+        }
+        if (!(last_pts && !p.use_viewdirs)) {
+          const bool relu = l < D;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const uint32_t h0 = relu ? ptx::cvt_relu_f16x2(acc[4 * j], acc[4 * j + 1]) : ptx::cvt_f16x2(acc[4 * j], acc[4 * j + 1]);
+            const uint32_t h1 = relu ? ptx::cvt_relu_f16x2(acc[4 * j + 2], acc[4 * j + 3]) : ptx::cvt_f16x2(acc[4 * j + 2], acc[4 * j + 3]);
+            ptx::st_shared_b32(pair_addr(act, ro0, r0, j), h0);
+            ptx::st_shared_b32(pair_addr(act, ro1, r1, j), h1);
+          }
+          ptx::fence_proxy_async_smem();
+          wg_sync();
+          if (EMIT && l < D && t == 0) {
+            ptx::bulk_s2g_hint(arec + rec_act_h(l) + (uint32_t)w * 32768u, act, 32768u, l2_first);
+            ptx::bulk_commit();
+          }
+        }
+      } else {
+        // ---- views_linears[0] (N = 128) + per-ray view bias, ReLU, rgb_linear ----
+        float* accv = acc;                                        // the first 64 accumulators
+        mma_layer(*reinterpret_cast<float(*)[64]>(accv), rg, ring, nch, true, a_of);
+        wg_sync();
+        const float* vb0 = p.vb + nray[0] * 128;
+        const float* vb1 = p.vb + nray[1] * 128;
+        uint32_t m0[4] = {0u, 0u, 0u, 0u}, m1[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int c = 8 * j + 2 * q4;
+          const float2 b0 = *reinterpret_cast<const float2*>(vb0 + c), b1 = *reinterpret_cast<const float2*>(vb1 + c);
+          const float x0 = acc[4 * j] + b0.x, x1 = acc[4 * j + 1] + b0.y, y0 = acc[4 * j + 2] + b1.x, y1 = acc[4 * j + 3] + b1.y;
+          if (EMIT) {
+            const int bit = 31 - (8 * (j & 3) + 2 * q4);
+            m0[j >> 2] |= ((__float_as_uint(x0) >> 31) << bit) | ((__float_as_uint(x1) >> 31) << (bit - 1));
+            m1[j >> 2] |= ((__float_as_uint(y0) >> 31) << bit) | ((__float_as_uint(y1) >> 31) << (bit - 1));
+            ptx::st_shared_b32(pair_addr(act, ro0, r0, j), ptx::cvt_relu_f16x2(x0, x1));
+            ptx::st_shared_b32(pair_addr(act, ro1, r1, j), ptx::cvt_relu_f16x2(y0, y1));
+          }
+          const float h00 = fmaxf(x0, 0.f), h01 = fmaxf(x1, 0.f), h10 = fmaxf(y0, 0.f), h11 = fmaxf(y1, 0.f);
+#pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            const float2 wk = *reinterpret_cast<const float2*>(s_heads + 256 + 128 * k + c);
+            hp[0][k] = fmaf(h01, wk.y, fmaf(h00, wk.x, hp[0][k]));
+            hp[1][k] = fmaf(h11, wk.y, fmaf(h10, wk.x, hp[1][k]));
+          }
+        }
+        if (EMIT) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) { m0[i] = quad_or(m0[i]); m1[i] = quad_or(m1[i]); }
+          uint32_t v0 = 0u, v1 = 0u;
+#pragma unroll
+          for (int k = 0; k < 4; ++k) if (q4 == k) { v0 = m0[k]; v1 = m1[k]; }
+          const uint32_t mo = (uint32_t)D * 4096u + (uint32_t)(q4 >> 1) * 1024u + (uint32_t)(q4 & 1) * 4u;
+          *reinterpret_cast<uint32_t*>(mrec + mo + (uint32_t)(64 * w + r0) * 8u) = v0;
+          *reinterpret_cast<uint32_t*>(mrec + mo + (uint32_t)(64 * w + r1) * 8u) = v1;
+          ptx::fence_proxy_async_smem();
+          wg_sync();
+          if (t == 0) {
+            ptx::bulk_s2g_hint(arec + rec_act_hv(D) + (uint32_t)w * 16384u, act, 16384u, l2_first);
+            ptx::bulk_commit();
+          }
+        }
+      }
+    }
+
+    // ---- heads: full row sums over the quad -> raw rows of the tile -> compositing ----
+    float raw[2][4];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) raw[h][k] = quad_sum(hp[h][k]);
+    const uint32_t a_raw = sb + SM_RAW + (uint32_t)(64 * w) * 16u;
+    if (q4 == 0) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float4 o;
+        if (p.use_viewdirs) o = make_float4(raw[h][0] + s_heads[641], raw[h][1] + s_heads[642], raw[h][2] + s_heads[643], raw[h][3] + s_heads[640]);
+        else o = make_float4(raw[h][0] + s_heads[1024], raw[h][1] + s_heads[1025], raw[h][2] + s_heads[1026], raw[h][3] + s_heads[1027]);
+        sts128(a_raw + (uint32_t)(h ? r1 : r0) * 16u, o);
+      }
+    }
+    wg_sync();
+    if (wq < 2) {
+      const int tr = 32 * wq + lane;                              // row of the warpgroup
+      const int lr = lrb + tr;
+      const bool valid = lr < nrows;
+      const int rl = (valid ? lr : nrows - 1) / p.S;
+      long long n_ray = ray0 + rl;
+      if (n_ray > p.N - 1) n_ray = p.N - 1;
+      if (n_ray < 0) n_ray = 0;
+      composite_rows(p, lds128(a_raw + (uint32_t)tr * 16u), valid, lr, rl, n_ray, row_begin, st, X, 2 * w + wq, lane, a_carry);
+    }
+  }
+  if (EMIT && t == 0) ptx::bulk_wait_all();
+}
+
+}  // namespace nb

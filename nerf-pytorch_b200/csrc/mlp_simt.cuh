@@ -1,6 +1,6 @@
 // mlp_simt.cuh -- exact-mode (fp32 CUDA-core) run_network: encode + NeRF.forward -> raw.
 // Mirrors run_nerf.py:37-51 and run_nerf_helpers.py:96-119 with fp32 FMA accumulation.  It is the
-// validation / "exact" path (NERF_B200_PREC_FP32); the production path is fused_tc.cuh.
+// validation / "exact" path (NERF_B200_PREC_FP32); the production path is fused_wg.cuh.
 #pragma once
 #include "common.cuh"
 #include "bwd_simt.cuh"

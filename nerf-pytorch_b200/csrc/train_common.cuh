@@ -1,5 +1,5 @@
-// train_common.cuh -- data layout shared by the training-mode forward (march_tc2_kernel<EMIT>) and the tensor-core
-// backward (bwd_tc2.cuh): the tile plan, the per-tile activation / mask / gradient records and the mask bit order.
+// train_common.cuh -- data layout shared by the training-mode forward (march_wg_kernel<EMIT>, fused_wg.cuh) and the
+// tensor-core backward (bwd_wg.cuh): the tile plan, the per-tile activation / mask / gradient records and the mask bit order.
 //
 // The forward walks each CTA's rows in 128-row tiles (two per 256-row super-tile).  In training mode it leaves, per
 // tile, a record of fp16 "tile images" -- [128 rows x C columns] in the shared-memory operand layout (K-blocks of 64
@@ -7,10 +7,9 @@
 // that bulk copies make a tile MMA-ready again, as a K-major A operand (dgrad) or as an MN-major operand (wgrad:
 // dW = dA^T H reduces over the sample rows).  In global memory an image is stored as TWO HALF IMAGES of 64 rows:
 //   [half h = r >> 6][K-block kb = col >> 6][64 rows x 128 B = 8 KB]
-// i.e. the 8 KB pieces of a K-block's upper and lower 64 rows are not adjacent (as they are in shared memory), the K-blocks of
-// one 64-row half are: the weight gradient streams 64-row half tiles, and reads each operand as ONE contiguous C/64 x 8 KB
-// piece instead of C/64 pieces 16 KB apart (HBM reads of scattered 8 KB pieces reach 4.1 TB/s, of 32 KB pieces 6.5: measured,
-// profiles/r02_dram_stream_probe.jsonl).  A warp of the forward / dgrad epilogue owns 32 rows = a 4 KB slice of either layout.
+// i.e. the K-blocks of one 64-row half are adjacent: the weight gradient streams 64-row half tiles and reads each operand as ONE
+// contiguous C/64 x 8 KB piece, and a half image is byte for byte the A operand of the MMA warpgroup that owns those 64 rows in
+// the forward / dgrad kernels (one bulk copy per layer).
 //
 //   activation record (forward -> backward), rec_act_bytes(D):
 //     [0, 16 KB)                       enc    : gamma(p), 64 columns (63 + zero pad)
@@ -30,25 +29,15 @@
 
 namespace nb {
 
-// Runtime switches of the record / weight-gradient experiments (NERF_B200_DBG_* environment variables: kernel variants without the
-// record copies, without the spare-warp sums, per-job finish times, per-warp wait cycles).  Compiled out of the product build;
-// `NERF_B200_EXPERIMENTS=1 python -c "import __graft_entry__ as g; g.build(force=True)"` builds them in.  The numbers under
-// profiles/r02_*_experiments* come from such a build.
-#ifdef NERF_B200_EXPERIMENTS
-constexpr bool kExp = true;
-#else
-constexpr bool kExp = false;
-#endif
-
 struct TilePlan {
   long long N; int S;
-  int grid;            // CTAs of the forward launch (even: whole CTA pairs)
+  int grid;            // CTAs of the forward launch (each owns at least one ray)
   int rays_per_cta;    // whole rays per CTA
   int nst;             // super-tiles (256 rows) per CTA: the record stride; a CTA may run fewer
   long long n_tiles;   // grid * nst * 2
 };
 
-// The forward's work split (launch_march): whole rays per CTA, balanced over the SMs, CTA pairs.
+// The forward's work split (launch_march): whole rays per CTA, balanced over the SMs.
 static inline TilePlan make_tile_plan(long long N, int S, int sms) {
   TilePlan t;
   t.N = N; t.S = S;
@@ -59,7 +48,7 @@ static inline TilePlan make_tile_plan(long long N, int S, int sms) {
   if (grid < 1) grid = 1;
   t.rays_per_cta = (int)((N + grid - 1) / grid);
   grid = (int)((N + t.rays_per_cta - 1) / t.rays_per_cta);
-  t.grid = (grid + 1) & ~1;
+  t.grid = grid;
   t.nst = (int)(((long long)t.rays_per_cta * S + 255) / 256);
   t.n_tiles = (long long)t.grid * t.nst * 2;
   return t;
@@ -77,20 +66,15 @@ __host__ __device__ __forceinline__ uint32_t rec_grad_dA(int l, int D) { return 
 __host__ __device__ __forceinline__ uint32_t img_off(int r, int col, int C) {
   return (uint32_t)((r >> 6) * (C >> 6) * 8192 + (col >> 6) * 8192 + ((r & 63) >> 3) * 1024 + (r & 7) * 128 + ((((col & 63) >> 3) ^ (r & 7)) << 4) + (col & 7) * 2);
 }
-// byte offset of the 4 KB slice (rows 32 q .. 32 q + 31) of K-block kb inside a [128 x C] tile image in global memory
-__host__ __device__ __forceinline__ uint32_t img_slice_off(int q, int kb, int C) {
-  return (uint32_t)((q >> 1) * (C >> 6) * 8192 + kb * 8192 + (q & 1) * 4096);
-}
 
-// rows of CTA `cta` and the super-tiles its PAIR runs (both CTAs of a pair run the same number)
+// rows of CTA `cta` and the super-tiles it runs
 __host__ __device__ __forceinline__ int plan_cta_rows(long long N, int S, int rays_per_cta, int cta) {
   const long long r0 = (long long)cta * rays_per_cta;
   const long long r1 = (r0 + rays_per_cta < N) ? r0 + rays_per_cta : N;
   return (r1 > r0) ? (int)(r1 - r0) * S : 0;
 }
 __host__ __device__ __forceinline__ int plan_cta_nst(long long N, int S, int rays_per_cta, int cta) {
-  const int a = plan_cta_rows(N, S, rays_per_cta, cta), b = plan_cta_rows(N, S, rays_per_cta, cta ^ 1);
-  return ((a > b ? a : b) + 255) / 256;
+  return (plan_cta_rows(N, S, rays_per_cta, cta) + 255) / 256;
 }
 
 // ---- mask bits ------------------------------------------------------------------------------------------------

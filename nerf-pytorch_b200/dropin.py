@@ -1,4 +1,4 @@
-"""Drop the B200 path into the UNMODIFIED reference script.
+"""Drop the H100 path into the UNMODIFIED reference script.
 
 `run_nerf.train()` resolves `create_nerf`, `render`, `render_path` (-> `render`) and, through them,
 `batchify_rays`, `render_rays`, `raw2outputs`, `sample_pdf`, `NeRF`, `get_embedder` as module

@@ -183,7 +183,7 @@ class FusedTrainStep:
             if fine:
                 check(lib.nerf_b200_mse_seed(api._ptr(o["rgb"]), api._ptr(self.target), N, gscale, api._ptr(o["g_rgb"]), api._ptr(self.state), st), "mse_seed")
             check(lib.nerf_b200_mse_seed(api._ptr(o["rgb0"]), api._ptr(self.target), N, gscale, api._ptr(o["g_rgb0"]), api._ptr(self.state), st), "mse_seed")
-            # backward of both passes into the flat gradient buffer (one call: the passes are scheduled side by side)
+            # backward of both passes into the flat gradient buffer (one call)
             check(lib.nerf_b200_render_rays_bwd_tc(api._ptr(self.packed_rays), N, C.byref(cfg), C.byref(self._bp_c),
                                                    C.byref(self._bp_f) if fine else None, api._ptr(self._bws), self._bws.numel(), st), "render_rays_bwd_tc")
 

@@ -1,6 +1,6 @@
 """Quantisation-aware restatement of the tensor-core path  --  TEST INFRASTRUCTURE ONLY.
 
-The fp16-operand / fp32-accumulate forward (csrc/fused_tc2.cuh) and the loss-scaled fp16 backward (csrc/bwd_tc2.cuh)
+The fp16-operand / fp32-accumulate forward (csrc/fused_wg.cuh) and the loss-scaled fp16 backward (csrc/bwd_wg.cuh)
 restated with stock torch ops on the CPU: every tensor the kernels round to fp16 is rounded here at the same place,
 sums are taken in float64 (the kernels accumulate in fp32; the difference is O(1e-7)).  It is the oracle for the
 tensor-core GRADIENTS: the reference's own fp32 autograd (tests/golden/lego_grads.npz) differs from any 10-bit-mantissa
@@ -76,7 +76,7 @@ def composite_adjoint(raw: torch.Tensor, z: torch.Tensor, rays_d: torch.Tensor, 
 
 def backward(sd: dict, acts: dict, masks: dict, d_raw: torch.Tensor, scale: float, ray_of_row: torch.Tensor, n_rays: int,
              D: int = 8, skip: int = 4, ic: int = 63):
-    """The backward of csrc/bwd_tc2.cuh given the forward's saved tensors.
+    """The backward of csrc/bwd_wg.cuh given the forward's saved tensors.
 
     acts: enc16, h16[l], feat16, hv16, encv (per row);  masks: 'h'[l] [M,256] bool (pre-activation > 0), 'hv' [M,128];
     d_raw [M,4] fp64 (unscaled).  Returns (grads by state_dict key, stages) where stages holds the loss-scaled fp16
@@ -105,7 +105,7 @@ def backward(sd: dict, acts: dict, masks: dict, d_raw: torch.Tensor, scale: floa
     g["alpha_linear.weight"] = d_sig.t() @ acts["h16"][D - 1]
     g["alpha_linear.bias"] = d_sig.sum(0)
     gv = torch.zeros_like(sd["views_linears.0.weight"])
-    # feature_linear's output is not recorded: d_hv^T feat = (d_hv^T h_{D-1}) W_feat^T + (sum_rows d_hv) b_feat^T  (csrc/bwd_tc2.cuh)
+    # feature_linear's output is not recorded: d_hv^T feat = (d_hv^T h_{D-1}) W_feat^T + (sum_rows d_hv) b_feat^T  (csrc/bwd_wg.cuh)
     gv[:, :256] = (d_hv16.t() @ acts["h16"][D - 1] * inv) @ sd["feature_linear.weight"].t() + torch.outer(d_hv16.sum(0) * inv, sd["feature_linear.bias"])
     dsum = torch.zeros((n_rays, 128), dtype=torch.float64).index_add_(0, ray_of_row, d_hv16 * inv)
     encv_ray = torch.zeros((n_rays, acts["encv"].shape[1]), dtype=torch.float64)

@@ -1,4 +1,4 @@
-"""The UNMODIFIED reference (baseline/_ref, tools/fetch_reference.py) on cuda:0, for the -m gpu tests: its own create_nerf /
+"""The UNMODIFIED reference (oracle/_ref, oracle/fetch_reference.py) on cuda:0, for the -m gpu tests: its own create_nerf /
 render with given weights, fp32 or TF32 matmuls (TF32 is the default of the reference's pinned torch 1.11)."""
 import argparse
 import importlib.util
@@ -11,7 +11,7 @@ import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def available():

@@ -35,10 +35,8 @@ class Plan:
         return np.where(lr < nrows, r0 * self.S + lr, -1)
 
     def cta_nst(self, cta):
-        def rows(c):
-            r0 = c * self.rays_per_cta
-            return max(min(r0 + self.rays_per_cta, self.N) - r0, 0) * self.S
-        return (max(rows(cta), rows(cta ^ 1)) + 255) // 256
+        r0 = cta * self.rays_per_cta
+        return (max(min(r0 + self.rays_per_cta, self.N) - r0, 0) * self.S + 255) // 256
 
     def valid_tiles(self):
         return [t for t in range(self.n_tiles) if (t // 2) % self.nst < self.cta_nst(t // (2 * self.nst))]

@@ -1,4 +1,4 @@
-"""The drop-in, EXECUTED: the unmodified reference script (baseline/_ref/run_nerf.py, copied there by tools/fetch_reference.py)
+"""The drop-in, EXECUTED: the unmodified reference script (oracle/_ref/run_nerf.py, copied there by oracle/fetch_reference.py)
 is imported twice, once as it is and once with `nerf_pytorch_b200.dropin.patch` applied, and its own `train()` runs on
 a small synthetic blender-format dataset written to a temp directory -- argument parsing, data loading, ray batching,
 `create_nerf` (run_nerf.py:640), `render(..., retraw=True)` (:760), the two MSE terms, `loss.backward()`,
@@ -23,7 +23,7 @@ import torch
 from conftest import ROOT, rel_l2
 
 pytestmark = pytest.mark.gpu
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 K_ITERS = 6
 
 
@@ -120,7 +120,7 @@ def _run_train(mod, argv, init_from=None):
     return captured["out"], captured["init"], [float(v) for v in losses]
 
 
-@pytest.mark.skipif(not os.path.isfile(os.path.join(REF, "run_nerf.py")), reason="baseline/_ref missing (run tools/fetch_reference.py where /root/reference exists)")
+@pytest.mark.skipif(not os.path.isfile(os.path.join(REF, "run_nerf.py")), reason="oracle/_ref missing (built by __graft_entry__.build() where the reference checkout exists)")
 def test_reference_train_runs_unchanged_through_the_dropin(tmp_path):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import dropin

@@ -1,7 +1,7 @@
 """Discriminating parity: fixtures WITH STRUCTURE (oracle/gen_trained.py: networks trained by the unmodified reference for
 a few hundred CPU steps on an analytic scene, so acc spans 0..1 and the weights are peaked) at 1024 rays, BASELINE config 3's
 shape (4096 fern NDC rays), the fused path's `weights` (coarse and fine) and sorted z, and the gradients on the trained
-networks.  Every measured deviation is written to gpurun_out/parity_r02.json (committed as profiles/parity_r02.json)."""
+networks.  Every measured deviation is also written to parity_r02.json in the git-ignored output directory."""
 import ctypes as C
 import json
 import os
@@ -100,7 +100,7 @@ def test_trained_networks_1024_rays_outputs_weights_and_z(G, prec):
 
 
 def _check_trained_gates(st, prec):
-    """Gates on networks WITH structure (measured values: profiles/parity_r02.json).
+    """Gates on networks WITH structure (the measured values go to parity_r02.json).
 
     fp32 (exact mode): the coarse pass agrees to fp32 round-off (<= 2e-5); the fine pass additionally sees the resampling's
     sensitivity -- a 1e-7 difference in a coarse weight can move an inverse-CDF sample across a bin knot (SURVEY App. D quirk 5),
@@ -183,7 +183,7 @@ def test_reference_tf32_deviates_as_much(G):
     that fp32 run -- on the trained networks, 1024 lego rays."""
     import ref_gpu
     if not ref_gpu.available():
-        pytest.skip("baseline/_ref missing")
+        pytest.skip("oracle/_ref missing (built where the reference checkout exists)")
     fx = load_golden("trained_lego_1024")
     sb = G.synth.ray_batch("lego", int(fx["N"]), seed=int(fx["ray_seed"]))
     w = load_golden("trained_weights")

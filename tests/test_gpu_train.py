@@ -1,7 +1,7 @@
-"""Training-mode forward records and the tensor-core backward (csrc/fused_tc2.cuh EMIT, csrc/bwd_tc2.cuh) through the
+"""Training-mode forward records and the tensor-core backward (csrc/fused_wg.cuh EMIT, csrc/bwd_wg.cuh) through the
 C ABI, stage by stage against the quantisation-aware restatement (oracle/tc_emul.py) and end to end against the exact
-mode and the reference's autograd (tests/golden/lego_grads.npz).  Measured deviations are appended to
-gpurun_out/parity_train.json (copied to profiles/ by the builder)."""
+mode and the reference's autograd (tests/golden/lego_grads.npz).  Measured deviations are appended to parity_train.json
+in the git-ignored output directory."""
 import ctypes as C
 import json
 import os
@@ -276,7 +276,7 @@ def test_tensor_core_gradients_end_to_end(G, fixture):
 
 
 def test_full_batch_tensor_core_gradients_are_stable_and_match_exact(G):
-    """BASELINE config 2 at full size (4096 rays x 64+128: every CTA walks many super-tiles, all 148 SMs stream records
+    """BASELINE config 2 at full size (4096 rays x 64+128: every CTA walks many super-tiles, every SM streams records
     concurrently) -- the sizes at which an ordering bug in the record copies would show: three evaluations of render() +
     loss.backward() on the tensor-core path agree with each other (atomics reorder sums: 1e-4) and with the exact fp32
     backward of the same library within the fp16 budget of the end-to-end test."""

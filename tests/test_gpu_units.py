@@ -17,9 +17,9 @@ def G():
 
 
 @pytest.mark.parametrize("K,N", [(32, 256), (64, 256), (256, 256), (256, 128), (128, 128)])
-def test_tcgen05_selftest_gemm(G, K, N):
-    """Operand layouts (128B-swizzled A written by threads, 64B-swizzled weight chunks via bulk copy),
-    UMMA descriptors and TMEM loads: D = fp16(A) fp16(W)^T with fp32 accumulation."""
+def test_wgmma_selftest_gemm(G, K, N):
+    """Operand layouts (128B-swizzled A written by threads, 64B-swizzled weight chunks via bulk copy) and
+    wgmma descriptors: D = fp16(A) fp16(W)^T with fp32 accumulation."""
     lib = G._lib.load_dev()
     rng = np.random.default_rng(K * 1000 + N)
     A = rng.standard_normal((128, K)).astype(np.float32)
@@ -34,7 +34,7 @@ def test_tcgen05_selftest_gemm(G, K, N):
     assert err < 2e-3, err          # only fp32 accumulation order differs
 
 
-def test_tcgen05_selftest_gemm_tn(G):
+def test_wgmma_selftest_gemm_tn(G):
     """MN-major operands straight from the activation layout (the weight-gradient GEMM's access pattern):
     out[256,256] = fp16(X)^T fp16(Y) over 128 sample rows, LBO = K-block stride, SBO = 8-row group stride."""
     lib = G._lib.load_dev()

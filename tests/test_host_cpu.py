@@ -11,6 +11,8 @@ import numpy as np
 import pytest
 import torch
 
+from conftest import load_golden
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -138,22 +140,26 @@ def test_cached_parameter_list_follows_the_module(nb):
 
 
 def test_keras_weight_import_matches_the_reference(nb):
-    """NeRF.load_weights_from_keras vs the reference's own (run_nerf_helpers.py:121-148) on a synthetic Keras-style weight list;
-    needs /root/reference (build container), otherwise checks the documented layout only."""
-    rng = np.random.default_rng(0)
-    shapes = [(63, 256)] + [(256, 256)] * 4 + [(319, 256)] + [(256, 256)] * 2 + [(256, 256), (283, 128), (128, 3), (256, 1)]
-    weights = []
-    for (i, o) in shapes:
-        weights += [rng.standard_normal((i, o)).astype(np.float32), rng.standard_normal((o,)).astype(np.float32)]
+    """NeRF.load_weights_from_keras vs the reference's own (run_nerf_helpers.py:121-148) on a seeded synthetic Keras-style weight
+    list: the keys, shapes and a seeded sample of every tensor the reference produced (tests/golden/keras_import.npz,
+    oracle/gen_keras_golden.py).  Where the reference checkout exists, the whole state_dict is compared as well."""
+    from oracle import gen_keras_golden as K
+    from oracle import ref_import
+    weights = K.keras_weights()
     m = nb.NeRF(D=8, W=256, input_ch=63, input_ch_views=27, output_ch=5, skips=[4], use_viewdirs=True)
     m.load_weights_from_keras(weights)
     assert torch.equal(m.pts_linears[5].weight, torch.from_numpy(weights[10].T)) and torch.equal(m.alpha_linear.bias, torch.from_numpy(weights[23]))
-    from oracle import ref_import
+    fx = load_golden("keras_import")
+    sd = m.state_dict()
+    assert list(sd.keys()) == [str(k) for k in fx["keys"]]
+    for k, t in enumerate(sd.values()):
+        assert tuple(t.shape) == tuple(fx[f"shape_{k}"]), k
+        np.testing.assert_array_equal(t.detach().numpy().reshape(-1)[fx[f"idx_{k}"]], fx[f"val_{k}"])
     if ref_import.available():
         _, rh = ref_import.load()
         r = rh.NeRF(D=8, W=256, input_ch=63, input_ch_views=27, output_ch=5, skips=[4], use_viewdirs=True)
         r.load_weights_from_keras(weights)
-        for (ka, a), (kb, b) in zip(m.state_dict().items(), r.state_dict().items()):
+        for (ka, a), (kb, b) in zip(sd.items(), r.state_dict().items()):
             assert ka == kb and torch.equal(a, b), ka
 
 
@@ -186,12 +192,11 @@ def _cuobjdump(*args):
     return subprocess.run([exe, *args, _lib.LIB_PATH], capture_output=True, text=True, timeout=600).stdout
 
 
-def test_built_kernels_use_blackwell_tensor_and_tma_instructions(nb):
-    """Static evidence in the cross-compiled sm_100a SASS (no GPU needed): the fused forward (inference and training
-    instantiations) and the dgrad chain issue cta_group::2 tcgen05.mma, load weights with tensor-map TMA, read
-    accumulators with tcgen05.ld and commit through multicast mbarrier arrives; the training-mode forward and the dgrad
-    chain copy their tiles out with bulk stores (the inference instantiation has none); the weight-gradient kernel issues
-    tcgen05.mma on bulk-loaded tiles.
+def test_built_kernels_use_hopper_tensor_and_tma_instructions(nb):
+    """Static evidence in the cross-compiled sm_90a SASS (no GPU needed): the fused forward (inference and training
+    instantiations), the dgrad chain and the weight gradient issue warpgroup MMAs (HGMMA) on operands that the TMA engine
+    bulk-loads into shared memory behind mbarrier waits, and hand registers from the producer to the MMA warpgroups; the
+    training-mode forward and the dgrad chain copy their tiles out with bulk stores (the inference instantiation has none).
     Guards against a silent regression to mma.sync / plain loads."""
     sass = _cuobjdump("-sass")
     funcs = {}
@@ -206,30 +211,46 @@ def test_built_kernels_use_blackwell_tensor_and_tma_instructions(nb):
         names = [k for k in funcs if sub in k]
         assert len(names) == 1, (sub, names)
         return "\n".join(funcs[names[0]])
-    infer, train, dgrad, wgrad = body("march_tc2_kernelILb0"), body("march_tc2_kernelILb1"), body("dgrad_tc2_kernel"), body("wgrad_tc_kernel")
-    for mnem in ("UTCHMMA.2CTA", "UTMALDG.2D.2CTA", "LDTM.x32", "UTCBAR.2CTA.MULTICAST", "SYNCS.PHASECHK.TRANS64.TRYWAIT", "ELECT", "F2FP.RELU"):
+    infer, train, dgrad, wgrad = body("march_wg_kernelILb0"), body("march_wg_kernelILb1"), body("dgrad_wg_kernel"), body("wgrad_wg_kernel")
+    common = ("UBLKCP.S.G", "SYNCS.PHASECHK.TRANS64.TRYWAIT", "USETMAXREG")
+    for mnem in common + ("HGMMA.64x256x16.F32", "HGMMA.64x128x16.F32", "F2FP.RELU"):
         assert mnem in infer and mnem in train, mnem
-    for mnem in ("UTCHMMA.2CTA", "UTMALDG.2D.2CTA", "LDTM.x32", "UTCBAR.2CTA.MULTICAST", "ELECT", "F2FP.SATFINITE", "UBLKCP.G.S"):
+    for mnem in common + ("HGMMA.64x256x16.F32", "F2FP.SATFINITE", "UBLKCP.G.S"):
         assert mnem in dgrad, mnem
     assert "UBLKCP.G.S" in train and "UBLKCP.G.S" not in infer          # shared -> global bulk stores: training mode only
-    for mnem in ("UTCHMMA", "UBLKCP", "LDTM.x32", "UTCBAR"):
+    for mnem in common + ("HGMMA.64x256x16.F32", "HGMMA.64x64x16.F32"):
         assert mnem in wgrad, mnem
     for b in (infer, train, dgrad, wgrad):
         assert "HMMA.16816" not in b                                    # no mma.sync path
 
 
 def test_fused_kernels_fit_their_resource_budget(nb):
-    """640 threads x 96 registers is the whole register file; the fused kernels must not exceed it, and their spill
-    stack stays small (sincosf slow path + the deferred raw values)."""
+    """The producer warpgroup gives its registers away (setmaxnreg.dec to 40) so that the two MMA warpgroups can hold a 64 x 256
+    fp32 accumulator each (setmaxnreg.inc); the accumulators must then stay in registers: no local-memory traffic at all in the
+    dgrad and weight-gradient kernels, and in the forward kernel only the 28-byte argument-reduction buffer of sincosf's slow
+    path (stack <= 32 bytes, as ptxas reports with 0 bytes of spills)."""
     usage = _cuobjdump("-res-usage")
     found = {}
     lines = usage.splitlines()
     for i, ln in enumerate(lines):
-        m = re.search(r"Function (\S*(?:march_tc2|dgrad_tc2)_kernel\S*):", ln)
+        m = re.search(r"Function (\S*(?:march_wg|dgrad_wg|wgrad_wg)_kernel\S*):", ln)
         if m and i + 1 < len(lines):
             r = re.search(r"REG:(\d+) STACK:(\d+)", lines[i + 1])
             found[m.group(1)] = (int(r.group(1)), int(r.group(2)))
-    assert len(found) == 3, found
+    assert len(found) == 4, found
+    sass = _cuobjdump("-sass")
+    bodies, cur = {}, None
+    for ln in sass.splitlines():
+        m = re.search(r"Function : (\S+)", ln)
+        if m:
+            cur = m.group(1); bodies[cur] = []
+        elif cur is not None:
+            bodies[cur].append(ln)
     for name, (reg, stack) in found.items():
-        assert reg <= 96, (name, reg)
-        assert stack <= 160, (name, stack)
+        body = "\n".join(bodies[name])
+        assert reg <= 168, (name, reg)                                  # 384 threads at launch
+        assert "USETMAXREG.DEALLOC.CTAPOOL 0x28" in body and "USETMAXREG.TRY_ALLOC" in body, name
+        if "march_wg" in name:
+            assert stack <= 32, (name, stack)
+        else:
+            assert stack == 0 and not re.search(r"\b(STL|LDL)\b", body), (name, stack)

@@ -1,7 +1,7 @@
 """CPU study for the round-2 tensor-core backward: which operand format may the gradient GEMMs use?
 
 Emulates the planned dataflow of one network pass on the CPU (numpy): forward with fp16 weights / activations and fp32
-accumulation (what march_tc2_kernel does), then dgrad  dH = dA W  and wgrad  dW = dA^T H  with the activation-gradient
+accumulation (what march_wg_kernel does), then dgrad  dH = dA W  and wgrad  dW = dA^T H  with the activation-gradient
 operand dA rounded to a candidate format (weights and saved activations stay fp16, accumulation fp32), and compares
 every parameter gradient with a float64 evaluation of the exact algorithm (oracle.nerf_backward).
 

@@ -9,7 +9,7 @@ from nerf_pytorch_b200 import _lib
 dev = torch.device("cuda:0")
 lib = _lib.load_dev()
 per = 16 << 20
-nb_max = 148
+nb_max = torch.cuda.get_device_properties(0).multi_processor_count
 buf = torch.zeros(8 * nb_max * per, dtype=torch.uint8, device=dev)
 out = torch.zeros(nb_max + 8, dtype=torch.int64, device=dev)
 st = torch.cuda.current_stream().cuda_stream
@@ -26,9 +26,9 @@ def run(mode, chunk, stages, nblk, scatter=0):
             best = e0.elapsed_time(e1); cyc = out[:nblk].cpu().double()
     print(json.dumps({"mechanism": names[mode], "chunk": chunk, "stages": stages, "ctas": nblk, "scatter": scatter, "TBps": round(nblk * per / (best * 1e-3) / 1e12, 3),
                       "bytes_per_clk_per_sm_median": round(per / float(cyc.median()), 2)}), flush=True)
-for nblk in (148, 74):
+for nblk in (nb_max, nb_max // 2):
     for mode, chunk, stages in ((0, 65536, 3), (0, 32768, 6), (0, 16384, 8), (0, 8192, 8), (1, 65536, 3), (1, 32768, 6), (1, 16384, 8),
                                 (2, 65536, 2), (2, 65536, 3), (2, 16384, 8), (3, 16384, 1), (4, 16384, 1)):
         run(mode, chunk, stages, nblk)
 for mode, chunk, stages in ((0, 65536, 3), (0, 8192, 8), (2, 65536, 3), (2, 16384, 8)):
-    run(mode, chunk, stages, 148, scatter=1)
+    run(mode, chunk, stages, nb_max, scatter=1)

@@ -1,4 +1,4 @@
-"""MN-major descriptor check for the round-2 weight-gradient GEMM: out = X^T Y through tcgen05 with both operands
+"""MN-major descriptor check for the round-2 weight-gradient GEMM: out = X^T Y through wgmma with both operands
 read from activation-layout tiles; sweeps (lbo, sbo) encodings and prints the error of each."""
 import ctypes as C, os, sys
 import numpy as np, torch
