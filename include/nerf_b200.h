@@ -187,7 +187,8 @@ int nerf_b200_render_fwd(const NerfRayGen* gen, float* rays, int64_t N, const Ne
  *      sign bits of the pre-activations (csrc/train_common.cuh) -- what the reference's autograd saves
  *      (run_nerf_helpers.py:96-119), but written once, in the MMA operand layout (two 64-row half images per
  *      tile image), by cp.async.bulk from the shared-memory tiles the forward produces anyway.
- *      use_viewdirs networks, tensor-core precision. ---------------------------------------------------------- */
+ *      Tensor-core precision, with or without view directions (one record layout: a net without them leaves
+ *      the view-layer slots unused). ----------------------------------------------------------------------- */
 typedef struct NerfTrainSave {
   void*  act;   size_t act_bytes;    /* activation records: nerf_b200_train_record_bytes(...)            */
   void*  mask;  size_t mask_bytes;   /* ReLU sign-bit records                                            */
@@ -222,7 +223,8 @@ typedef struct NerfNetGrads {
 } NerfNetGrads;
 /* tensor-core backward (csrc/bwd_wg.cuh): compositing adjoint, wgmma dgrad chain with loss-scaled fp16
  * activation gradients, layer-major wgmma weight gradient; consumes the records of the training-mode pass
- * and its raw [N,S,4]. */
+ * and its raw [N,S,4].  Networks with view directions or with output_linear (output_ch >= 4; its rows >= 4 never
+ * reach the loss and get no gradient). */
 int nerf_b200_march_bwd_tc(const float* rays, const float* z_vals, const float* noise, int64_t N, int S,
                            const NerfNetParams* net, const void* packed, const NerfRenderCfg* cfg,
                            const float* raw, const NerfTrainSave* save, const float* g_rgb,
@@ -235,7 +237,7 @@ int nerf_b200_march_bwd_tc_layout(int64_t N, int S, const NerfNetParams* net, in
 /* Backward of BOTH passes of one render_rays call -- what loss.backward() triggers for loss = img2mse(rgb) + img2mse(rgb0)
  * (run_nerf.py:765-772; z_samples is detached at :394, so the two passes are independent).  Same kernels as
  * nerf_b200_march_bwd_tc per pass, one pass after the other on `stream` (CUDA-graph capturable).  `fine` may be NULL
- * (N_importance == 0). */
+ * (N_importance == 0).  Both networks must agree on use_viewdirs: they share the ray batch. */
 typedef struct {
   const float* z_vals;      /* [N,S] */
   const float* noise;       /* [N,S] or NULL */

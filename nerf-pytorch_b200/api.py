@@ -49,8 +49,8 @@ def get_precision() -> str:
 
 
 def set_backward(mode: str):
-    """'tc' (default in tc_fp16 precision: wgmma backward from the forward's saved tile records) or 'exact'
-    (fp32 CUDA-core recompute backward; always used in fp32 precision and for networks without view directions)."""
+    """'tc' (default in tc_fp16 precision: wgmma backward from the forward's saved tile records, with or without view
+    directions) or 'exact' (fp32 CUDA-core recompute backward; always used in fp32 precision)."""
     if mode not in ("tc", "exact"):
         raise ValueError(mode)
     _PRECISION["backward"] = mode
@@ -521,8 +521,9 @@ class _RenderRays(torch.autograd.Function):
         retraw, fine = cfgd["retraw"], Ni > 0
         # cfgd["want_grad"]: grad mode was on at the call AND a parameter requires a gradient (inside Function.forward grad mode is
         # always off, and ctx.needs_input_grad stays True under torch.no_grad()): only then the training-mode kernel runs
-        train_tc = bool(tc and cfgd["want_grad"] and get_backward() == "tc" and net_c.use_viewdirs and
-                        (net_f is None or net_f.use_viewdirs))
+        # (the tensor-core backward needs both nets alike with or without view directions: they share the ray batch)
+        train_tc = bool(tc and cfgd["want_grad"] and get_backward() == "tc" and
+                        (net_f is None or bool(net_f.use_viewdirs) == bool(net_c.use_viewdirs)))
         raw_c = torch.empty((N, Sc, 4), **f32) if ((retraw and not fine) or not tc or train_tc) else None
         out_c = NerfPassOut(_ptr(o["rgb0"]), _ptr(o["disp0"]), _ptr(o["acc0"]), C.c_void_p(0), _ptr(o["w0"]), _ptr(raw_c))
         z_f = z_std = raw_f = None

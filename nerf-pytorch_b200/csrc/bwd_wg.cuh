@@ -8,6 +8,8 @@
 //
 //   raw2outputs_bwd_kernel (small_kernels.cuh)  dL/draw per sample                       (SURVEY App. E)
 //   dhv_seed_heads_kernel  d_hv = relu'(hv) * (d_rgb W_rgb) as tile images + rgb_linear's weight / bias gradient (:114)
+//   dA_seed_output_kernel  (no view directions) dA_{D-1} = relu'(a_{D-1}) * (d_raw W_out[:4]) as tile images + output_linear's
+//                        weight / bias gradient (:117); the chain below then starts at dA_{D-1}
 //   dgrad_wg_kernel      the chain  d_hv -> d_feat -> dA_{D-1} -> ... -> dA_0  as wgmma passes with TRANSPOSED weight chunks
 //                        streamed through the forward's weight ring; the epilogue applies the ReLU mask (and the alpha_linear
 //                        rank-1 term), writes the next A operand in place and copies it to the gradient record.  Activation
@@ -34,10 +36,13 @@ namespace nb {
 // ---------------------------------------------------------------------------------------------------------------
 // backward weight stream: step 0 = views_linears[0].weight[:, :W]^T (K = W/2: 4 chunks), step 1 = feature_linear^T,
 // step j >= 2 = pts_linears[D+1-j].weight[:, h columns]^T (8 chunks each); every chunk is [N = 256 x K = 32] fp16 in the
-// forward's SWIZZLE_64B K-major image (pack_weights)
+// forward's SWIZZLE_64B K-major image (pack_weights).  A net without view directions has no steps 0 and 1: its stream
+// starts at step 2.
 // ---------------------------------------------------------------------------------------------------------------
 __host__ __device__ __forceinline__ int bwd_step_units(int j) { return j == 0 ? 4 : 8; }
-static inline int bwd_stream_chunks(int D) { return 4 + 8 * D; }
+static inline int bwd_stream_chunks(int D, int use_viewdirs) { return use_viewdirs ? 4 + 8 * D : 8 * (D - 1); }
+// first dgrad step: 0 (d_hv seed -> d_feat -> ...) with view directions, 2 (dA_{D-1} seed) without
+__host__ __device__ __forceinline__ int bwd_first_step(int use_viewdirs) { return use_viewdirs ? 0 : 2; }
 
 // ---------------------------------------------------------------------------------------------------------------
 // max |g| over n floats -> *out (bit pattern; non-negative floats order like unsigned ints).  *out zeroed by the caller.
@@ -154,19 +159,122 @@ __global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// output_linear's backward (run_nerf_helpers.py:117: a net without view directions), both halves in one sweep over the rows:
+//   seed of the dgrad chain: dA_{D-1}[row][c] = (pre_{D-1}[row][c] > 0) * sum_{k<4} (scale d_raw[row][k]) W_out[k][c], written as
+//     the step-1 image of every tile's gradient record -- where the view-direction chain leaves dA_{D-1} too, so that dgrad and
+//     wgrad read one layout (rows beyond the CTA's range: zeros, they rely on that);
+//   weight / bias gradient: dW_out[k][c] += sum_rows d_raw[row][k] h_{D-1}[row][c],  db_out[k] += sum_rows d_raw[row][k]   (k < 4,
+//     fp32; rows >= 4 of a 5-output head never reach the loss (run_nerf.py:187) and keep their zero gradient)
+// One warp per row, lane = eight columns: a row is 512 contiguous bytes of h_{D-1} in and of dA_{D-1} out.
+// ---------------------------------------------------------------------------------------------------------------
+struct SeedOutParams {
+  const float* d_raw; const uint8_t* mask; const uint8_t* act; uint8_t* grad; const float* out_w; const unsigned int* amax;
+  long long N; int S, rays_per_cta, nst_plan, D;
+  uint32_t rec_mask, rec_act, rec_grad; long long n_tiles;
+  float* g_out_w; float* g_out_b;
+};
+constexpr int SEED_OUT_BATCH = 4;         // rows of a warp whose loads are in flight together
+
+__global__ void __launch_bounds__(256, 2) dA_seed_output_kernel(const SeedOutParams p) {
+  __shared__ float s_acc[8][32 * 32 + 4];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int c = lane * 8, word = (lane >> 4) * 4 + ((lane >> 2) & 3), bit0 = 8 * (lane & 3);
+  const float scale = loss_scale_from_absmax(__uint_as_float(*p.amax));
+  float wk[4][8], a[4][8], b[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { wk[k][i] = p.out_w[256 * k + c + i] * scale; a[k][i] = 0.f; }
+  for (long long t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
+    const int cta = (int)(t / (2 * p.nst_plan)), st = (int)((t >> 1) % p.nst_plan), X = (int)(t & 1);
+    if (st >= plan_cta_nst(p.N, p.S, p.rays_per_cta, cta)) continue;          // never read (the CTA has no rows there)
+    const int nrows = plan_cta_rows(p.N, p.S, p.rays_per_cta, cta);
+    const int lr0 = st * 256 + X * 128;
+    const long long row_begin = (long long)cta * p.rays_per_cta * p.S;
+    const int nv = (nrows - lr0 < 128) ? nrows - lr0 : 128;                   // (<= 0: past the CTA's rows -> a tile of zeros)
+    const uint8_t* h = p.act + (size_t)t * p.rec_act + rec_act_h(p.D - 1);
+    // mask word of this lane's columns: layer D-1, half ch = c >> 7, word (c >> 5) & 3 of the row's uint4
+    const uint8_t* mrec = p.mask + (size_t)t * p.rec_mask + (uint32_t)(p.D - 1) * 4096u + (uint32_t)(word >> 2) * 2048u + (uint32_t)(word & 3) * 4u;
+    uint8_t* const g = p.grad + (size_t)t * p.rec_grad + rec_grad_step(1);
+    // warp w takes rows 16 w .. 16 w + 15; their dL/draw rows come in as one coalesced load (lane i < 16 holds row i's float4)
+    const int rbase = warp * 16;
+    float4 dmine = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (lane < 16 && rbase + lane < nv) dmine = reinterpret_cast<const float4*>(p.d_raw)[row_begin + lr0 + rbase + lane];
+    for (int r8 = 0; r8 < 16; r8 += SEED_OUT_BATCH) {
+      uint4 hw[SEED_OUT_BATCH];
+      uint32_t mw[SEED_OUT_BATCH];
+#pragma unroll
+      for (int k = 0; k < SEED_OUT_BATCH; ++k) {
+        const int r = rbase + r8 + k;
+        hw[k] = make_uint4(0u, 0u, 0u, 0u); mw[k] = 0u;
+        if (r < nv) {
+          hw[k] = *reinterpret_cast<const uint4*>(h + img_off(r, c, 256));
+          mw[k] = *reinterpret_cast<const uint32_t*>(mrec + (uint32_t)r * 16u);
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < SEED_OUT_BATCH; ++k) {
+        const int r = rbase + r8 + k;
+        const float d[4] = {__shfl_sync(0xffffffffu, dmine.x, r8 + k), __shfl_sync(0xffffffffu, dmine.y, r8 + k),
+                            __shfl_sync(0xffffffffu, dmine.z, r8 + k), __shfl_sync(0xffffffffu, dmine.w, r8 + k)};
+        uint4 out = make_uint4(0u, 0u, 0u, 0u);
+        if (r < nv) {
+          const uint32_t hu[4] = {hw[k].x, hw[k].y, hw[k].z, hw[k].w};
+          float x[8];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const __half2 hh = *reinterpret_cast<const __half2*>(&hu[q]);
+            const float hv2[2] = {__low2float(hh), __high2float(hh)};
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int i = 2 * q + e;
+#pragma unroll
+              for (int kk = 0; kk < 4; ++kk) a[kk][i] = fmaf(d[kk], hv2[e], a[kk][i]);
+              x[i] = mask_apply(mw[k], bit0 + i, fmaf(d[0], wk[0][i], fmaf(d[1], wk[1][i], fmaf(d[2], wk[2][i], d[3] * wk[3][i]))));
+            }
+          }
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) b[kk] += d[kk];
+          out = make_uint4(ptx::cvt_sat_f16x2(x[0], x[1]), ptx::cvt_sat_f16x2(x[2], x[3]), ptx::cvt_sat_f16x2(x[4], x[5]), ptx::cvt_sat_f16x2(x[6], x[7]));
+        }
+        *reinterpret_cast<uint4*>(g + img_off(r, c, 256)) = out;
+      }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s_acc[warp][(8 * k + i) * 32 + lane] = a[k][i];
+  if (lane == 0) { s_acc[warp][1024] = b[0]; s_acc[warp][1025] = b[1]; s_acc[warp][1026] = b[2]; s_acc[warp][1027] = b[3]; }
+  __syncthreads();
+  for (int i = threadIdx.x; i < 1028; i += 256) {
+    float v = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) v += s_acc[w][i];
+    if (i < 1024) {                                     // i = (k * 8 + e) * 32 + lane  ->  weight[k][lane * 8 + e]
+      const int k = i >> 8, e = (i >> 5) & 7, ln = i & 31;
+      atomicAdd(p.g_out_w + k * 256 + ln * 8 + e, v);
+    } else atomicAdd(p.g_out_b + (i - 1024), v);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // dgrad chain -- the warpgroup roles, weight ring and operand layout of march_wg_kernel (fused_wg.cuh), with the backward
 // weight stream (transposed chunks) and the gradient record: each MMA warpgroup loads its 64 rows of the tile's d_hv seed
 // (16 KB, one bulk copy), then runs steps j = 0..D: step 0 = d_hv W_v[:, :W] -> d_feat, step j >= 1 = the previous step's
 // output times the transposed weights of the layer above -> (+ d_sigma alpha_linear.weight at j = 1) -> ReLU mask of pts layer
 // D - j from the forward's sign bits -> saturating fp16, in place as the next step's A operand and, byte for byte, the
 // warpgroup's half of the step's image in the gradient record (one 32 KB bulk store).
+// Without view directions (first_step = 2) the seed is dA_{D-1} itself (dA_seed_output_kernel, the step-1 image): each MMA
+// warpgroup loads its 32 KB half straight into its A operand and the chain runs steps 2..D; d_raw and alpha_w are not read.
 // ---------------------------------------------------------------------------------------------------------------
 struct DgradParams {
   const uint8_t* mask; uint8_t* grad; const float* d_raw; const unsigned int* amax; const float* alpha_w;
-  const uint8_t* chunks;                    // backward weight stream (pack_weights)
+  const uint8_t* chunks;                    // backward weight stream (pack_weights), starting at step first_step
   long long N; int S, rays_per_cta, nst_plan, D;
   uint32_t rec_mask, rec_grad;
   int vc0, vc1;                             // forward CTAs [vc0, vc1): this launch's CTA b serves vc0 + b, vc0 + b + gridDim, ...
+  int first_step;                           // 0: d_hv seed (view directions), 2: dA_{D-1} seed (output_linear head)
 };
 
 __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradParams p) {
@@ -174,10 +282,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
   const uint32_t sb = ptx::smem_u32(smem);
   if ((sb & 1023u) != 0) __trap();
   float* s_alpha = reinterpret_cast<float*>(smem + SM_HEADS);
-  const int D = p.D, NS = D + 1;
+  const int D = p.D, NS = D + 1, j0 = p.first_step;
   Ring rg{sb + SM_BARS, sb + SM_BARS + 8 * TC_NST, 0, 0};
   const uint32_t bar_seed = sb + SM_BARS + 16 * TC_NST;          // [2]: one per MMA warpgroup
-  for (int i = threadIdx.x; i < 256; i += TC_THREADS) s_alpha[i] = p.alpha_w[i];
+  if (j0 == 0)
+    for (int i = threadIdx.x; i < 256; i += TC_THREADS) s_alpha[i] = p.alpha_w[i];
   if (threadIdx.x == 0) {
     for (int i = 0; i < TC_NST; ++i) { ptx::mbar_init(rg.full + 8 * i, 1); ptx::mbar_init(rg.empty + 8 * i, 256); }
     ptx::mbar_init(bar_seed, 1); ptx::mbar_init(bar_seed + 8, 1);
@@ -192,7 +301,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
       for (int vc = p.vc0 + (int)blockIdx.x; vc < p.vc1; vc += (int)gridDim.x)
         for (int tile = 0, nt = 2 * plan_cta_nst(p.N, p.S, p.rays_per_cta, vc); tile < nt; ++tile) {
           const uint8_t* src = p.chunks;
-          for (int j = 0; j < NS; ++j)
+          for (int j = j0; j < NS; ++j)
             for (int u = 0; u < bwd_step_units(j); ++u) {
               ptx::mbar_wait(rg.empty + 8 * rg.stage, rg.phase ^ 1);
               ptx::mbar_arrive_expect_tx(rg.full + 8 * rg.stage, TC_STAGE_BYTES);
@@ -229,20 +338,29 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
       const uint8_t* const mrec = p.mask + (size_t)tid * p.rec_mask;
       uint8_t* const grec = p.grad + (size_t)tid * p.rec_grad;
       const int lrb = st * TC_ST + X * TC_TILE + 64 * w;
-      // the warpgroup's 64 rows of the seed (the MMAs of the previous tile's step 0 have read the buffer)
+      // the warpgroup's 64 rows of the seed (the MMAs of the previous tile's step 0 have read the buffer); a dA_{D-1} seed goes
+      // to the A operand, once the previous tile's last record copy has read it
       if (t == 0) {
-        ptx::mbar_arrive_expect_tx(bar_seed + 8 * w, 16384u);
-        ptx::bulk_g2s(seed, grec + (uint32_t)w * 16384u, 16384u, bar_seed + 8 * w);
+        if (j0 == 0) {
+          ptx::mbar_arrive_expect_tx(bar_seed + 8 * w, 16384u);
+          ptx::bulk_g2s(seed, grec + (uint32_t)w * 16384u, 16384u, bar_seed + 8 * w);
+        } else {
+          ptx::bulk_wait_read0();
+          ptx::mbar_arrive_expect_tx(bar_seed + 8 * w, 32768u);
+          ptx::bulk_g2s(act, grec + rec_grad_step(1) + (uint32_t)w * 32768u, 32768u, bar_seed + 8 * w);
+        }
       }
-      float dsig[2];
+      float dsig[2] = {0.f, 0.f};
+      if (j0 == 0) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int lr = lrb + (h ? r1 : r0);
-        dsig[h] = lr < nrows ? p.d_raw[(row_begin + lr) * 4 + 3] * scale : 0.f;
+        for (int h = 0; h < 2; ++h) {
+          const int lr = lrb + (h ? r1 : r0);
+          dsig[h] = lr < nrows ? p.d_raw[(row_begin + lr) * 4 + 3] * scale : 0.f;
+        }
       }
       ptx::mbar_wait(bar_seed + 8 * w, sph);
       sph ^= 1;
-      for (int j = 0; j < NS; ++j) {
+      for (int j = j0; j < NS; ++j) {
         // ReLU mask of this step's output (the pre-activation of pts layer D - j), fetched before the MMAs
         uint4 mk[2][2];
 #pragma unroll

@@ -119,7 +119,6 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
   TrainSaveDev sv;
   memset(&sv, 0, sizeof(sv));
   if (save) {
-    NB_CHECK_ARG(net->use_viewdirs, "training-mode records are implemented for use_viewdirs networks");
     NB_CHECK_ARG(save->act && save->mask, "training-mode save buffers are NULL");
     NB_CHECK_ARG(save->act_bytes >= (size_t)plan.n_tiles * rec_act_bytes(net->D) && save->mask_bytes >= (size_t)plan.n_tiles * rec_mask_bytes(net->D),
                  "training-mode save buffers too small (see nerf_b200_train_record_bytes)");
@@ -222,7 +221,8 @@ int nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t packed
   if (PL.bwd_bytes) {
     // backward (dgrad) stream, bwd_wg.cuh: chunk [n][k] = W[k0 + k][col0 + n] -- the transposed weights, so that the
     // chain dA_{l-1} = dA_l W_l runs through the forward's operand layouts.  Step 0: views_linears[0].weight[:, :W]
-    // (K = W/2), step 1: feature_linear, then pts_linears[D-1] ... [1] restricted to their h columns.
+    // (K = W/2), step 1: feature_linear, then pts_linears[D-1] ... [1] restricted to their h columns.  Without view
+    // directions the chain starts at step 2 (dA_{D-1} is seeded from output_linear): only the pts-layer chunks.
     PackJob bj2;
     bj2.n = 0;
     unsigned boff = (unsigned)PL.off_bwd;
@@ -231,13 +231,15 @@ int nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t packed
       c.src = src + col0; c.sn = 1; c.sk = ld; c.k0 = k0; c.kvalid = 32; c.nrows = 256; c.dst_off = boff;
       boff += 256u * 64u;
     };
-    for (int c = 0; c < 4; ++c) addT(net->views_w, W + net->input_ch_views, 0, 32 * c);
-    for (int c = 0; c < 8; ++c) addT(net->feature_w, W, 0, 32 * c);
+    if (net->use_viewdirs) {
+      for (int c = 0; c < 4; ++c) addT(net->views_w, W + net->input_ch_views, 0, 32 * c);
+      for (int c = 0; c < 8; ++c) addT(net->feature_w, W, 0, 32 * c);
+    }
     for (int l = net->D - 1; l >= 1; --l) {
       const bool sk = (net->skip >= 0 && l == net->skip + 1);
       for (int c = 0; c < 8; ++c) addT(net->pts_w[l], sk ? W + IC : W, sk ? IC : 0, 32 * c);
     }
-    NB_CHECK_ARG(bj2.n == 4 + 8 * net->D && boff == PL.off_bwd + PL.bwd_bytes, "internal: backward chunk table mismatch");
+    NB_CHECK_ARG(bj2.n == bwd_stream_chunks(net->D, net->use_viewdirs) && boff == PL.off_bwd + PL.bwd_bytes, "internal: backward chunk table mismatch");
     dim3 g2(4, bj2.n);
     pack_chunks_kernel<<<g2, 256, 0, st>>>(bj2, static_cast<uint8_t*>(packed));
     NB_LAUNCH_OK("pack_chunks_kernel (backward stream)");
@@ -687,9 +689,12 @@ BwdTcJobs make_bwd_jobs(const NerfNetParams& n, const NerfNetGrads* g, int sms) 
     }
   };
   // job 0: G = d_hv^T h_{D-1} (-> views_linears[0].weight[:, :W] through views_feat_wgrad_kernel; its reduce target is a scratch
-  // block set by the caller);  jobs 1, 2: feature_linear = d_feat^T h_{D-1} (job 1 also forms alpha_linear's gradient)
-  add(0, 128, rec_act_h(D - 1), 256, nullptr, 256, 256, g ? g->views_b : nullptr);
-  add(rec_grad_step(0), 256, rec_act_h(D - 1), 256, g ? g->feature_w : nullptr, W, W, g ? g->feature_b : nullptr);
+  // block set by the caller);  jobs 1, 2: feature_linear = d_feat^T h_{D-1} (job 1 also forms alpha_linear's gradient).
+  // Without view directions the pts layers are all (output_linear's gradient comes from dA_seed_output_kernel).
+  if (n.use_viewdirs) {
+    add(0, 128, rec_act_h(D - 1), 256, nullptr, 256, 256, g ? g->views_b : nullptr);
+    add(rec_grad_step(0), 256, rec_act_h(D - 1), 256, g ? g->feature_w : nullptr, W, W, g ? g->feature_b : nullptr);
+  }
   for (int l = D - 1; l >= 1; --l) {
     const bool sk = (n.skip >= 0 && l == n.skip + 1);
     add(rec_grad_dA(l, D), 256, rec_act_h(l - 1), 256, g ? g->pts_w[l] + (sk ? IC : 0) : nullptr, sk ? W + IC : W, W, g ? g->pts_b[l] : nullptr);
@@ -755,7 +760,7 @@ static size_t bwd_pass_bytes(int64_t N, int S, const NerfNetParams* net) {
 }
 
 size_t nerf_b200_march_bwd_tc_workspace_bytes(int64_t N, int S, const NerfNetParams* net) {
-  if (!net || check_tc_net(net) || !net->use_viewdirs || N <= 0 || S <= 0) return 0;
+  if (!net || check_tc_net(net) || N <= 0 || S <= 0) return 0;
   return bwd_pass_bytes(N, S, net);
 }
 
@@ -764,7 +769,7 @@ size_t nerf_b200_march_bwd_tc_workspace_bytes(int64_t N, int S, const NerfNetPar
 // rec_grad_bytes, grid, rays_per_cta, nst, n_tiles, off_amax, off_dsum, off_partial
 int nerf_b200_march_bwd_tc_layout(int64_t N, int S, const NerfNetParams* net, int64_t* out) {
   if (int rc = check_tc_net(net)) return rc;
-  NB_CHECK_ARG(out && N > 0 && S > 0 && net->use_viewdirs, "bad arguments");
+  NB_CHECK_ARG(out && N > 0 && S > 0, "bad arguments");
   const int sms = num_sms();
   const TilePlan plan = make_tile_plan(N, S, sms);
   const BwdTcLayout LY = make_bwd_layout(N, S, *net, plan, (long long)sms * 256 * 256);
@@ -810,15 +815,28 @@ struct BwdTcPass {
     return 0;
   }
 
-  // 1. loss scale from max |dL/drgb_map|; compositing adjoint -> dL/draw (SURVEY App. E);  2. seed of the chain: d_hv tiles
+  // 1. loss scale from max |dL/drgb_map|; compositing adjoint -> dL/draw (SURVEY App. E);  2. seed of the chain: d_hv tiles, or
+  // without view directions dA_{D-1} tiles (+ output_linear's gradient)
   int prologue(cudaStream_t st) {
     const int sms = ds->sms, D = net->D;
     NB_CUDA(cudaMemsetAsync(amax, 0, 256, st));
-    NB_CUDA(cudaMemsetAsync(dsum, 0, (size_t)N * 128 * 4, st));
-    NB_CUDA(cudaMemsetAsync(gv, 0, (size_t)(128 * 256 + 128) * 4, st));
+    if (net->use_viewdirs) {
+      NB_CUDA(cudaMemsetAsync(dsum, 0, (size_t)N * 128 * 4, st));
+      NB_CUDA(cudaMemsetAsync(gv, 0, (size_t)(128 * 256 + 128) * 4, st));
+    }
     absmax_kernel<<<cdiv(N * 3, 1024) < 64 ? cdiv(N * 3, 1024) : 64, 256, 0, st>>>(g_rgb, N * 3, amax);
     NB_LAUNCH_OK("absmax_kernel");
     NB_TRY(nerf_b200_raw2outputs_bwd(raw, z, rays + 3, cfg->ray_stride, noise, N, S, cfg->white_bkgd, g_rgb, d_raw, (void*)st));
+    if (!net->use_viewdirs) {
+      SeedOutParams so;
+      so.d_raw = d_raw; so.mask = mask; so.act = act; so.grad = grec; so.out_w = net->output_w; so.amax = amax;
+      so.N = N; so.S = S; so.rays_per_cta = plan.rays_per_cta; so.nst_plan = plan.nst; so.D = D;
+      so.rec_mask = rec_mask_bytes(D); so.rec_act = rec_act_bytes(D); so.rec_grad = rec_grad_bytes(D); so.n_tiles = plan.n_tiles;
+      so.g_out_w = grads->output_w; so.g_out_b = grads->output_b;
+      dA_seed_output_kernel<<<(int)(plan.n_tiles < 2 * sms ? plan.n_tiles : 2 * sms), 256, 0, st>>>(so);
+      NB_LAUNCH_OK("dA_seed_output_kernel");
+      return 0;
+    }
     SeedParams sp;
     sp.d_raw = d_raw; sp.mask = mask; sp.act = act; sp.grad = grec; sp.rgb_w = net->rgb_w; sp.amax = amax;
     sp.N = N; sp.S = S; sp.rays_per_cta = plan.rays_per_cta; sp.nst_plan = plan.nst; sp.D = D;
@@ -835,17 +853,22 @@ struct BwdTcPass {
     const int D = net->D;
     const uint8_t* pk = static_cast<const uint8_t*>(packed);
     DgradParams dp;
-    dp.mask = mask; dp.grad = grec; dp.d_raw = d_raw; dp.amax = amax; dp.alpha_w = net->alpha_w;
+    const bool views = net->use_viewdirs != 0;
+    dp.mask = mask; dp.grad = grec; dp.amax = amax;
+    dp.d_raw = views ? d_raw : nullptr; dp.alpha_w = views ? net->alpha_w : nullptr;
     dp.chunks = pk + PL.off_bwd;
     dp.N = N; dp.S = S; dp.rays_per_cta = plan.rays_per_cta; dp.nst_plan = plan.nst; dp.D = D;
     dp.rec_mask = rec_mask_bytes(D); dp.rec_grad = rec_grad_bytes(D);
     dp.vc0 = vc0; dp.vc1 = vc1;
+    dp.first_step = bwd_first_step(net->use_viewdirs);
     const int grid = plan.grid;
     TimedLaunch* tl = nullptr;
     if (g_timing && g_ntimed < 4096) {
       tl = &g_timed[g_ntimed++];
       cudaEventCreate(&tl->a); cudaEventCreate(&tl->b);
-      tl->flops = 2.0 * ((double)(net->W / 2) * net->W + (double)D * net->W * net->W) * (double)(N * (long long)S) * (double)(vc1 - vc0) / (double)plan.grid;
+      // MACs per row of the steps the kernel runs: K = W/2 (step 0) + D steps of W x W, or without view directions D - 1 steps
+      const double macs = views ? (double)(net->W / 2) * net->W + (double)D * net->W * net->W : (double)(D - 1) * net->W * net->W;
+      tl->flops = 2.0 * macs * (double)(N * (long long)S) * (double)(vc1 - vc0) / (double)plan.grid;
       tl->kind = 1;
       cudaEventRecord(tl->a, st);
     }
@@ -862,8 +885,11 @@ struct BwdTcPass {
     const int D = net->D;
     BwdTcJobs J = make_bwd_jobs(*net, grads, ctas);
     NB_CHECK_ARG(!J.overflow && J.n <= ctas, "weight gradient: %d jobs need at least as many CTAs (have %d; at most %d jobs)", J.n, ctas, WG2_MAX_JOBS);
-    J.w[0].aux = 1; J.w[0].aux_dst = dsum;            // views job: per-ray row sums of d_hv
-    J.w[1].aux = 2; J.w[1].aux_dst = grads->alpha_w; J.w[1].aux_b = grads->alpha_b;   // feature job, first block: alpha_linear gradients
+    const bool views = net->use_viewdirs != 0;
+    if (views) {
+      J.w[0].aux = 1; J.w[0].aux_dst = dsum;            // views job: per-ray row sums of d_hv
+      J.w[1].aux = 2; J.w[1].aux_dst = grads->alpha_w; J.w[1].aux_b = grads->alpha_b;   // feature job, first block: alpha_linear gradients
+    }
     WgradParams wp;
     memset(&wp, 0, sizeof(wp));
     wp.act = act; wp.grad = grec; wp.rec_act = rec_act_bytes(D); wp.rec_grad = rec_grad_bytes(D);
@@ -875,7 +901,9 @@ struct BwdTcPass {
     if (g_timing && g_ntimed < 4096) {
       tl = &g_timed[g_ntimed++];
       cudaEventCreate(&tl->a); cudaEventCreate(&tl->b);
-      tl->flops = 2.0 * (net_macs_per_row(*net) - (double)net->W - 3.0 * (net->W / 2) - (double)net->input_ch_views * (net->W / 2)) * (double)(N * (long long)S) * (double)(vc1 - vc0) / (double)plan.grid;
+      // every Linear but the heads (alpha / rgb_linear and the view columns, or output_linear: other kernels form those)
+      const double heads = views ? (double)net->W + 3.0 * (net->W / 2) + (double)net->input_ch_views * (net->W / 2) : (double)net->W * net->output_ch;
+      tl->flops = 2.0 * (net_macs_per_row(*net) - heads) * (double)(N * (long long)S) * (double)(vc1 - vc0) / (double)plan.grid;
       tl->kind = 2;
       cudaEventRecord(tl->a, st);
     }
@@ -885,7 +913,7 @@ struct BwdTcPass {
     ReduceParams rp;
     memset(&rp, 0, sizeof(rp));
     rp.partial = partial; rp.amax = amax; rp.njobs = J.n;
-    J.r[0].dst = gv;                                  // job 0 reduces into the scratch block G
+    if (views) J.r[0].dst = gv;                       // job 0 reduces into the scratch block G
     for (int i = 0; i < J.n; ++i) rp.jobs[i] = J.r[i];
     dim3 rg(128, J.n);
     wgrad_reduce_kernel<<<rg, 256, 0, st>>>(rp);
@@ -893,8 +921,9 @@ struct BwdTcPass {
     return 0;
   }
 
-  // 5. the view columns of views_linears[0] (after ALL of the pass's weight-gradient launches)
+  // 5. the view columns of views_linears[0] (after ALL of the pass's weight-gradient launches); nothing without view directions
   int heads(cudaStream_t st) {
+    if (!net->use_viewdirs) return 0;
     const int ICV = net->input_ch_views;
     encv_kernel<<<cdiv(N * ICV, 256), 256, 0, st>>>(rays + 8, cfg->ray_stride, N, ICV, encv);
     NB_LAUNCH_OK("encv_kernel");
@@ -910,7 +939,7 @@ struct BwdTcPass {
 int check_bwd_pass(const float* rays, const NerfBwdPass* q, const NerfRenderCfg* cfg) {
   NB_CHECK_ARG(rays && q && q->z_vals && q->net && q->packed && cfg && q->raw && q->save && q->g_rgb && q->grads, "NULL pointer");
   if (int rc = check_tc_net(q->net)) return rc;
-  NB_CHECK_ARG(q->net->use_viewdirs, "the tensor-core backward serves use_viewdirs networks (exact mode serves the others)");
+  NB_CHECK_ARG(q->net->use_viewdirs || q->net->output_ch >= 4, "output_linear needs output_ch >= 4 (got %d)", q->net->output_ch);
   NB_CHECK_ARG(q->net->W == 256, "the tensor-core backward supports netwidth == 256");
   NB_CHECK_ARG(q->S > 0, "S must be positive");
   return 0;
@@ -942,10 +971,10 @@ int nerf_b200_march_bwd_tc(const float* rays, const float* z_vals, const float* 
 }
 
 size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, const NerfNetParams* net_coarse, int S_fine, const NerfNetParams* net_fine) {
-  if (!net_coarse || check_tc_net(net_coarse) || !net_coarse->use_viewdirs || N <= 0 || S_coarse <= 0) return 0;
+  if (!net_coarse || check_tc_net(net_coarse) || N <= 0 || S_coarse <= 0) return 0;
   size_t b = bwd_pass_bytes(N, S_coarse, net_coarse);
   if (net_fine && S_fine > 0) {
-    if (check_tc_net(net_fine) || !net_fine->use_viewdirs) return 0;
+    if (check_tc_net(net_fine) || net_fine->use_viewdirs != net_coarse->use_viewdirs) return 0;
     b += bwd_pass_bytes(N, S_fine, net_fine);
   }
   return b;
@@ -958,6 +987,8 @@ int nerf_b200_render_rays_bwd_tc(const float* rays, int64_t N, const NerfRenderC
                                  void* workspace, size_t workspace_bytes, void* stream) {
   if (int rc = check_bwd_pass(rays, coarse, cfg)) return rc;
   if (fine) if (int rc = check_bwd_pass(rays, fine, cfg)) return rc;
+  NB_CHECK_ARG(!fine || (fine->net->use_viewdirs != 0) == (coarse->net->use_viewdirs != 0),
+               "coarse and fine networks must agree on use_viewdirs (they share one ray batch)");
   if (N == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   BwdTcPass c = bind_pass(rays, N, cfg, coarse);

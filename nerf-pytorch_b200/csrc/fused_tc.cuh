@@ -46,8 +46,8 @@ struct PackLayout {
   int D, skip, use_viewdirs, IC, ICV, NL;
   int n_chunks;
   size_t off_chunks, chunk_bytes, off_bias, off_heads, off_vdir, total;
-  // backward (dgrad) stream: transposed weight chunks (bwd_wg.cuh); 0 bytes when the net has no view head (the tensor-core
-  // backward serves use_viewdirs nets)
+  // backward (dgrad) stream: transposed weight chunks (bwd_wg.cuh: bwd_stream_chunks); without view directions only the
+  // pts-layer steps j >= 2
   size_t off_bwd, bwd_bytes;
 };
 
@@ -76,7 +76,7 @@ static inline PackLayout make_pack_layout(const NerfNetParams& n) {
   L.off_vdir = L.off_heads + HEADS_FLOATS * 4;
   L.off_bwd = L.off_vdir + (size_t)(128 * (n.input_ch_views > 0 ? n.input_ch_views : 1) + 128) * 4;
   L.off_bwd = (L.off_bwd + 1023) & ~(size_t)1023;
-  L.bwd_bytes = n.use_viewdirs ? (size_t)(4 + 8 * n.D) * TC_STAGE_BYTES : 0;
+  L.bwd_bytes = (size_t)(n.use_viewdirs ? 4 + 8 * n.D : 8 * (n.D - 1)) * TC_STAGE_BYTES;
   L.total = L.off_bwd + L.bwd_bytes;
   return L;
 }

@@ -246,7 +246,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
             }
           }
         }
-        if (!(last_pts && !p.use_viewdirs)) {
+        // without view directions only the fp32 head above reads h_{D-1}: inference skips the fp16 image, training mode still
+        // records it (output_linear's weight gradient reads it, dA_seed_output_kernel in bwd_wg.cuh)
+        if (EMIT || !(last_pts && !p.use_viewdirs)) {
           const bool relu = l < D;
 #pragma unroll
           for (int j = 0; j < 32; ++j) {

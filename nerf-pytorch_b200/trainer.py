@@ -36,8 +36,9 @@ class FusedTrainStep:
         self.lib = _lib.load()
         kw = dict(render_kwargs)
         self.net_c, self.net_f = kw["network_fn"], kw.get("network_fine")
-        if not isinstance(self.net_c, api.NeRF) or not self.net_c.use_viewdirs:
-            raise RuntimeError("FusedTrainStep needs nerf_b200.NeRF networks with use_viewdirs=True")
+        if not isinstance(self.net_c, api.NeRF):
+            raise RuntimeError("FusedTrainStep needs nerf_b200.NeRF networks (with or without view directions)")
+        self.use_viewdirs = bool(self.net_c.use_viewdirs)
         if api.get_precision() != "tc_fp16":
             raise RuntimeError("FusedTrainStep runs the tensor-core path (set_precision('tc_fp16'))")
         self.dev = self.net_c._check_device()
@@ -45,6 +46,9 @@ class FusedTrainStep:
         self.Sc, self.Ni = int(kw["N_samples"]), int(kw.get("N_importance", 0))
         if self.Ni > 0 and self.net_f is None:
             self.net_f = self.net_c
+        if self.Ni > 0 and bool(self.net_f.use_viewdirs) != self.use_viewdirs:
+            raise RuntimeError("FusedTrainStep: coarse and fine networks must agree on use_viewdirs (they share the ray batch)")
+        self.ray_stride = 11 if self.use_viewdirs else 8
         q = kw.get("network_query_fn")
         self.cfgd = dict(N_samples=self.Sc, N_importance=self.Ni, multires=int(getattr(q, "multires", 10)),
                          multires_views=int(getattr(q, "multires_views", 4)), lindisp=bool(kw.get("lindisp", False)),
@@ -81,7 +85,7 @@ class FusedTrainStep:
         self.rays = torch.zeros((2, N, 3), **f32)
         self.rays[1, :, 2] = -1.0
         self.target = torch.zeros((N, 3), **f32)
-        self.packed_rays = torch.empty((N, 11), **f32)
+        self.packed_rays = torch.empty((N, self.ray_stride), **f32)
         self.t_rand = torch.zeros((N, Sc), **f32) if self.cfgd["perturb"] > 0 else None
         self.u_rand = torch.zeros((N, self.Ni), **f32) if (self.cfgd["perturb"] > 0 and self.Ni > 0) else None
         self.noise0 = torch.zeros((N, Sc), **f32) if self.noise_std > 0 else None
@@ -114,7 +118,7 @@ class FusedTrainStep:
         self._bp_f = _lib.NerfBwdPass(api._ptr(self.z_f), api._ptr(self.noise1), Sf, C.pointer(self._np_f), api._ptr(self._pk_f), api._ptr(o["raw"]),
                                       C.pointer(self._sv_f), api._ptr(o["g_rgb"]), C.pointer(self._gs[-1])) if self.Ni > 0 else None
         self._cam = api._camera(self.H, self.W, self.K)
-        self._cfg = api._cfg_struct(self.cfgd, 11)
+        self._cfg = api._cfg_struct(self.cfgd, self.ray_stride)
         self.host_loss = torch.zeros(4, dtype=torch.float32, device="cpu").pin_memory()
         # ---- capture ----
         self.graph = self.graph_adam = None
@@ -141,15 +145,17 @@ class FusedTrainStep:
 
     # ---- the step, as library calls on the current stream ----
     def _pack_rays(self, c2w=None, pixel_index=None):
-        """The ray batch -> packed [N,11] rows.  Outside the graph (one launch): the camera travels in the kernel arguments, so a
-        per-step pose could not be replayed.  Given rays (self.rays) or -- SURVEY 8f rank 3 -- pixels of one posed image."""
+        """The ray batch -> packed [N,11] rows ([N,8] without view directions).  Outside the graph (one launch): the camera travels
+        in the kernel arguments, so a per-step pose could not be replayed.  Given rays (self.rays) or -- SURVEY 8f rank 3 -- pixels of
+        one posed image."""
+        vd = int(self.use_viewdirs)
         with api._on(self.rays):
             if pixel_index is None:
                 check(self.lib.nerf_b200_pack_rays(api._ptr(self.rays[0]), api._ptr(self.rays[1]), None, C.byref(self._cam), self.N, 0, self.ndc, self.near,
-                                                   self.far, 1, api._ptr(self.packed_rays), api._stream(self.rays)), "pack_rays")
+                                                   self.far, vd, api._ptr(self.packed_rays), api._stream(self.rays)), "pack_rays")
             else:
                 cam = api._camera(self.H, self.W, self.K, c2w)
-                check(self.lib.nerf_b200_pack_rays_pixels(C.byref(cam), api._ptr(pixel_index), self.N, self.ndc, self.near, self.far, 1,
+                check(self.lib.nerf_b200_pack_rays_pixels(C.byref(cam), api._ptr(pixel_index), self.N, self.ndc, self.near, self.far, vd,
                                                           api._ptr(self.packed_rays), api._stream(self.rays)), "pack_rays_pixels")
 
     def _fwd_bwd(self):
