@@ -102,6 +102,24 @@ int nerf_b200_raw2outputs(const float* raw, const float* z_vals, const float* ra
 int nerf_b200_raw2outputs_bwd(const float* raw, const float* z_vals, const float* rays_d, int d_stride,
                               const float* noise, int64_t N, int S, int white_bkgd,
                               const float* g_rgb /*[N,3]*/, float* d_raw /*[N,S,4]*/, void* stream);
+/* Gradients of a loss w.r.t. the outputs of one pass, i.e. the seeds of its backward: what autograd hands to
+ * raw2outputs / render_rays when the loss reads more than rgb_map (depth or disparity supervision, a mask loss on
+ * acc_map, a density regulariser on raw).  Every member is optional: NULL = that output does not reach the loss.
+ * disp_map's gradient follows the reference's autograd of 1 / max(1e-10, depth / acc): none where depth/acc < 1e-10
+ * and NaN on rays with acc = 0 (the reference's disp_map is NaN there too).  At least one member must be given. */
+typedef struct NerfOutGrads {
+  const float* rgb_map;    /* [N,3]    dL/drgb_map   */
+  const float* disp_map;   /* [N]      dL/ddisp_map  */
+  const float* acc_map;    /* [N]      dL/dacc_map   */
+  const float* depth_map;  /* [N]      dL/ddepth_map */
+  const float* weights;    /* [N,S]    dL/dweights   */
+  const float* raw;        /* [N,S,4]  dL/draw       */
+} NerfOutGrads;
+/* nerf_b200_raw2outputs_bwd with every output's gradient: d_raw = dL/draw through all of them (nerf_b200_raw2outputs_bwd
+ * is this call with only rgb_map given, and gives bit-identical results) */
+int nerf_b200_raw2outputs_bwd_outs(const float* raw, const float* z_vals, const float* rays_d, int d_stride,
+                                   const float* noise, int64_t N, int S, int white_bkgd,
+                                   const NerfOutGrads* g, float* d_raw /*[N,S,4]*/, void* stream);
 
 /* ---- sample_pdf (run_nerf_helpers.py:196-239): bins [N,B], weights [N,B-1], u [N or 1, n_samples]
  *      (u_row_stride 0 = the det linspace row shared by all rays) -> samples [N,n_samples] ------- */
@@ -213,8 +231,9 @@ int nerf_b200_render_rays_fwd_train(const float* rays, int64_t N, const NerfRend
 
 /* ---- backward of one network pass: what loss.backward() (run_nerf.py:775) does through
  *      run_nerf.py:381-386 / :397-403.  dL/dtheta is ACCUMULATED (+=) into fp32 grads laid out like the
- *      reference parameters; g_rgb [N,3] = dL/drgb_map (the only output the reference's loss reads,
- *      run_nerf.py:765-772); no gradient flows to rays or z (run_nerf.py:394). ---------------------------- */
+ *      reference parameters; g_rgb [N,3] = dL/drgb_map (the only output the reference's train() loss reads,
+ *      run_nerf.py:765-772; the _outs variants take the gradients of every output, NerfOutGrads); no gradient
+ *      flows to rays or z (run_nerf.py:394). ------------------------------------------------------------------ */
 typedef struct NerfNetGrads {
   float* pts_w[NERF_B200_MAX_D]; float* pts_b[NERF_B200_MAX_D];
   float* feature_w; float* feature_b; float* alpha_w; float* alpha_b;
@@ -229,6 +248,15 @@ int nerf_b200_march_bwd_tc(const float* rays, const float* z_vals, const float* 
                            const NerfNetParams* net, const void* packed, const NerfRenderCfg* cfg,
                            const float* raw, const NerfTrainSave* save, const float* g_rgb,
                            const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream);
+/* same with the gradients of every output of the pass (NerfOutGrads: rgb_map, disp_map, acc_map, depth_map, weights,
+ * raw).  The pass's power-of-two loss scale then comes from
+ *   amax = max( |g_rgb|, |g_acc_eff|, |g_depth_eff * z_k|, |g_weights|, |g_raw| )
+ * over the seeds given, where g_acc_eff / g_depth_eff include disp_map's chain rule; with only rgb_map given this is
+ * nerf_b200_march_bwd_tc (same kernels, same results). */
+int nerf_b200_march_bwd_tc_outs(const float* rays, const float* z_vals, const float* noise, int64_t N, int S,
+                                const NerfNetParams* net, const void* packed, const NerfRenderCfg* cfg,
+                                const float* raw, const NerfTrainSave* save, const NerfOutGrads* g,
+                                const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream);
 size_t nerf_b200_march_bwd_tc_workspace_bytes(int64_t N, int S, const NerfNetParams* net);
 /* introspection (tests / tools): offsets of the intermediates inside the 1 KB-aligned workspace and the tile plan:
  * out[12] = off_d_raw, off_grad_records, rec_act_bytes, rec_mask_bytes, rec_grad_bytes, grid, rays_per_cta, nst,
@@ -251,6 +279,11 @@ typedef struct {
 } NerfBwdPass;
 int nerf_b200_render_rays_bwd_tc(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse,
                                  const NerfBwdPass* fine, void* workspace, size_t workspace_bytes, void* stream);
+/* same with the gradients of every output of each pass (loss-scale rule of nerf_b200_march_bwd_tc_outs): a non-NULL
+ * coarse_g / fine_g replaces that pass's NerfBwdPass.g_rgb (which is then ignored). */
+int nerf_b200_render_rays_bwd_tc_outs(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse,
+                                      const NerfBwdPass* fine, const NerfOutGrads* coarse_g, const NerfOutGrads* fine_g,
+                                      void* workspace, size_t workspace_bytes, void* stream);
 size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, const NerfNetParams* net_coarse, int S_fine,
                                                     const NerfNetParams* net_fine);
 /* exact mode (csrc/bwd_simt.cuh): fp32 recompute with saved activations + fp32 CUDA-core GEMMs; any network
@@ -259,6 +292,11 @@ int nerf_b200_march_bwd(const float* rays, const float* z_vals, const float* noi
                         const NerfNetParams* net, const void* packed, const NerfRenderCfg* cfg,
                         const float* g_rgb, const NerfNetGrads* grads, void* workspace,
                         size_t workspace_bytes, void* stream);
+/* same with the gradients of every output of the pass (NerfOutGrads; nerf_b200_march_bwd is this call with rgb_map only) */
+int nerf_b200_march_bwd_outs(const float* rays, const float* z_vals, const float* noise, int64_t N, int S,
+                             const NerfNetParams* net, const void* packed, const NerfRenderCfg* cfg,
+                             const NerfOutGrads* g, const NerfNetGrads* grads, void* workspace,
+                             size_t workspace_bytes, void* stream);
 size_t nerf_b200_march_bwd_workspace_bytes(int64_t N, int S, const NerfNetParams* net);
 
 /* ---- the two ends of the optimisation step (SURVEY 8f rank 2; csrc/train_step.cuh) ------------------------------

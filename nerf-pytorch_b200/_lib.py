@@ -57,6 +57,10 @@ class NerfRayGen(C.Structure):
                 ("ndc", C.c_int32), ("use_viewdirs", C.c_int32), ("near", C.c_float), ("far", C.c_float)]
 
 
+class NerfOutGrads(C.Structure):
+    _fields_ = [("rgb_map", c_fp), ("disp_map", c_fp), ("acc_map", c_fp), ("depth_map", c_fp), ("weights", c_fp), ("raw", c_fp)]
+
+
 class NerfBwdPass(C.Structure):
     _fields_ = [("z_vals", c_fp), ("noise", c_fp), ("S", C.c_int), ("net", C.POINTER(NerfNetParams)), ("packed", c_fp), ("raw", c_fp),
                 ("save", C.POINTER(NerfTrainSave)), ("g_rgb", c_fp), ("grads", C.POINTER(NerfNetGrads))]
@@ -75,6 +79,8 @@ SIGNATURES = {
     "nerf_b200_raw2outputs": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, c_fp, C.c_int64, C.c_int, C.c_int,
                                         C.POINTER(NerfPassOut), c_fp]),
     "nerf_b200_raw2outputs_bwd": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, c_fp, C.c_int64, C.c_int, C.c_int, c_fp, c_fp, c_fp]),
+    "nerf_b200_raw2outputs_bwd_outs": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, c_fp, C.c_int64, C.c_int, C.c_int,
+                                                 C.POINTER(NerfOutGrads), c_fp, c_fp]),
     "nerf_b200_pack_rays": (C.c_int, [c_fp, c_fp, c_fp, C.POINTER(NerfCamera), C.c_int64, C.c_int64, C.c_int, C.c_float,
                                       C.c_float, C.c_int, c_fp, c_fp]),
     "nerf_b200_pack_rays_pixels": (C.c_int, [C.POINTER(NerfCamera), c_fp, C.c_int64, C.c_int, C.c_float, C.c_float, C.c_int, c_fp, c_fp]),
@@ -107,14 +113,23 @@ SIGNATURES = {
     "nerf_b200_march_bwd_tc": (C.c_int, [c_fp, c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp,
                                          C.POINTER(NerfRenderCfg), c_fp, C.POINTER(NerfTrainSave), c_fp,
                                          C.POINTER(NerfNetGrads), c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_march_bwd_tc_outs": (C.c_int, [c_fp, c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp,
+                                              C.POINTER(NerfRenderCfg), c_fp, C.POINTER(NerfTrainSave), C.POINTER(NerfOutGrads),
+                                              C.POINTER(NerfNetGrads), c_fp, C.c_size_t, c_fp]),
     "nerf_b200_march_bwd_tc_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.POINTER(NerfNetParams)]),
     "nerf_b200_march_bwd_tc_layout": (C.c_int, [C.c_int64, C.c_int, C.POINTER(NerfNetParams), C.POINTER(C.c_int64)]),
     "nerf_b200_render_rays_bwd_tc": (C.c_int, [c_fp, C.c_int64, C.POINTER(NerfRenderCfg), C.POINTER(NerfBwdPass), C.POINTER(NerfBwdPass),
                                                c_fp, C.c_size_t, c_fp]),
-    "nerf_b200_render_rays_bwd_tc_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.POINTER(NerfNetParams), C.c_int, C.POINTER(NerfNetParams)]),
+    "nerf_b200_render_rays_bwd_tc_outs": (C.c_int, [c_fp, C.c_int64, C.POINTER(NerfRenderCfg), C.POINTER(NerfBwdPass),
+                                                    C.POINTER(NerfBwdPass), C.POINTER(NerfOutGrads), C.POINTER(NerfOutGrads),
+                                                    c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_render_rays_bwd_tc_workspace_bytes":(C.c_size_t, [C.c_int64, C.c_int, C.POINTER(NerfNetParams), C.c_int, C.POINTER(NerfNetParams)]),
     "nerf_b200_march_bwd": (C.c_int, [c_fp, c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp,
                                       C.POINTER(NerfRenderCfg), c_fp, C.POINTER(NerfNetGrads), c_fp, C.c_size_t, c_fp]),
-    "nerf_b200_march_bwd_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.POINTER(NerfNetParams)]),
+    "nerf_b200_march_bwd_outs": (C.c_int, [c_fp, c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp,
+                                           C.POINTER(NerfRenderCfg), C.POINTER(NerfOutGrads), C.POINTER(NerfNetGrads), c_fp,
+                                           C.c_size_t, c_fp]),
+    "nerf_b200_march_bwd_workspace_bytes":(C.c_size_t, [C.c_int64, C.c_int, C.POINTER(NerfNetParams)]),
     "nerf_b200_mse_seed": (C.c_int, [c_fp, c_fp, C.c_int64, C.c_float, c_fp, c_fp, c_fp]),
     "nerf_b200_adam_step": (C.c_int, [c_fp, c_fp, c_fp, c_fp, C.c_int64, c_fp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
                                       C.c_float, C.c_float, c_fp]),

@@ -325,26 +325,36 @@ class _Raw2Outputs(torch.autograd.Function):
                                                     int(white_bkgd), C.byref(out), _stream(raw)), "raw2outputs")
         ctx.save_for_backward(raw, z_vals, rays_d, noise if noise is not None else torch.empty(0, device=dev))
         ctx.white_bkgd = bool(white_bkgd)
-        ctx.mark_non_differentiable(disp, acc, weights, depth)
+        ctx.set_materialize_grads(False)
         return rgb, disp, acc, weights, depth
 
     @staticmethod
-    def backward(ctx, g_rgb, *_):
+    def backward(ctx, g_rgb, g_disp, g_acc, g_weights, g_depth):
         raw, z_vals, rays_d, noise = ctx.saved_tensors
         noise = noise if noise.numel() else None
         N, S = z_vals.shape
         d_raw = torch.empty_like(raw)
-        g_rgb = g_rgb.contiguous().float()
+        lib = _lib.load()
+        args = (_ptr(raw), _ptr(z_vals), _ptr(rays_d), 3, _ptr(noise), N, S, int(ctx.white_bkgd))
         with _on(raw):
-            check(_lib.load().nerf_b200_raw2outputs_bwd(_ptr(raw), _ptr(z_vals), _ptr(rays_d), 3, _ptr(noise), N, S,
-                                                        int(ctx.white_bkgd), _ptr(g_rgb), _ptr(d_raw), _stream(raw)), "raw2outputs_bwd")
+            if g_disp is None and g_acc is None and g_weights is None and g_depth is None:
+                g_rgb = g_rgb.contiguous().float()
+                check(lib.nerf_b200_raw2outputs_bwd(*args, _ptr(g_rgb), _ptr(d_raw), _stream(raw)), "raw2outputs_bwd")
+            else:
+                og, keep = _out_grads(rgb_map=g_rgb, disp_map=g_disp, acc_map=g_acc, depth_map=g_depth, weights=g_weights)
+                check(lib.nerf_b200_raw2outputs_bwd_outs(*args, C.byref(og), _ptr(d_raw), _stream(raw)), "raw2outputs_bwd_outs")
         return d_raw, None, None, None, None
 
 
+def _out_grads(**seeds):
+    """NerfOutGrads over the given output gradients (None -> NULL) -> (struct, the contiguous fp32 tensors it points to)."""
+    keep = {k: v.contiguous().float() for k, v in seeds.items() if v is not None}
+    return _lib.NerfOutGrads(**{k: _ptr(v) for k, v in keep.items()}), keep
+
+
 def raw2outputs(raw, z_vals, rays_d, raw_noise_std=0, white_bkgd=False, pytest=False):
-    """-> rgb_map, disp_map, acc_map, weights, depth_map.  Gradient flows to `raw` through rgb_map
-    (the only output the reference's loss reads, run_nerf.py:765-772); the other outputs are
-    returned non-differentiable."""
+    """-> rgb_map, disp_map, acc_map, weights, depth_map, all differentiable w.r.t. `raw` as in the reference
+    (nerf_b200_raw2outputs_bwd_outs; a loss on rgb_map alone takes nerf_b200_raw2outputs_bwd)."""
     raw, z_vals, rays_d = _f32c(raw, "raw"), _f32c(z_vals, "z_vals"), _f32c(rays_d, "rays_d")
     if raw.shape[-1] != 4:
         raw = raw[..., :4].contiguous()
@@ -497,9 +507,10 @@ class _RenderRays(torch.autograd.Function):
     """Forward: nerf_b200_render_rays_fwd (coarse z -> fused pass -> resample -> fused pass); when a parameter needs a
     gradient and the tensor-core backward is selected, the training-mode variant that also leaves the per-tile
     activation records.  Backward: per pass nerf_b200_march_bwd_tc (wgmma dgrad chain + layer-major wgrad from
-    those records) or, in exact mode, nerf_b200_march_bwd (fp32 recompute + GEMM backprop).  Gradients w.r.t. rgb_map
-    and rgb0 only -- exactly the terms of the reference's loss (run_nerf.py:765-772); z_samples is detached in the
-    reference (:394) so nothing flows through the resampling."""
+    those records) or, in exact mode, nerf_b200_march_bwd (fp32 recompute + GEMM backprop).  Every output but z_std
+    carries a gradient, as in the reference: a loss on rgb_map / rgb0 alone (run_nerf.py:765-772) takes those entry
+    points, a loss that also reads disp, acc, disp0, acc0 or raw takes their _outs variants (NerfOutGrads seeds per
+    pass).  z_samples is detached in the reference (:394) so nothing flows through the resampling."""
 
     @staticmethod
     def forward(ctx, ray_batch, cfgd, net_c, net_f, t_rand, u_rand, noise0, noise1, *params):
@@ -564,15 +575,18 @@ class _RenderRays(torch.autograd.Function):
             ctx.save_for_backward(ray_batch, z_c, z_f if fine else torch.empty(0, device=dev),
                                   noise0 if noise0 is not None else torch.empty(0, device=dev),
                                   noise1 if noise1 is not None else torch.empty(0, device=dev), *saved_rec)
+        # as in the reference every map and raw carry a gradient; z_std does not (z_samples is detached, :394)
         if fine:
             rets = (o["rgb"], o["disp"], o["acc"], o["rgb0"], o["disp0"], o["acc0"], z_std,
                     raw_f if retraw else torch.empty(0, device=dev))
             if ctx is not None:
-                ctx.mark_non_differentiable(o["disp"], o["acc"], o["disp0"], o["acc0"], z_std, rets[7])
+                ctx.mark_non_differentiable(z_std, *(() if retraw else (rets[7],)))
         else:
             rets = (o["rgb0"], o["disp0"], o["acc0"], raw_c if retraw else torch.empty(0, device=dev))
-            if ctx is not None:
-                ctx.mark_non_differentiable(o["disp0"], o["acc0"], rets[3])
+            if ctx is not None and not retraw:
+                ctx.mark_non_differentiable(rets[3])
+        if ctx is not None:
+            ctx.set_materialize_grads(False)
         return rets
 
     @staticmethod
@@ -580,18 +594,98 @@ class _RenderRays(torch.autograd.Function):
         lib = _lib.load()
         ray_batch, z_c, z_f, noise0, noise1 = ctx.saved_tensors[:5]
         rec = ctx.saved_tensors[5:]
-        cfgd = ctx.cfgd
-        net_c, net_f = ctx.nets
-        fine = cfgd["N_importance"] > 0
+        fine = ctx.cfgd["N_importance"] > 0
         N = ray_batch.shape[0]
-        cfg = _cfg_struct(cfgd, ray_batch.shape[1])
-        g_fine, g_coarse = (g[0], g[3]) if fine else (None, g[0])
+        cfg = _cfg_struct(ctx.cfgd, ray_batch.shape[1])
+        # seeds per pass: fine <- rgb, disp, acc, raw;  coarse <- rgb0, disp0, acc0 (and raw without fine samples)
+        if fine:
+            s_fine = dict(rgb_map=g[0], disp_map=g[1], acc_map=g[2], raw=g[7])
+            s_coarse = dict(rgb_map=g[3], disp_map=g[4], acc_map=g[5])
+        else:
+            s_fine, s_coarse = {}, dict(rgb_map=g[0], disp_map=g[1], acc_map=g[2], raw=g[3])
+        extra = any(v is not None for s in (s_fine, s_coarse) for k, v in s.items() if k != "rgb_map")
+        if not extra:
+            # rgb / rgb0 only: the entry points (and the zero gradient of an unused rgb output) of the rgb-only backward
+            g_fine = None
+            if fine:
+                g_fine = s_fine["rgb_map"] if s_fine["rgb_map"] is not None else torch.zeros((N, 3), device=ray_batch.device)
+                g_coarse = s_coarse["rgb_map"] if s_coarse["rgb_map"] is not None else torch.zeros((N, 3), device=ray_batch.device)
+            else:
+                g_coarse = s_coarse["rgb_map"]
+            return _RenderRays._backward_rgb(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg, g_fine, g_coarse)
+        return _RenderRays._backward_outs(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg,
+                                          s_fine if fine else None, s_coarse)
+
+    @staticmethod
+    def _passes(ctx, z_c, z_f, noise0, noise1, rec, seed_f, seed_c):
+        """[(seed, z, noise, net, grad buffers, records)] of the coarse and (with fine samples) the fine pass, and the parameter
+        gradients autograd receives."""
+        net_c, net_f = ctx.nets
+        fine = ctx.cfgd["N_importance"] > 0
         grads_c = _grad_buffers(net_c)
         same_net = fine and (net_f is None)
         grads_f = grads_c if same_net else (_grad_buffers(net_f) if fine else None)
-        passes = [(g_coarse, z_c, noise0, net_c, grads_c, rec[0:3])]
+        passes = [(seed_c, z_c, noise0, net_c, grads_c, rec[0:3])]
         if fine:
-            passes.append((g_fine, z_f, noise1, net_c if same_net else net_f, grads_f, rec[3:6]))
+            passes.append((seed_f, z_f, noise1, net_c if same_net else net_f, grads_f, rec[3:6]))
+        out = [None] * 8
+        out += [grads_c[k] for _, _, k, _ in net_c._named_params()]
+        if net_f is not None:
+            out += [grads_f[k] for _, _, k, _ in net_f._named_params()]
+        return passes, tuple(out)
+
+    @staticmethod
+    def _backward_outs(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg, s_fine, s_coarse):
+        """Backward from the gradients of any of the outputs (NerfOutGrads per pass): the _outs entry points.  A pass runs
+        when any of its seeds is present."""
+        N = ray_batch.shape[0]
+        og_f = _out_grads(**s_fine) if s_fine is not None and any(v is not None for v in s_fine.values()) else None
+        og_c = _out_grads(**s_coarse) if any(v is not None for v in s_coarse.values()) else None
+        passes, out = _RenderRays._passes(ctx, z_c, z_f, noise0, noise1, rec, og_f, og_c)
+        with _on(ray_batch):
+            if ctx.train_tc and og_f is not None and og_c is not None:
+                keep, bp = [], []
+                for (og, _), z, noise, net, gbuf, rc in passes:
+                    raw, act, mask = rc
+                    n, gs = net.net_params(), net.grad_struct(gbuf)
+                    sv = NerfTrainSave(_ptr(act), act.numel(), _ptr(mask), mask.numel())
+                    keep += [n, gs, sv]
+                    bp.append(_lib.NerfBwdPass(_ptr(z), _ptr(noise if noise.numel() else None), z.shape[1], C.pointer(n), _ptr(net.packed()),
+                                               _ptr(raw), C.pointer(sv), _ptr(None), C.pointer(gs)))
+                ws_bytes = lib.nerf_b200_render_rays_bwd_tc_workspace_bytes(N, bp[0].S, bp[0].net, bp[1].S, bp[1].net)
+                ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=ray_batch.device)
+                check(lib.nerf_b200_render_rays_bwd_tc_outs(_ptr(ray_batch), N, C.byref(cfg), C.byref(bp[0]), C.byref(bp[1]),
+                                                            C.byref(og_c[0]), C.byref(og_f[0]), _ptr(ws), ws_bytes, _stream(ray_batch)),
+                      "render_rays_bwd_tc_outs")
+                return out
+            for og, z, noise, net, gbuf, rc in passes:
+                if og is None:
+                    continue
+                S = z.shape[1]
+                n = net.net_params()
+                gs = net.grad_struct(gbuf)
+                nz = _ptr(noise if noise.numel() else None)
+                if ctx.train_tc:
+                    raw, act, mask = rc
+                    sv = NerfTrainSave(_ptr(act), act.numel(), _ptr(mask), mask.numel())
+                    ws_bytes = lib.nerf_b200_march_bwd_tc_workspace_bytes(N, S, C.byref(n))
+                    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=z.device)
+                    check(lib.nerf_b200_march_bwd_tc_outs(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(net.packed()), C.byref(cfg),
+                                                          _ptr(raw), C.byref(sv), C.byref(og[0]), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)),
+                          "march_bwd_tc_outs")
+                else:
+                    ws_bytes = lib.nerf_b200_march_bwd_workspace_bytes(N, S, C.byref(n))
+                    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=z.device)
+                    check(lib.nerf_b200_march_bwd_outs(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(None), C.byref(cfg),
+                                                       C.byref(og[0]), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)), "march_bwd_outs")
+        return out
+
+    @staticmethod
+    def _backward_rgb(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg, g_fine, g_coarse):
+        """Backward from dL/drgb_map (and dL/drgb0) alone: nerf_b200_render_rays_bwd_tc / march_bwd_tc / march_bwd."""
+        N = ray_batch.shape[0]
+        fine = ctx.cfgd["N_importance"] > 0
+        passes, out = _RenderRays._passes(ctx, z_c, z_f, noise0, noise1, rec, g_fine, g_coarse)
         with _on(ray_batch):
             if ctx.train_tc and fine and g_fine is not None and g_coarse is not None:
                 # both passes in one call: the chain of one pass runs next to the weight gradient of the other (capi.cu)
@@ -629,11 +723,7 @@ class _RenderRays(torch.autograd.Function):
                     ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=z.device)
                     check(lib.nerf_b200_march_bwd(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(None), C.byref(cfg),
                                                   _ptr(g_rgb), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)), "march_bwd")
-        out = [None] * 8
-        out += [grads_c[k] for _, _, k, _ in net_c._named_params()]
-        if net_f is not None:
-            out += [grads_f[k] for _, _, k, _ in net_f._named_params()]
-        return tuple(out)
+        return out
 
 
 def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False, lindisp=False, perturb=0.,

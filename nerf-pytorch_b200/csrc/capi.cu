@@ -285,17 +285,63 @@ int nerf_b200_raw2outputs(const float* raw, const float* z_vals, const float* ra
   return 0;
 }
 
-int nerf_b200_raw2outputs_bwd(const float* raw, const float* z_vals, const float* rays_d, int d_stride, const float* noise,
-                              int64_t N, int S, int white_bkgd, const float* g_rgb, float* d_raw, void* stream) {
-  NB_CHECK_ARG(raw && z_vals && rays_d && g_rgb && d_raw, "NULL pointer");
+}  // extern "C"
+
+static NerfOutGrads rgb_seed(const float* g_rgb) {
+  NerfOutGrads g;
+  memset(&g, 0, sizeof(g));
+  g.rgb_map = g_rgb;
+  return g;
+}
+static bool seeds_rgb_only(const NerfOutGrads& g) { return !(g.disp_map || g.acc_map || g.depth_map || g.weights || g.raw); }
+static bool seeds_none(const NerfOutGrads& g) { return !g.rgb_map && seeds_rgb_only(g); }
+// the seeds of rays [n0, n0 + nn) of a pass with S samples per ray
+static NerfOutGrads seeds_at(const NerfOutGrads& g, int64_t n0, int S) {
+  NerfOutGrads o = g;
+  const long long nS = n0 * (long long)S;
+  if (o.rgb_map) o.rgb_map += n0 * 3;
+  if (o.disp_map) o.disp_map += n0;
+  if (o.acc_map) o.acc_map += n0;
+  if (o.depth_map) o.depth_map += n0;
+  if (o.weights) o.weights += nS;
+  if (o.raw) o.raw += nS * 4;
+  return o;
+}
+
+// the compositing adjoint for any set of seeds.  rgb_map alone without `amax`: the rgb-only instantiation (the library's
+// original arithmetic); otherwise the seeded one, which with `amax` also forms the loss-scale input of the pass.
+static int raw2outputs_bwd_impl(const float* raw, const float* z_vals, const float* rays_d, int d_stride, const float* noise,
+                                int64_t N, int S, int white_bkgd, const NerfOutGrads& g, unsigned int* amax, float* d_raw,
+                                cudaStream_t st) {
+  NB_CHECK_ARG(raw && z_vals && rays_d && d_raw, "NULL pointer");
+  NB_CHECK_ARG(!seeds_none(g), "no output gradient given (every NerfOutGrads member is NULL)");
   NB_CHECK_ARG(S >= 1 && S <= 1024, "S must be in [1,1024]");
   if (N == 0) return 0;
   const int wpb = 4;
   const size_t sm = (size_t)wpb * 4 * S * sizeof(float);
-  if (int rc = smem_optin((const void*)raw2outputs_bwd_kernel, sm)) return rc;
-  raw2outputs_bwd_kernel<<<cdiv(N, wpb), wpb * 32, sm, (cudaStream_t)stream>>>(raw, z_vals, rays_d, d_stride, noise, N, S, white_bkgd, g_rgb, d_raw);
+  R2OSeeds s = {g.rgb_map, g.disp_map, g.acc_map, g.depth_map, g.weights, g.raw, amax};
+  if (seeds_rgb_only(g) && !amax) {
+    if (int rc = smem_optin((const void*)raw2outputs_bwd_kernel<false>, sm)) return rc;
+    raw2outputs_bwd_kernel<false><<<cdiv(N, wpb), wpb * 32, sm, st>>>(raw, z_vals, rays_d, d_stride, noise, N, S, white_bkgd, s, d_raw);
+  } else {
+    if (int rc = smem_optin((const void*)raw2outputs_bwd_kernel<true>, sm)) return rc;
+    raw2outputs_bwd_kernel<true><<<cdiv(N, wpb), wpb * 32, sm, st>>>(raw, z_vals, rays_d, d_stride, noise, N, S, white_bkgd, s, d_raw);
+  }
   NB_LAUNCH_OK("raw2outputs_bwd_kernel");
   return 0;
+}
+
+extern "C" {
+
+int nerf_b200_raw2outputs_bwd(const float* raw, const float* z_vals, const float* rays_d, int d_stride, const float* noise,
+                              int64_t N, int S, int white_bkgd, const float* g_rgb, float* d_raw, void* stream) {
+  return raw2outputs_bwd_impl(raw, z_vals, rays_d, d_stride, noise, N, S, white_bkgd, rgb_seed(g_rgb), nullptr, d_raw, (cudaStream_t)stream);
+}
+
+int nerf_b200_raw2outputs_bwd_outs(const float* raw, const float* z_vals, const float* rays_d, int d_stride, const float* noise,
+                                   int64_t N, int S, int white_bkgd, const NerfOutGrads* g, float* d_raw, void* stream) {
+  NB_CHECK_ARG(g, "NULL pointer");
+  return raw2outputs_bwd_impl(raw, z_vals, rays_d, d_stride, noise, N, S, white_bkgd, *g, nullptr, d_raw, (cudaStream_t)stream);
 }
 
 static int fill_pack_args(PackRaysArgs& a, const float* rays_o, const float* rays_d, const float* view_src, const NerfCamera* cam, int64_t N,
@@ -582,11 +628,11 @@ static int mask_colsum(float* d, int ldd, const float* h, int ldh, long long M, 
 }
 #define NB_TRY(expr) do { if (int rc__ = (expr)) return rc__; } while (0)
 
-int nerf_b200_march_bwd(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
-                        const void* packed, const NerfRenderCfg* cfg, const float* g_rgb, const NerfNetGrads* grads,
-                        void* workspace, size_t workspace_bytes, void* stream) {
-  (void)packed;
-  NB_CHECK_ARG(rays && z_vals && net && cfg && g_rgb && grads, "NULL pointer");
+static int march_bwd_impl(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                          const NerfRenderCfg* cfg, const NerfOutGrads& g, const NerfNetGrads* grads,
+                          void* workspace, size_t workspace_bytes, void* stream) {
+  NB_CHECK_ARG(rays && z_vals && net && cfg && grads, "NULL pointer");
+  NB_CHECK_ARG(!seeds_none(g), "no output gradient given (every NerfOutGrads member is NULL)");
   NB_CHECK_ARG(net->W <= SIMT_THREADS && net->W % 4 == 0 && net->D <= NERF_B200_MAX_D, "unsupported network shape");
   if (N == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
@@ -620,7 +666,7 @@ int nerf_b200_march_bwd(const float* rays, const float* z_vals, const float* noi
     mlp_simt_kernel<<<cdiv(M, SIMT_ROWS), SIMT_THREADS, sm, st>>>(pts, net->use_viewdirs ? ry + 8 : nullptr, rs, M, S, *net, cfg->multires, cfg->multires_views, raw, sv);
     NB_LAUNCH_OK("mlp_simt_kernel");
     // 2. compositing adjoint -> dL/draw
-    NB_TRY(nerf_b200_raw2outputs_bwd(raw, zz, ry + 3, rs, nz, nn, S, cfg->white_bkgd, g_rgb + n0 * 3, d_raw, stream));
+    NB_TRY(raw2outputs_bwd_impl(raw, zz, ry + 3, rs, nz, nn, S, cfg->white_bkgd, seeds_at(g, n0, S), nullptr, d_raw, st));
     const float* h_last = sv.h + (size_t)(D - 1) * M * W;
     if (net->use_viewdirs) {
       // 3. rgb_linear (run_nerf_helpers.py:114)
@@ -665,6 +711,21 @@ int nerf_b200_march_bwd(const float* rays, const float* z_vals, const float* noi
     }
   }
   return 0;
+}
+
+int nerf_b200_march_bwd(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                        const void* packed, const NerfRenderCfg* cfg, const float* g_rgb, const NerfNetGrads* grads,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  (void)packed;
+  return march_bwd_impl(rays, z_vals, noise, N, S, net, cfg, rgb_seed(g_rgb), grads, workspace, workspace_bytes, stream);
+}
+
+int nerf_b200_march_bwd_outs(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                             const void* packed, const NerfRenderCfg* cfg, const NerfOutGrads* g, const NerfNetGrads* grads,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+  (void)packed;
+  NB_CHECK_ARG(g, "NULL pointer");
+  return march_bwd_impl(rays, z_vals, noise, N, S, net, cfg, *g, grads, workspace, workspace_bytes, stream);
 }
 
 // ---- tensor-core backward of one pass (bwd_wg.cuh) ------------------------------------------------
@@ -784,7 +845,7 @@ namespace {
 // weight gradients, view-column gradients.
 struct BwdTcPass {
   const float* rays; const float* z; const float* noise; int64_t N; int S; const NerfNetParams* net; const void* packed;
-  const NerfRenderCfg* cfg; const float* raw; const NerfTrainSave* save; const float* g_rgb; const NerfNetGrads* grads;
+  const NerfRenderCfg* cfg; const float* raw; const NerfTrainSave* save; NerfOutGrads seeds; const NerfNetGrads* grads;
   DeviceState* ds; TilePlan plan; BwdTcLayout LY; PackLayout PL;
   unsigned int* amax; float *d_raw, *encv, *dsum, *gv, *dbv, *partial; uint8_t* grec; const uint8_t *act, *mask;
 
@@ -815,8 +876,9 @@ struct BwdTcPass {
     return 0;
   }
 
-  // 1. loss scale from max |dL/drgb_map|; compositing adjoint -> dL/draw (SURVEY App. E);  2. seed of the chain: d_hv tiles, or
-  // without view directions dA_{D-1} tiles (+ output_linear's gradient)
+  // 1. compositing adjoint -> dL/draw (SURVEY App. E) and the loss scale: from max |dL/drgb_map| (absmax_kernel) when rgb_map
+  // is the only seed, else from the adjoint's max over all effective seeds;  2. seed of the chain: d_hv tiles, or
+  // without view directions dA_{D-1} tiles (+ output_linear's gradient).  Both read amax after the adjoint, on the same stream.
   int prologue(cudaStream_t st) {
     const int sms = ds->sms, D = net->D;
     NB_CUDA(cudaMemsetAsync(amax, 0, 256, st));
@@ -824,9 +886,13 @@ struct BwdTcPass {
       NB_CUDA(cudaMemsetAsync(dsum, 0, (size_t)N * 128 * 4, st));
       NB_CUDA(cudaMemsetAsync(gv, 0, (size_t)(128 * 256 + 128) * 4, st));
     }
-    absmax_kernel<<<cdiv(N * 3, 1024) < 64 ? cdiv(N * 3, 1024) : 64, 256, 0, st>>>(g_rgb, N * 3, amax);
-    NB_LAUNCH_OK("absmax_kernel");
-    NB_TRY(nerf_b200_raw2outputs_bwd(raw, z, rays + 3, cfg->ray_stride, noise, N, S, cfg->white_bkgd, g_rgb, d_raw, (void*)st));
+    if (seeds_rgb_only(seeds)) {
+      absmax_kernel<<<cdiv(N * 3, 1024) < 64 ? cdiv(N * 3, 1024) : 64, 256, 0, st>>>(seeds.rgb_map, N * 3, amax);
+      NB_LAUNCH_OK("absmax_kernel");
+      NB_TRY(raw2outputs_bwd_impl(raw, z, rays + 3, cfg->ray_stride, noise, N, S, cfg->white_bkgd, seeds, nullptr, d_raw, st));
+    } else {
+      NB_TRY(raw2outputs_bwd_impl(raw, z, rays + 3, cfg->ray_stride, noise, N, S, cfg->white_bkgd, seeds, amax, d_raw, st));
+    }
     if (!net->use_viewdirs) {
       SeedOutParams so;
       so.d_raw = d_raw; so.mask = mask; so.act = act; so.grad = grec; so.out_w = net->output_w; so.amax = amax;
@@ -936,38 +1002,55 @@ struct BwdTcPass {
   }
 };
 
-int check_bwd_pass(const float* rays, const NerfBwdPass* q, const NerfRenderCfg* cfg) {
-  NB_CHECK_ARG(rays && q && q->z_vals && q->net && q->packed && cfg && q->raw && q->save && q->g_rgb && q->grads, "NULL pointer");
+// q's seeds: `g` when given, else {rgb_map = q->g_rgb}
+NerfOutGrads pass_seeds(const NerfBwdPass* q, const NerfOutGrads* g) { return g ? *g : rgb_seed(q->g_rgb); }
+
+int check_bwd_pass(const float* rays, const NerfBwdPass* q, const NerfRenderCfg* cfg, const NerfOutGrads* g) {
+  NB_CHECK_ARG(rays && q && q->z_vals && q->net && q->packed && cfg && q->raw && q->save && q->grads, "NULL pointer");
+  NB_CHECK_ARG(!seeds_none(pass_seeds(q, g)), "no output gradient given for a backward pass (g_rgb / every NerfOutGrads member is NULL)");
   if (int rc = check_tc_net(q->net)) return rc;
   NB_CHECK_ARG(q->net->use_viewdirs || q->net->output_ch >= 4, "output_linear needs output_ch >= 4 (got %d)", q->net->output_ch);
   NB_CHECK_ARG(q->net->W == 256, "the tensor-core backward supports netwidth == 256");
   NB_CHECK_ARG(q->S > 0, "S must be positive");
   return 0;
 }
-BwdTcPass bind_pass(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* q) {
+BwdTcPass bind_pass(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* q, const NerfOutGrads* g) {
   BwdTcPass b;
   memset(&b, 0, sizeof(b));
   b.rays = rays; b.z = q->z_vals; b.noise = q->noise; b.N = N; b.S = q->S; b.net = q->net; b.packed = q->packed; b.cfg = cfg;
-  b.raw = q->raw; b.save = q->save; b.g_rgb = q->g_rgb; b.grads = q->grads;
+  b.raw = q->raw; b.save = q->save; b.seeds = pass_seeds(q, g); b.grads = q->grads;
   return b;
 }
-}  // namespace
 
-int nerf_b200_march_bwd_tc(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
-                           const void* packed, const NerfRenderCfg* cfg, const float* raw, const NerfTrainSave* save,
-                           const float* g_rgb, const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
+int march_bwd_tc_impl(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                      const void* packed, const NerfRenderCfg* cfg, const float* raw, const NerfTrainSave* save,
+                      const NerfOutGrads& g, const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
   NerfBwdPass q;
-  q.z_vals = z_vals; q.noise = noise; q.S = S; q.net = net; q.packed = packed; q.raw = raw; q.save = save; q.g_rgb = g_rgb; q.grads = grads;
-  if (int rc = check_bwd_pass(rays, &q, cfg)) return rc;
+  q.z_vals = z_vals; q.noise = noise; q.S = S; q.net = net; q.packed = packed; q.raw = raw; q.save = save; q.g_rgb = g.rgb_map; q.grads = grads;
+  if (int rc = check_bwd_pass(rays, &q, cfg, &g)) return rc;
   if (N == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  BwdTcPass b = bind_pass(rays, N, cfg, &q);
+  BwdTcPass b = bind_pass(rays, N, cfg, &q, &g);
   NB_TRY(b.init(workspace, workspace_bytes));
   NB_TRY(b.prologue(st));
   NB_TRY(b.dgrad(st));
   NB_TRY(b.wgrad(st));
   NB_TRY(b.heads(st));
   return 0;
+}
+}  // namespace
+
+int nerf_b200_march_bwd_tc(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                           const void* packed, const NerfRenderCfg* cfg, const float* raw, const NerfTrainSave* save,
+                           const float* g_rgb, const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
+  return march_bwd_tc_impl(rays, z_vals, noise, N, S, net, packed, cfg, raw, save, rgb_seed(g_rgb), grads, workspace, workspace_bytes, stream);
+}
+
+int nerf_b200_march_bwd_tc_outs(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                                const void* packed, const NerfRenderCfg* cfg, const float* raw, const NerfTrainSave* save,
+                                const NerfOutGrads* g, const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
+  NB_CHECK_ARG(g, "NULL pointer");
+  return march_bwd_tc_impl(rays, z_vals, noise, N, S, net, packed, cfg, raw, save, *g, grads, workspace, workspace_bytes, stream);
 }
 
 size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, const NerfNetParams* net_coarse, int S_fine, const NerfNetParams* net_fine) {
@@ -983,24 +1066,36 @@ size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, con
 // Backward of both passes of render_rays (run_nerf.py:765-772: loss = img2mse(rgb) + img2mse(rgb0); z_samples is detached, :394,
 // so the passes are independent): one pass after the other on `stream`.  The weight-gradient kernel holds a whole SM (384 threads
 // x 168 registers), so nothing of the other pass could run beside it.
-int nerf_b200_render_rays_bwd_tc(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse, const NerfBwdPass* fine,
-                                 void* workspace, size_t workspace_bytes, void* stream) {
-  if (int rc = check_bwd_pass(rays, coarse, cfg)) return rc;
-  if (fine) if (int rc = check_bwd_pass(rays, fine, cfg)) return rc;
+static int render_rays_bwd_tc_impl(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse, const NerfBwdPass* fine,
+                                   const NerfOutGrads* coarse_g, const NerfOutGrads* fine_g, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+  if (int rc = check_bwd_pass(rays, coarse, cfg, coarse_g)) return rc;
+  if (fine) if (int rc = check_bwd_pass(rays, fine, cfg, fine_g)) return rc;
   NB_CHECK_ARG(!fine || (fine->net->use_viewdirs != 0) == (coarse->net->use_viewdirs != 0),
                "coarse and fine networks must agree on use_viewdirs (they share one ray batch)");
   if (N == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  BwdTcPass c = bind_pass(rays, N, cfg, coarse);
+  BwdTcPass c = bind_pass(rays, N, cfg, coarse, coarse_g);
   const size_t cb = bwd_pass_bytes(N, coarse->S, coarse->net);
   NB_CHECK_ARG(workspace && workspace_bytes >= cb, "render_rays_bwd_tc workspace too small");
   NB_TRY(c.init(workspace, cb));
   NB_TRY(c.prologue(st)); NB_TRY(c.dgrad(st)); NB_TRY(c.wgrad(st)); NB_TRY(c.heads(st));
   if (!fine) return 0;
-  BwdTcPass f = bind_pass(rays, N, cfg, fine);
+  BwdTcPass f = bind_pass(rays, N, cfg, fine, fine_g);
   NB_TRY(f.init(static_cast<uint8_t*>(workspace) + cb, workspace_bytes - cb));
   NB_TRY(f.prologue(st)); NB_TRY(f.dgrad(st)); NB_TRY(f.wgrad(st)); NB_TRY(f.heads(st));
   return 0;
+}
+
+int nerf_b200_render_rays_bwd_tc(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse, const NerfBwdPass* fine,
+                                 void* workspace, size_t workspace_bytes, void* stream) {
+  return render_rays_bwd_tc_impl(rays, N, cfg, coarse, fine, nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
+int nerf_b200_render_rays_bwd_tc_outs(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse, const NerfBwdPass* fine,
+                                      const NerfOutGrads* coarse_g, const NerfOutGrads* fine_g, void* workspace, size_t workspace_bytes,
+                                      void* stream) {
+  return render_rays_bwd_tc_impl(rays, N, cfg, coarse, fine, coarse_g, fine_g, workspace, workspace_bytes, stream);
 }
 
 // ---- the two ends of the optimisation step (train_step.cuh) ------------------------------------------

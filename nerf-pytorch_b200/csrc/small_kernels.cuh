@@ -197,12 +197,39 @@ __global__ void raw2outputs_kernel(const float* __restrict__ raw, const float* _
   }
 }
 
-// Adjoint of raw2outputs w.r.t. raw, given g = dL/drgb_map (SURVEY Appendix E).  One warp per ray,
-// per-warp scratch of 4*S floats in dynamic shared memory.
+// Seeds of the compositing adjoint: dL/d(each output of raw2outputs), as in include/nerf_b200.h's NerfOutGrads.  Any
+// pointer may be NULL (that output does not reach the loss).  amax: see raw2outputs_bwd_kernel.
+struct R2OSeeds {
+  const float* rgb;        // [N,3]
+  const float* disp;       // [N]
+  const float* acc;        // [N]
+  const float* depth;      // [N]
+  const float* weights;    // [N,S]
+  const float* raw;        // [N,S,4]
+  unsigned int* amax;      // NULL, or max |effective seed| as a float bit pattern (atomicMax, zeroed by the caller)
+};
+
+// NaN-propagating max of |v| (absmax_kernel's rule: non-negative floats order like their bit patterns)
+__device__ __forceinline__ float absmax_step(float m, float v) { v = fabsf(v); return (v > m || v != v) ? v : m; }
+
+// Adjoint of raw2outputs w.r.t. raw (SURVEY Appendix E).  One warp per ray, per-warp scratch of 4*S floats in dynamic
+// shared memory.  With e_k = dL/dw_k, dL/dalpha_k = T_k e_k - sum_{j>k} w_j e_j / q_k; every seed reaches raw through e_k:
+//   rgb:     e_k += sum_c g_c (c_k - off)           (off = 1 with a white background: rgb_map += 1 - acc)
+//   acc:     e_k += g_acc          depth: e_k += g_depth z_k          weights: e_k += g_w[k]
+//   disp  =  1 / max(1e-10, depth / acc)  (run_nerf.py:299) becomes acc and depth seeds; the ray's depth and acc are
+//            RECOMPUTED here from raw with composite_chunk, the order of raw2outputs_kernel.  Like the reference's autograd:
+//            no gradient where depth/acc < 1e-10, half of it at equality (torch.max's tie rule), NaN where acc = 0.
+//   raw:     added to dL/draw.
+// kSeeds = false is the rgb-only adjoint (g.rgb required, everything else ignored): its arithmetic is the one the library
+// always had.  kSeeds = true branches on the NULLs; with g.amax it also forms the pass's loss-scale input
+//   amax = max( |g_rgb|, |g_acc_eff|, |g_depth_eff z_k|, |g_w|, |g_raw| )   (only over the seeds given)
+// which with g_rgb alone equals absmax_kernel's max |g_rgb|.  Rays with acc = 0 under a disp seed are left out of the
+// acc / depth terms: their NaN reaches dL/draw only where the density is > 0, and must not reset the whole pass's scale.
+template <bool kSeeds>
 __global__ void raw2outputs_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z_vals,
                                        const float* __restrict__ rays_d, int d_stride,
                                        const float* __restrict__ noise, long long N, int S, int white_bkgd,
-                                       const float* __restrict__ g_rgb, float* __restrict__ d_raw) {
+                                       const R2OSeeds g, float* __restrict__ d_raw) {
   extern __shared__ float smem[];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   long long n = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -213,12 +240,49 @@ __global__ void raw2outputs_bwd_kernel(const float* __restrict__ raw, const floa
   float* sF = sQ + S;                          // dist * (1-alpha) * [s>0]
   const float dx = rays_d[n * d_stride], dy = rays_d[n * d_stride + 1], dz = rays_d[n * d_stride + 2];
   const float norm = sqrtf(dx * dx + dy * dy + dz * dz);
-  const float gr = g_rgb[n * 3], gg = g_rgb[n * 3 + 1], gb = g_rgb[n * 3 + 2];
+  const bool has_rgb = !kSeeds || g.rgb != nullptr;
+  float gr = 0.f, gg = 0.f, gb = 0.f;
+  if (has_rgb) { gr = g.rgb[n * 3]; gg = g.rgb[n * 3 + 1]; gb = g.rgb[n * 3 + 2]; }
+  float g_acc = 0.f, g_depth = 0.f, m = 0.f;   // effective per-ray acc / depth seeds; running max for g.amax
+  bool disp_nan = false;                       // acc = 0 with a disp seed: g_acc / g_depth are NaN on this ray
+  if constexpr (kSeeds) {
+    if (g.acc) g_acc = g.acc[n];
+    if (g.depth) g_depth = g.depth[n];
+    if (g.disp) {
+      CompositeAcc a = {0, 0, 0, 0, 0, 1.0f};
+      for (int base = 0; base < S; base += 32) {
+        int k = base + lane;
+        bool valid = k < S;
+        float alpha = 0, z = 0;
+        if (valid) {
+          z = z_vals[n * S + k];
+          float dist = (k == S - 1) ? 1e10f : __fsub_rn(z_vals[n * S + k + 1], z);
+          dist = __fmul_rn(dist, norm);
+          float s = raw[(n * S + k) * 4 + 3] + (noise ? noise[n * S + k] : 0.0f);
+          alpha = __fsub_rn(1.0f, expf(-fmaxf(s, 0.0f) * dist));
+        }
+        composite_chunk(alpha, 0.f, 0.f, 0.f, z, valid, lane, a);
+      }
+      const float depth = warp_sum(a.depth), acc = warp_sum(a.acc);
+      const float ratio = depth / acc;
+      const float mx = (ratio != ratio) ? ratio : fmaxf(1e-10f, ratio);
+      float g_ratio = -g.disp[n] / (mx * mx);                         // d(1/mx)/dmx
+      if (ratio < 1e-10f) g_ratio = 0.f; else if (ratio == 1e-10f) g_ratio *= 0.5f;
+      g_depth += g_ratio / acc;
+      g_acc -= g_ratio * depth / (acc * acc);
+      disp_nan = ratio != ratio;
+    }
+    if (g.amax) {
+      if (has_rgb) { m = absmax_step(m, gr); m = absmax_step(m, gg); m = absmax_step(m, gb); }
+      if ((g.acc || g.disp) && !disp_nan) m = absmax_step(m, g_acc);
+    }
+  }
   float carryT = 1.0f;
   for (int base = 0; base < S; base += 32) {
     int k = base + lane;
     bool valid = k < S;
     float q = 1.0f, alpha = 0, e = 0, f = 0, cr = 0, cg = 0, cb = 0;
+    float4 gw4 = make_float4(0.f, 0.f, 0.f, 0.f);                  // dL/draw seed of this sample
     if (valid) {
       float4 r4 = reinterpret_cast<const float4*>(raw)[n * S + k];
       float z = z_vals[n * S + k];
@@ -230,7 +294,24 @@ __global__ void raw2outputs_bwd_kernel(const float* __restrict__ raw, const floa
       q = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
       cr = sigmoidf_acc(r4.x); cg = sigmoidf_acc(r4.y); cb = sigmoidf_acc(r4.z);
       float off = white_bkgd ? 1.0f : 0.0f;
-      e = gr * (cr - off) + gg * (cg - off) + gb * (cb - off);
+      if (has_rgb) e = gr * (cr - off) + gg * (cg - off) + gb * (cb - off);
+      if constexpr (kSeeds) {
+        if (g.acc || g.disp) e += g_acc;
+        if (g.depth || g.disp) {
+          const float t = g_depth * z;
+          e += t;
+          if (g.amax && !disp_nan) m = absmax_step(m, t);
+        }
+        if (g.weights) {
+          const float t = g.weights[n * S + k];
+          e += t;
+          if (g.amax) m = absmax_step(m, t);
+        }
+        if (g.raw) {
+          gw4 = reinterpret_cast<const float4*>(g.raw)[n * S + k];
+          if (g.amax) { m = absmax_step(m, gw4.x); m = absmax_step(m, gw4.y); m = absmax_step(m, gw4.z); m = absmax_step(m, gw4.w); }
+        }
+      }
       f = (s > 0.0f) ? dist * oma : 0.0f;
     }
     float incl = warp_scan_mul(q, lane);
@@ -242,9 +323,23 @@ __global__ void raw2outputs_bwd_kernel(const float* __restrict__ raw, const floa
       float w = alpha * T;
       sT[k] = T * e; sWE[k] = w * e; sQ[k] = q; sF[k] = f;   // sT holds the first term of dL/dalpha
       float* o = d_raw + (n * S + k) * 4;
-      o[0] = w * gr * cr * (1.0f - cr);
-      o[1] = w * gg * cg * (1.0f - cg);
-      o[2] = w * gb * cb * (1.0f - cb);
+      if (has_rgb) {
+        o[0] = w * gr * cr * (1.0f - cr);
+        o[1] = w * gg * cg * (1.0f - cg);
+        o[2] = w * gb * cb * (1.0f - cb);
+      } else {
+        o[0] = 0.f; o[1] = 0.f; o[2] = 0.f;
+      }
+      if constexpr (kSeeds) {
+        if (g.raw) { o[0] += gw4.x; o[1] += gw4.y; o[2] += gw4.z; }
+      }
+    }
+  }
+  if constexpr (kSeeds) {
+    if (g.amax) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) { const float t = __shfl_xor_sync(0xffffffffu, m, o); m = (t > m || t != t) ? t : m; }
+      if (lane == 0) atomicMax(g.amax, __float_as_uint(m));
     }
   }
   __syncwarp();
@@ -262,6 +357,13 @@ __global__ void raw2outputs_bwd_kernel(const float* __restrict__ raw, const floa
       float* o = d_raw + (n * S + k) * 4;
       float dalpha = sT[k] - suffix / sQ[k];
       o[3] = dalpha * sF[k];
+      if constexpr (kSeeds) {
+        if (disp_nan) {                  // relu's gradient is a select: the NaN reaches only samples with density > 0
+          const float s = raw[(n * S + k) * 4 + 3] + (noise ? noise[n * S + k] : 0.0f);
+          if (!(s > 0.0f)) o[3] = 0.0f;
+        }
+        if (g.raw) o[3] += g.raw[(n * S + k) * 4 + 3];
+      }
     }
   }
 }
