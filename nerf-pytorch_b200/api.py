@@ -131,6 +131,17 @@ def get_embedder(multires, i=0):
 # NeRF module  (run_nerf_helpers.py:67-119): parameter container with the reference's state_dict keys
 # ------------------------------------------------------------------------------------------------
 
+def effective_skip(skips, D):
+    """The one skip connection of a D-layer net (-1: none).  The reference's forward concatenates after layer i only for
+    i in range(D) (run_nerf_helpers.py:99-103), so entries >= D and negative ones never take effect: create_nerf's
+    skips = [4] with netdepth <= 4 is a net without a skip.  Entry D - 1 stays and is rejected by the library, as the
+    reference fails on it (its heads would receive W + input_ch columns)."""
+    live = [s for s in skips if 0 <= s < D]
+    if len(live) > 1:
+        raise NotImplementedError("nerf_b200 supports at most one skip connection")
+    return live[0] if live else -1
+
+
 class NeRF(nn.Module):
     def __init__(self, D=8, W=256, input_ch=3, input_ch_views=3, output_ch=4, skips=[4], use_viewdirs=False):
         super().__init__()
@@ -193,12 +204,10 @@ class NeRF(nn.Module):
 
     def net_params(self) -> NerfNetParams:
         self._check_device()
-        if len(self.skips) > 1:
-            raise NotImplementedError("nerf_b200 supports at most one skip connection")
         n = NerfNetParams()
         n.D, n.W, n.input_ch = self.D, self.W, self.input_ch
         n.input_ch_views = self.input_ch_views if self.use_viewdirs else 0
-        n.skip = self.skips[0] if len(self.skips) == 1 else -1
+        n.skip = effective_skip(self.skips, self.D)
         n.use_viewdirs, n.output_ch = int(self.use_viewdirs), self.output_ch
         for i, l in enumerate(self.pts_linears):
             if not (l.weight.is_contiguous() and l.weight.dtype == torch.float32):

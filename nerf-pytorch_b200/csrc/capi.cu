@@ -447,11 +447,13 @@ static int march_impl(const float* rays, const float* z_vals, const float* noise
     // exact mode (validation path): materialise pts -> fp32 CUDA-core MLP -> raw2outputs kernel
     NB_CHECK_ARG(save == nullptr, "training-mode records belong to the tensor-core path");
     const long long M = N * (long long)S;
-    const size_t need = (size_t)M * 12 + (out->raw ? 0 : (size_t)M * 16);
+    // mlp_simt_kernel stores raw as float4: its scratch starts on a 16-byte boundary whatever M is
+    const size_t pts_floats = ((size_t)M * 3 + 3) & ~(size_t)3;
+    const size_t need = pts_floats * 4 + (out->raw ? 0 : (size_t)M * 16);
     NB_CHECK_ARG(workspace && workspace_bytes >= need, "exact-mode workspace too small: need %zu bytes", need);
     NB_CHECK_ARG(net->W <= SIMT_THREADS && net->W % 4 == 0, "exact path supports netwidth <= 256");
     float* pts = static_cast<float*>(workspace);
-    float* raw = out->raw ? out->raw : pts + (size_t)M * 3;
+    float* raw = out->raw ? out->raw : pts + pts_floats;
     pts_kernel<<<cdiv(M, 256), 256, 0, st>>>(rays, cfg->ray_stride, z_vals, M, S, pts);
     NB_LAUNCH_OK("pts_kernel");
     const size_t sm = simt_smem_bytes(*net);
@@ -644,11 +646,14 @@ static int march_bwd_impl(const float* rays, const float* z_vals, const float* n
     const float* ry = rays + n0 * rs;
     const float* zz = z_vals + n0 * S;
     const float* nz = noise ? noise + n0 * S : nullptr;
+    // every buffer starts on a 16-byte boundary: mlp_simt_kernel stores raw as float4, and M * (3 + IC + ICV) need not be a
+    // multiple of 4 (the rounding takes at most 24 of the workspace's 1024 spare bytes)
     float* p = static_cast<float*>(workspace);
-    float* pts = p;        p += M * 3;
+    auto q4 = [](long long n) { return (n + 3) & ~3ll; };
+    float* pts = p;        p += q4(M * 3);
     SimtSave sv;
-    sv.enc = p;            p += M * IC;
-    sv.encv = p;           p += M * ICV;
+    sv.enc = p;            p += q4(M * IC);
+    sv.encv = p;           p += q4(M * ICV);
     sv.h = p;              p += (size_t)D * M * W;
     sv.feat = p;           p += M * W;
     sv.hv = p;             p += M * W2;

@@ -14,7 +14,7 @@ import numpy as np
 import torch
 
 from . import synth
-from . import torch_ref as T
+from . import tc_emul
 from .tc_emul import f16
 
 
@@ -36,15 +36,16 @@ def nerf_state_noviews(seed=0, sharpen=False, output_ch=5, D=8, W=256, input_ch=
     return p
 
 
-def forward_noviews(sd: dict, pts: torch.Tensor, D: int = 8, skip: int = 4, ic: int = 63):
-    """pts [M,3] -> dict: enc16 [M,64), h16[l] [M,256] (post-ReLU, fp16-rounded), pre[l] (fp64 pre-activations), raw [M,4].
+def forward_noviews(sd: dict, pts: torch.Tensor, D: int = 8, skip: int = 4, L: int = 10):
+    """pts [M,3] -> dict: enc16 [M, 3 + 6L], enc64 [M, 64] (as tc_emul.forward; L = 0: i_embed = -1), h16[l] [M,256] (post-ReLU, fp16-rounded), pre[l] (fp64 pre-activations), raw [M,4].
 
     The head is fp32 on the UN-rounded h_{D-1} (the kernel's FMA chains on the accumulators); the training-mode pass
     records h16[D-1] besides, for output_linear's weight gradient."""
     sd = {k: v.to(torch.float64) for k, v in sd.items()}
     w16 = {k: f16(v) for k, v in sd.items() if k.endswith("weight")}
-    enc16 = f16(T.embed(pts.to(torch.float32), 10).to(torch.float64))
-    out = {"enc16": enc16, "h16": [], "pre": []}
+    ic = tc_emul.input_ch(L)
+    enc16, enc64 = tc_emul.encode16(pts, L)
+    out = {"enc16": enc16, "enc64": enc64, "h16": [], "pre": []}
     h16 = h32 = None
     for l in range(D):
         W = w16[f"pts_linears.{l}.weight"]
@@ -63,7 +64,7 @@ def forward_noviews(sd: dict, pts: torch.Tensor, D: int = 8, skip: int = 4, ic: 
     return out
 
 
-def backward_noviews(sd: dict, acts: dict, masks: dict, d_raw: torch.Tensor, scale: float, D: int = 8, skip: int = 4, ic: int = 63):
+def backward_noviews(sd: dict, acts: dict, masks: dict, d_raw: torch.Tensor, scale: float, D: int = 8, skip: int = 4, L: int = 10):
     """The backward of csrc/bwd_wg.cuh for an output_linear head, given the forward's saved tensors.
 
     acts: enc16, h16[l] (per row);  masks: 'h'[l] [M,256] (pre-activation > 0);  d_raw [M,4] fp64 (unscaled).
@@ -71,6 +72,7 @@ def backward_noviews(sd: dict, acts: dict, masks: dict, d_raw: torch.Tensor, sca
     at step j of the gradient record, dA16 of pts layer D - j (index 0 unused: None)."""
     sd = {k: v.to(torch.float64) for k, v in sd.items()}
     w16 = {k: f16(v) for k, v in sd.items() if k.endswith("weight")}
+    ic = tc_emul.input_ch(L)
     d4 = d_raw[:, :4].to(torch.float64)
     Wout = sd["output_linear.weight"]
     # seed: fp32 head weights, the ReLU mask of layer D-1, one saturating fp16 rounding

@@ -29,16 +29,28 @@ def loss_scale(amax: float) -> float:
     return float(2.0 ** np.floor(np.log2(np.float32(2048.0) / np.float32(amax))))
 
 
-def forward(sd: dict, pts: torch.Tensor, viewdirs_rows: torch.Tensor, D: int = 8, skip: int = 4, ic: int = 63):
+def input_ch(L: int) -> int:
+    """run_nerf_helpers.py:48-63: 3 + 6 L columns; L = 0 is i_embed = -1 (the raw coordinates)."""
+    return 3 + 6 * L
+
+
+def encode16(pts: torch.Tensor, L: int):
+    """gamma(p) rounded to fp16 -> (enc16 [M, 3 + 6L], enc64 [M, 64]: the encoding record, zero past column 3 + 6L)."""
+    enc16 = f16(T.embed(pts.to(torch.float32), L).to(torch.float64))
+    return enc16, torch.nn.functional.pad(enc16, (0, 64 - enc16.shape[1]))
+
+
+def forward(sd: dict, pts: torch.Tensor, viewdirs_rows: torch.Tensor, D: int = 8, skip: int = 4, L: int = 10, Lv: int = 4):
     """pts [M,3], viewdirs_rows [M,3] (the ray's direction repeated per sample) -> dict of the tensors the kernel keeps.
 
-    enc16 [M,64], h16[l] [M,256] (post-ReLU, fp16-rounded), pre[l] (fp64 pre-activations), feat16, hv16, pre_v, raw [M,4]."""
+    L / Lv: multires / multires_views (0: i_embed = -1); skip -1: none.  enc16 [M, 3 + 6L], enc64 [M, 64] (the encoding
+    record), h16[l] [M,256] (post-ReLU, fp16-rounded), pre[l] (fp64 pre-activations), feat16, hv16, pre_v, raw [M,4]."""
     sd = {k: v.to(torch.float64) for k, v in sd.items()}
     w16 = {k: f16(v) for k, v in sd.items() if k.endswith("weight")}
-    enc = T.embed(pts.to(torch.float32), 10).to(torch.float64)
-    enc16 = f16(enc)
-    encv = T.embed(viewdirs_rows.to(torch.float32), 4).to(torch.float64)
-    out = {"enc16": enc16, "h16": [], "pre": [], "encv": encv}
+    ic = input_ch(L)
+    enc16, enc64 = encode16(pts, L)
+    encv = T.embed(viewdirs_rows.to(torch.float32), Lv).to(torch.float64)
+    out = {"enc16": enc16, "enc64": enc64, "h16": [], "pre": [], "encv": encv}
     h16 = None
     h32 = None
     for l in range(D):
@@ -75,14 +87,15 @@ def composite_adjoint(raw: torch.Tensor, z: torch.Tensor, rays_d: torch.Tensor, 
 
 
 def backward(sd: dict, acts: dict, masks: dict, d_raw: torch.Tensor, scale: float, ray_of_row: torch.Tensor, n_rays: int,
-             D: int = 8, skip: int = 4, ic: int = 63):
-    """The backward of csrc/bwd_wg.cuh given the forward's saved tensors.
+             D: int = 8, skip: int = 4, L: int = 10):
+    """The backward of csrc/bwd_wg.cuh given the forward's saved tensors (L: multires; the view encoding is acts['encv']).
 
     acts: enc16, h16[l], feat16, hv16, encv (per row);  masks: 'h'[l] [M,256] bool (pre-activation > 0), 'hv' [M,128];
     d_raw [M,4] fp64 (unscaled).  Returns (grads by state_dict key, stages) where stages holds the loss-scaled fp16
     tensors the kernels write: d_hv16, step[j] (j = 0: d_feat16, j >= 1: dA16 of pts layer D - j)."""
     sd = {k: v.to(torch.float64) for k, v in sd.items()}
     w16 = {k: f16(v) for k, v in sd.items() if k.endswith("weight")}
+    ic = input_ch(L)
     d_rgb, d_sig = d_raw[:, :3].to(torch.float64), d_raw[:, 3:4].to(torch.float64)
     g = {}
     d_hv16 = f16((d_rgb * scale) @ sd["rgb_linear.weight"] * masks["hv"])

@@ -25,13 +25,16 @@ def embed(x: torch.Tensor, L: int) -> torch.Tensor:
 
 
 def mlp(sd: dict, x: torch.Tensor, ic: int = 63, icv: int = 27, skip: int = 4, D: int = 8) -> torch.Tensor:
-    """H:96-119 with the reference's state_dict keys; x [M, ic + icv] -> [M, 4] (rgb, sigma)."""
+    """H:96-119 with the reference's state_dict keys; x [M, ic + icv] -> [M, 4] (rgb, sigma).  skip -1: none.  A net without
+    view directions (an output_linear head, H:117) returns the first four of its outputs, the ones raw2outputs reads."""
     pts, views = x[:, :ic], x[:, ic:ic + icv]
     h = pts
     for i in range(D):
         h = F.relu(F.linear(h, sd[f"pts_linears.{i}.weight"], sd[f"pts_linears.{i}.bias"]))
         if i == skip:
             h = torch.cat([pts, h], -1)
+    if "output_linear.weight" in sd:
+        return F.linear(h, sd["output_linear.weight"], sd["output_linear.bias"])[:, :4]
     sigma = F.linear(h, sd["alpha_linear.weight"], sd["alpha_linear.bias"])
     feat = F.linear(h, sd["feature_linear.weight"], sd["feature_linear.bias"])
     hv = F.relu(F.linear(torch.cat([feat, views], -1), sd["views_linears.0.weight"], sd["views_linears.0.bias"]))

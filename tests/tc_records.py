@@ -14,6 +14,41 @@ def img_index(Ccols):
     return off // 2
 
 
+def rec_act_h(l):
+    """byte offset of h_l (l < D; l = D: hv) inside an activation record"""
+    return 16384 + l * 65536
+
+
+def rec_grad_step(j):
+    """byte offset of dgrad step j's output inside a gradient record"""
+    return 32768 + j * 65536
+
+
+def restate_layout(N, S, D, input_ch_views, sms):
+    """csrc/train_common.cuh make_tile_plan and capi.cu make_bwd_layout restated -> the 12 values of
+    nerf_b200_march_bwd_tc_layout (Plan's order), nerf_b200_march_bwd_tc_workspace_bytes and nerf_b200_train_record_bytes"""
+    want = (N * S + 255) // 256
+    grid = max(min(want, sms, N), 1)
+    rpc = -(-N // grid)
+    grid = -(-N // rpc)
+    nst = (rpc * S + 255) // 256
+    n_tiles = grid * nst * 2
+    rec_act, rec_mask, rec_grad = 16384 + D * 65536 + 32768, D * 4096 + 2048, 32768 + (D + 1) * 65536
+
+    def up(x):
+        return (x + 1023) & ~1023
+    off_amax = 0
+    off_draw = up(off_amax + 256)
+    off_encv = up(off_draw + N * S * 16)
+    off_dsum = up(off_encv + N * max(input_ch_views, 1) * 4)
+    off_gv = up(off_dsum + N * 128 * 4)
+    off_partial = up(off_gv + (128 * 256 + 128) * 4)
+    off_grad = up(off_partial + sms * 256 * 256 * 4)
+    total = up(off_grad + n_tiles * rec_grad)
+    layout = (off_draw, off_grad, rec_act, rec_mask, rec_grad, grid, rpc, nst, n_tiles, off_amax, off_dsum, off_partial)
+    return layout, total + 1024, (n_tiles * rec_act, n_tiles * rec_mask)
+
+
 class Plan:
     """tile plan of one pass: nerf_b200_march_bwd_tc_layout"""
 

@@ -2,7 +2,6 @@
 C ABI, stage by stage against the quantisation-aware restatement (oracle/tc_emul.py) and end to end against the exact
 mode and the reference's autograd (tests/golden/lego_grads.npz).  Measured deviations are appended to parity_train.json
 in the git-ignored output directory."""
-import ctypes as C
 import json
 import os
 
@@ -31,37 +30,6 @@ def _record(name, value):
     data[name] = value
     with open(path, "w") as f:
         json.dump(data, f, indent=1, sort_keys=True)
-
-
-def _cfg(G, S, white=True):
-    cfg = G._lib.NerfRenderCfg()
-    cfg.N_samples, cfg.N_importance, cfg.multires, cfg.multires_views = S, 0, 10, 4
-    cfg.lindisp, cfg.perturb, cfg.white_bkgd, cfg.ray_stride, cfg.precision = 0, 0, int(white), 11, G._lib.PREC_TC_FP16
-    return cfg
-
-
-def _march(G, net, rays11, z, train):
-    """one fused pass through the C ABI -> (outputs dict, act, mask) (act / mask None when not training)"""
-    from nerf_pytorch_b200 import api
-    lib = G._lib.load()
-    N, S = z.shape
-    n, pk = net.net_params(), net.packed()
-    cfg = _cfg(G, S)
-    o = {k: torch.zeros(s, device=G.DEV) for k, s in (("rgb", (N, 3)), ("disp", (N,)), ("acc", (N,)), ("w", (N, S)), ("raw", (N, S, 4)))}
-    out = G._lib.NerfPassOut(G.ptr(o["rgb"]), G.ptr(o["disp"]), G.ptr(o["acc"]), C.c_void_p(0), G.ptr(o["w"]), G.ptr(o["raw"]))
-    ws_bytes = lib.nerf_b200_march_workspace_bytes(N, S)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=G.DEV)
-    if train:
-        sv, act, mask = api._train_save(lib, N, S, n, G.DEV)
-        act.zero_(); mask.zero_()
-        G._lib.check(lib.nerf_b200_march_train(G.ptr(rays11), G.ptr(z), None, N, S, C.byref(n), G.ptr(pk), C.byref(cfg), C.byref(out),
-                                               G.ptr(ws), ws_bytes, C.byref(sv), G.stream()), "march_train")
-    else:
-        act = mask = None
-        G._lib.check(lib.nerf_b200_march(G.ptr(rays11), G.ptr(z), None, N, S, C.byref(n), G.ptr(pk), C.byref(cfg), C.byref(out),
-                                         G.ptr(ws), ws_bytes, G.stream()), "march")
-    torch.cuda.synchronize()
-    return o, act, mask
 
 
 def _inputs(G, N, S, seed, sharpen=False):
@@ -96,8 +64,8 @@ def test_training_forward_records(G, N, S):
     import tc_records as R
     packed, z, state, net = _inputs(G, N, S, seed=5)
     rays11, zd = G.dev(packed), G.dev(z)
-    o_inf, _, _ = _march(G, net, rays11, zd, train=False)
-    o_tr, act, mask = _march(G, net, rays11, zd, train=True)
+    o_inf, _, _ = G.march(net, rays11, zd, train=False)
+    o_tr, act, mask = G.march(net, rays11, zd, train=True)
     for k in ("rgb", "acc", "w", "raw"):
         assert torch.equal(o_inf[k], o_tr[k]), k
     plan = R.Plan(G._lib.load(), N, S, net.net_params())
@@ -157,25 +125,6 @@ def test_inference_render_stays_on_the_inference_kernel(G):
     assert out[0].requires_grad
 
 
-def _bwd_tc(G, net, rays11, zd, raw, act, mask, g_rgb):
-    """nerf_b200_march_bwd_tc through the C ABI -> (grads dict name -> np, workspace bytes np)"""
-    lib = G._lib.load()
-    N, S = zd.shape
-    n = net.net_params()
-    cfg = _cfg(G, S)
-    grads = {k: torch.zeros_like(p, dtype=torch.float32) for k, p in net.named_parameters()}
-    gs = net.grad_struct(grads)
-    sv = G._lib.NerfTrainSave(G.ptr(act), act.numel(), G.ptr(mask), mask.numel())
-    ws_bytes = lib.nerf_b200_march_bwd_tc_workspace_bytes(N, S, C.byref(n))
-    assert ws_bytes > 0
-    ws = torch.zeros(ws_bytes + 1024, dtype=torch.uint8, device=G.DEV)
-    base = (ws.data_ptr() + 1023) // 1024 * 1024 - ws.data_ptr()          # the library aligns the same way
-    G._lib.check(lib.nerf_b200_march_bwd_tc(G.ptr(rays11), G.ptr(zd), None, N, S, C.byref(n), G.ptr(net.packed()), C.byref(cfg), G.ptr(raw),
-                                            C.byref(sv), G.ptr(g_rgb), C.byref(gs), G.ptr(ws), ws_bytes + 1024, G.stream()), "march_bwd_tc")
-    torch.cuda.synchronize()
-    return {k: v.cpu().numpy() for k, v in grads.items()}, ws.cpu().numpy()[base:]
-
-
 @pytest.mark.parametrize("N,S,sharpen", [(100, 64, False), (37, 192, False), (64, 64, True), (50, 40, False)])
 def test_backward_stages_match_emulation(G, N, S, sharpen):
     """Every stage of the tensor-core backward, given the CUDA forward's own records: dL/draw, the d_hv seed, each dgrad
@@ -184,10 +133,10 @@ def test_backward_stages_match_emulation(G, N, S, sharpen):
     from oracle import tc_emul as E
     packed, z, state, net = _inputs(G, N, S, seed=7, sharpen=sharpen)
     rays11, zd = G.dev(packed), G.dev(z)
-    o, act, mask = _march(G, net, rays11, zd, train=True)
+    o, act, mask = G.march(net, rays11, zd, train=True)
     rng = np.random.default_rng(11)
     g_rgb = ((rng.random((N, 3), dtype=np.float32) - 0.5) * (4.0 / (3 * N))).astype(np.float32)
-    grads, ws = _bwd_tc(G, net, rays11, zd, o["raw"], act, mask, G.dev(g_rgb))
+    grads, ws = G.march_bwd_tc(net, rays11, zd, o["raw"], act, mask, G.dev(g_rgb))
     plan = R.Plan(G._lib.load(), N, S, net.net_params())
     D, M = 8, N * S
     A, Mk = act.cpu().numpy(), mask.cpu().numpy()

@@ -45,37 +45,6 @@ def _net(G, seed, sharpen=False, output_ch=5):
     return G.make_net(state, use_viewdirs=False, output_ch=output_ch), state
 
 
-def _cfg(G, S, white=True):
-    cfg = G._lib.NerfRenderCfg()
-    cfg.N_samples, cfg.N_importance, cfg.multires, cfg.multires_views = S, 0, 10, 4
-    cfg.lindisp, cfg.perturb, cfg.white_bkgd, cfg.ray_stride, cfg.precision = 0, 0, int(white), 8, G._lib.PREC_TC_FP16
-    return cfg
-
-
-def _march(G, net, rays8, z, train):
-    """one fused pass through the C ABI -> (outputs dict, act, mask) (act / mask None when not training)"""
-    from nerf_pytorch_b200 import api
-    lib = G._lib.load()
-    N, S = z.shape
-    n, pk = net.net_params(), net.packed()
-    cfg = _cfg(G, S)
-    o = {k: torch.zeros(s, device=G.DEV) for k, s in (("rgb", (N, 3)), ("disp", (N,)), ("acc", (N,)), ("w", (N, S)), ("raw", (N, S, 4)))}
-    out = G._lib.NerfPassOut(G.ptr(o["rgb"]), G.ptr(o["disp"]), G.ptr(o["acc"]), C.c_void_p(0), G.ptr(o["w"]), G.ptr(o["raw"]))
-    ws_bytes = lib.nerf_b200_march_workspace_bytes(N, S)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=G.DEV)
-    if train:
-        sv, act, mask = api._train_save(lib, N, S, n, G.DEV)
-        act.zero_(); mask.zero_()
-        G._lib.check(lib.nerf_b200_march_train(G.ptr(rays8), G.ptr(z), None, N, S, C.byref(n), G.ptr(pk), C.byref(cfg), C.byref(out),
-                                               G.ptr(ws), ws_bytes, C.byref(sv), G.stream()), "march_train")
-    else:
-        act = mask = None
-        G._lib.check(lib.nerf_b200_march(G.ptr(rays8), G.ptr(z), None, N, S, C.byref(n), G.ptr(pk), C.byref(cfg), C.byref(out),
-                                         G.ptr(ws), ws_bytes, G.stream()), "march")
-    torch.cuda.synchronize()
-    return o, act, mask
-
-
 def _inputs(G, N, S, seed, sharpen=False):
     sb = G.synth.ray_batch("lego", N, seed=seed)
     packed = G.O.pack_rays(400, 400, sb["K"], sb["rays"][0], sb["rays"][1], False, 2.0, 6.0, False).astype(np.float32)
@@ -103,8 +72,8 @@ def test_training_forward_records_noviews(G, N, S):
     import tc_records as R
     packed, z, state, net = _inputs(G, N, S, seed=5)
     rays8, zd = G.dev(packed), G.dev(z)
-    o_inf, _, _ = _march(G, net, rays8, zd, train=False)
-    o_tr, act, mask = _march(G, net, rays8, zd, train=True)
+    o_inf, _, _ = G.march(net, rays8, zd, train=False)
+    o_tr, act, mask = G.march(net, rays8, zd, train=True)
     for k in ("rgb", "disp", "acc", "w", "raw"):                       # bit patterns: disp is NaN where acc = 0 (run_nerf.py:299)
         assert torch.equal(o_inf[k].view(torch.int32), o_tr[k].view(torch.int32)), k
     plan = R.Plan(G._lib.load(), N, S, net.net_params())
@@ -129,25 +98,6 @@ def test_training_forward_records_noviews(G, N, S):
     _record(f"records_N{N}_S{S}", stats)
 
 
-def _bwd_tc(G, net, rays8, zd, raw, act, mask, g_rgb):
-    """nerf_b200_march_bwd_tc through the C ABI -> (grads dict name -> np, workspace bytes np)"""
-    lib = G._lib.load()
-    N, S = zd.shape
-    n = net.net_params()
-    cfg = _cfg(G, S)
-    grads = {k: torch.zeros_like(p, dtype=torch.float32) for k, p in net.named_parameters()}
-    gs = net.grad_struct(grads)
-    sv = G._lib.NerfTrainSave(G.ptr(act), act.numel(), G.ptr(mask), mask.numel())
-    ws_bytes = lib.nerf_b200_march_bwd_tc_workspace_bytes(N, S, C.byref(n))
-    assert ws_bytes > 0
-    ws = torch.zeros(ws_bytes + 1024, dtype=torch.uint8, device=G.DEV)
-    base = (ws.data_ptr() + 1023) // 1024 * 1024 - ws.data_ptr()          # the library aligns the same way
-    G._lib.check(lib.nerf_b200_march_bwd_tc(G.ptr(rays8), G.ptr(zd), None, N, S, C.byref(n), G.ptr(net.packed()), C.byref(cfg), G.ptr(raw),
-                                            C.byref(sv), G.ptr(g_rgb), C.byref(gs), G.ptr(ws), ws_bytes + 1024, G.stream()), "march_bwd_tc")
-    torch.cuda.synchronize()
-    return {k: v.cpu().numpy() for k, v in grads.items()}, ws.cpu().numpy()[base:]
-
-
 @pytest.mark.parametrize("N,S,sharpen", [(100, 64, False), (37, 192, False), (64, 64, True), (50, 40, False)])
 def test_backward_stages_match_emulation_noviews(G, N, S, sharpen):
     """dL/draw, the dA_{D-1} seed (output_linear head), each dgrad step's fp16 tile image and every gradient tensor, output_linear's
@@ -157,10 +107,10 @@ def test_backward_stages_match_emulation_noviews(G, N, S, sharpen):
     from oracle import tc_emul as E
     packed, z, state, net = _inputs(G, N, S, seed=7, sharpen=sharpen)
     rays8, zd = G.dev(packed), G.dev(z)
-    o, act, mask = _march(G, net, rays8, zd, train=True)
+    o, act, mask = G.march(net, rays8, zd, train=True)
     rng = np.random.default_rng(11)
     g_rgb = ((rng.random((N, 3), dtype=np.float32) - 0.5) * (4.0 / (3 * N))).astype(np.float32)
-    grads, ws = _bwd_tc(G, net, rays8, zd, o["raw"], act, mask, G.dev(g_rgb))
+    grads, ws = G.march_bwd_tc(net, rays8, zd, o["raw"], act, mask, G.dev(g_rgb))
     plan = R.Plan(G._lib.load(), N, S, net.net_params())
     M = N * S
     A, Mk = act.cpu().numpy(), mask.cpu().numpy()
@@ -433,7 +383,7 @@ def test_c_abi_noviews_queries_and_mismatch(G):
     # packed weights: the backward stream of a no-view net is the 8 (D - 1) pts-layer chunks (16 KB each)
     assert lib.nerf_b200_packed_bytes(C.byref(n_nv)) >= 8 * (D - 1) * 16384
     dummy = torch.zeros(1 << 16, device=G.DEV)
-    cfg = _cfg(G, Sc)
+    cfg = G.cfg(Sc, 8)
     grads = [{k: torch.zeros_like(p) for k, p in n.named_parameters()} for n in (net_nv, net_vd)]
     gs = [net_nv.grad_struct(grads[0]), net_vd.grad_struct(grads[1])]
     sv = G._lib.NerfTrainSave(G.ptr(dummy), dummy.numel() * 4, G.ptr(dummy), dummy.numel() * 4)
