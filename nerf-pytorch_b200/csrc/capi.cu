@@ -419,12 +419,18 @@ int nerf_b200_coarse_z(const float* rays, int ray_stride, const float* t_vals, c
 int nerf_b200_fine_z(const float* z_vals, const float* weights, const float* u, int64_t u_row_stride, int64_t N, int S,
                      int n_imp, float* z_fine, float* z_samples, float* z_std, void* stream) {
   NB_CHECK_ARG(z_vals && weights && u && z_fine, "NULL pointer");
-  NB_CHECK_ARG(S >= 3 && n_imp >= 1 && S + n_imp <= 4096, "bad S / n_imp");
+  NB_CHECK_ARG(S >= 3 && n_imp >= 1 && S + n_imp <= 4096, "bad S / n_imp");   // S = 2: the reference fails too (empty cdf)
   if (N == 0) return 0;
   int P = 1;
   while (P < S + n_imp) P <<= 1;
-  const int wpb = 4;
-  const size_t sm = (size_t)wpb * (3 * S + P) * sizeof(float);
+  // four warps (rays) per block, fewer where their rows would pass the opt-in shared-memory limit (from S ~ 3478 at P = 4096)
+  int dev = 0, optin = 0;
+  NB_CUDA(cudaGetDevice(&dev));
+  NB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const size_t row_bytes = (size_t)(3 * S + P) * sizeof(float);
+  int wpb = 4;
+  while (wpb > 1 && (size_t)wpb * row_bytes > (size_t)optin) --wpb;
+  const size_t sm = (size_t)wpb * row_bytes;
   if (int rc = smem_optin((const void*)fine_z_kernel, sm)) return rc;
   fine_z_kernel<<<cdiv(N, wpb), wpb * 32, sm, (cudaStream_t)stream>>>(z_vals, weights, u, u_row_stride, N, S, n_imp, P, z_fine, z_samples, z_std);
   NB_LAUNCH_OK("fine_z_kernel");

@@ -371,20 +371,55 @@ __global__ void raw2outputs_bwd_kernel(const float* __restrict__ raw, const floa
 // ---------------------------------------------------------------------------------------------
 // sample_pdf  (run_nerf_helpers.py:196-239) on per-warp shared-memory rows
 // ---------------------------------------------------------------------------------------------
+// sum(w + 1e-5) over w = s_w[0..n) (:198-199), rounded exactly as CPU torch's float32 sum(-1) of a contiguous row, so the
+// cdf and every sample match the reference to the bit (oracle/resample.py torch_sum states the order).  Warp-uniform result.
+//   n < 8:  four accumulators a_k += x[4j+k], the leftover x[4*(n/4)..] into a_0, then ((a_0 + a_1) + a_2) + a_3.
+//   n >= 8: the same over 8-wide vectors v_i = x[8i..8i+7] (V = n/8 of them), which is one accumulator per lane here:
+//           lane l sums x[32r + l] for r < n/32, with a cascade that moves the running sum into a second accumulator
+//           after every 16 rows (the next cascade level needs >= 256 rows, n >= 8192, beyond the accepted sizes);
+//           lanes 0-7 add the leftover vectors and then lanes 8-15, 16-23, 24-31 in that order; the total is 0, plus the
+//           scalar tail x[8V..n) in order, plus the 8 lanes in order.
+__device__ __forceinline__ float torch_row_sum(const float* s_w, int n, int lane) {
+  auto x = [&](int i) { return __fadd_rn(s_w[i], 1e-5f); };
+  if (n < 8) {
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    if (n >= 4) { a0 = __fadd_rn(a0, x(0)); a1 = __fadd_rn(a1, x(1)); a2 = __fadd_rn(a2, x(2)); a3 = __fadd_rn(a3, x(3)); }
+    for (int i = n & ~3; i < n; ++i) a0 = __fadd_rn(a0, x(i));
+    return __fadd_rn(__fadd_rn(__fadd_rn(a0, a1), a2), a3);
+  }
+  const int V = n >> 3, rows = V >> 2;
+  float a0 = 0.f, a1 = 0.f;
+  int r = 0;
+  for (; r + 16 <= rows; r += 16) {
+    for (int k = 0; k < 16; ++k) a0 = __fadd_rn(a0, x(32 * (r + k) + lane));
+    a1 = __fadd_rn(a1, a0);
+    a0 = 0.f;
+  }
+  for (; r < rows; ++r) a0 = __fadd_rn(a0, x(32 * r + lane));
+  a0 = __fadd_rn(a0, a1);
+  if (lane < 8) for (int v = 4 * rows; v < V; ++v) a0 = __fadd_rn(a0, x(8 * v + lane));
+  const float p1 = __shfl_down_sync(0xffffffffu, a0, 8), p2 = __shfl_down_sync(0xffffffffu, a0, 16),
+              p3 = __shfl_down_sync(0xffffffffu, a0, 24);
+  a0 = __fadd_rn(__fadd_rn(__fadd_rn(a0, p1), p2), p3);
+  float total = 0.f;
+  for (int i = 8 * V; i < n; ++i) total = __fadd_rn(total, x(i));
+#pragma unroll
+  for (int l = 0; l < 8; ++l) total = __fadd_rn(total, __shfl_sync(0xffffffffu, a0, l));
+  return total;
+}
+
 // s_bins[B], s_w[B-1] in; s_cdf[B] scratch.  Writes n_samples values through `emit(j, value)`.
 template <class Emit>
 __device__ __forceinline__ void sample_pdf_row(const float* s_bins, const float* s_w, float* s_cdf, int B,
                                                const float* __restrict__ u_row, int n_samples, int lane,
                                                Emit emit) {
-  float part = 0.0f;
-  for (int i = lane; i < B - 1; i += 32) part += __fadd_rn(s_w[i], 1e-5f);                    // :198
-  const float total = warp_sum(part);                                                         // :199
+  const float total = torch_row_sum(s_w, B - 1, lane);                                        // :198-199
   for (int i = lane; i < B - 1; i += 32) s_cdf[i + 1] = __fdiv_rn(__fadd_rn(s_w[i], 1e-5f), total);   // pdf (:199)
   __syncwarp();
-  if (lane == 0) {                                  // sequential cumsum, like torch/numpy (:200-201)
-    float c = 0.0f;
+  if (lane == 0) {                                  // cumsum (:200-201) as CPU torch: a float64 running sum, each prefix
+    double c = 0.0;                                 // rounded to float32
     s_cdf[0] = 0.0f;
-    for (int i = 1; i < B; ++i) { c = __fadd_rn(c, s_cdf[i]); s_cdf[i] = c; }
+    for (int i = 1; i < B; ++i) { c = __dadd_rn(c, (double)s_cdf[i]); s_cdf[i] = __double2float_rn(c); }
   }
   __syncwarp();
   for (int j = lane; j < n_samples; j += 32) {
@@ -444,14 +479,16 @@ __global__ void fine_z_kernel(const float* __restrict__ z_vals, const float* __r
   __syncwarp();
   float* o = s_all + S;
   sample_pdf_row(s_bins, s_w, s_cdf, B, u + n * u_row_stride, n_imp, lane, [&](int j, float v) { o[j] = v; });
-  // z_std = std(z_samples, unbiased=False) (:412): two-pass
-  float sum = 0.0f;
-  for (int j = lane; j < n_imp; j += 32) sum += o[j];
-  const float mean = warp_sum(sum) / (float)n_imp;
-  float var = 0.0f;
-  for (int j = lane; j < n_imp; j += 32) { float d = o[j] - mean; var += d * d; }
-  var = warp_sum(var) / (float)n_imp;
-  if (lane == 0 && z_std) z_std[n] = sqrtf(var);
+  // z_std = std(z_samples, unbiased=False) (:412): CPU torch accumulates in float64 and rounds the result; two-pass float64
+  if (z_std) {
+    double sum = 0.0;
+    for (int j = lane; j < n_imp; j += 32) sum = __dadd_rn(sum, (double)o[j]);
+    const double mean = __ddiv_rn(warp_sum_f64(sum), (double)n_imp);
+    double var = 0.0;
+    for (int j = lane; j < n_imp; j += 32) { const double d = __dsub_rn((double)o[j], mean); var = __dadd_rn(var, __dmul_rn(d, d)); }
+    var = __ddiv_rn(warp_sum_f64(var), (double)n_imp);
+    if (lane == 0) z_std[n] = __double2float_rn(__dsqrt_rn(var));
+  }
   if (z_samples_out) for (int j = lane; j < n_imp; j += 32) z_samples_out[n * n_imp + j] = o[j];
   __syncwarp();
   // sort(cat[z_vals, z_samples]) (:396) by ranking: z_vals is already ascending, so

@@ -19,6 +19,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from oracle import resample
+
 # --------------------------------------------------------------------------------------
 # Positional encoding  (run_nerf_helpers.py:15-63)
 # --------------------------------------------------------------------------------------
@@ -146,33 +148,14 @@ def raw2outputs(raw, z_vals, rays_d, noise=None, white_bkgd=False):
 # sample_pdf  (run_nerf_helpers.py:196-239)
 # --------------------------------------------------------------------------------------
 
-def sample_pdf(bins, weights, N_samples, det=False, u=None):
+def sample_pdf(bins, weights, N_samples, det=False, u=None, pytest=False):
     """bins [N,B], weights [N,B-1] -> samples [N,N_samples].
 
-    run_nerf_helpers.py:198-237.  `u` ([N,N_samples]) replaces the RNG draw (:208 / :216).
-    searchsorted(right=True) (:223) == first index with cdf > u.
+    run_nerf_helpers.py:198-237, rounded as the reference on CPU torch (oracle/resample.py).  `u`
+    ([N,N_samples]) replaces the RNG draw (:208 / :216); det without `u` takes torch.linspace (:205), or
+    np.linspace under `pytest` (:215).  searchsorted(right=True) (:223) == first index with cdf > u.
     """
-    dt = bins.dtype.type
-    weights = weights + dt(1e-5)                                                 # :198
-    pdf = weights / np.sum(weights, -1, keepdims=True)                           # :199
-    cdf = np.cumsum(pdf, -1, dtype=bins.dtype)                                   # :200
-    cdf = np.concatenate([np.zeros_like(cdf[..., :1]), cdf], -1)                 # :201
-    if u is None:
-        assert det, "random u must be injected (oracle does not own an RNG stream)"
-        u = np.linspace(0.0, 1.0, N_samples).astype(bins.dtype)                  # :205
-        u = np.broadcast_to(u, cdf.shape[:-1] + (N_samples,))
-    u = np.ascontiguousarray(u.astype(bins.dtype))
-    inds = np.stack([np.searchsorted(cdf[i], u[i], side="right") for i in range(cdf.shape[0])])
-    below = np.maximum(0, inds - 1)                                              # :224
-    above = np.minimum(cdf.shape[-1] - 1, inds)                                  # :225
-    cdf_lo = np.take_along_axis(cdf, below, -1)                                  # :230-232
-    cdf_hi = np.take_along_axis(cdf, above, -1)
-    bins_lo = np.take_along_axis(bins, below, -1)
-    bins_hi = np.take_along_axis(bins, above, -1)
-    denom = cdf_hi - cdf_lo                                                      # :234
-    denom = np.where(denom < dt(1e-5), np.ones_like(denom), denom)               # :235
-    t = (u - cdf_lo) / denom                                                     # :236
-    return bins_lo + t * (bins_hi - bins_lo)                                     # :237
+    return resample.sample_pdf(bins, weights, N_samples, det, u, pytest, dtype=bins.dtype)
 
 
 # --------------------------------------------------------------------------------------
@@ -181,20 +164,9 @@ def sample_pdf(bins, weights, N_samples, det=False, u=None):
 
 def coarse_z_vals(near, far, N_samples, lindisp=False, perturb=0.0, t_rand=None):
     """near, far [N,1] -> z_vals [N,N_samples].  run_nerf.py:357-379."""
-    dt = near.dtype.type
-    t_vals = np.linspace(0.0, 1.0, N_samples).astype(near.dtype)                 # :357
-    if not lindisp:
-        z_vals = near * (dt(1.0) - t_vals) + far * t_vals                        # :359
-    else:
-        z_vals = dt(1.0) / (dt(1.0) / near * (dt(1.0) - t_vals) + dt(1.0) / far * t_vals)  # :361
-    z_vals = np.broadcast_to(z_vals, (near.shape[0], N_samples)).copy()          # :363
     if perturb > 0.0:
         assert t_rand is not None, "stratified jitter must be injected"
-        mids = dt(0.5) * (z_vals[..., 1:] + z_vals[..., :-1])                    # :367
-        upper = np.concatenate([mids, z_vals[..., -1:]], -1)
-        lower = np.concatenate([z_vals[..., :1], mids], -1)
-        z_vals = lower + (upper - lower) * t_rand.astype(near.dtype)             # :379
-    return z_vals
+    return resample.coarse_z(near, far, N_samples, lindisp, t_rand if perturb > 0.0 else None, dtype=near.dtype)
 
 
 def render_rays(ray_batch, p_coarse, N_samples, p_fine=None, N_importance=0, retraw=False,
@@ -231,7 +203,7 @@ def render_rays(ray_batch, p_coarse, N_samples, p_fine=None, N_importance=0, ret
         ret["raw"] = raw
     if N_importance > 0:
         ret["rgb0"], ret["disp0"], ret["acc0"] = rgb0, disp0, acc0               # :409-411
-        ret["z_std"] = np.std(z_samples, axis=-1)                                # :412 (unbiased=False)
+        ret["z_std"] = resample.z_std(z_samples)                                 # :412 (unbiased=False)
     if return_debug:
         dbg.update({"z_vals": z_vals, "weights": weights, "depth_map": depth_map})
         ret["_debug"] = dbg

@@ -78,10 +78,12 @@ def test_gradients_match_oracle_larger_batch(G):
     for net, g in ((nets[0], gc), (nets[1], gf)):
         for name, p in net.named_parameters():
             errs.append((rel_l2(p.grad.cpu().numpy(), g[name]), name))
-    # a searchsorted knot flip moves one fine sample (see tests/test_oracle_golden.py); the layers that read the
-    # 2^9-frequency encoding directly feel it most.  Budget: median 2e-3, every tensor 5e-2.
-    assert np.median([e for e, _ in errs]) < 2e-3, sorted(errs)[-5:]
-    assert max(errs)[0] < 5e-2, sorted(errs)[-5:]
+    # the fine samples are the oracle's bit for bit given equal coarse weights (tests/test_gpu_resample.py); fp32 round-off
+    # in those weights can still move a sample near a cdf knot.  Measured on an H100: median 1.7e-5, worst tensor 6.7e-4
+    # (pts_linears.0.weight).  Budget: median 1e-4, every tensor 5e-3.
+    print("median", np.median([e for e, _ in errs]), "worst", sorted(errs)[-5:])
+    assert np.median([e for e, _ in errs]) < 1e-4, sorted(errs)[-5:]
+    assert max(errs)[0] < 5e-3, sorted(errs)[-5:]
 
 
 def test_training_steps_reduce_loss(G):

@@ -111,9 +111,12 @@ def _check_trained_gates(st, prec):
     own GPU default (TF32) deviates as much from its fp32 run (test_reference_tf32_deviates_as_much)."""
     if prec == "fp32":
         assert st["rgb0"] < 2e-5 and st["acc0"] < 2e-5, st
-        assert st["rgb_map"] < 3e-4 and st["acc_map"] < 3e-4, st
+        # fine pass: the resampling is bit-exact given the coarse weights (tests/test_gpu_resample.py); what remains is the
+        # coarse weights' fp32 round-off moving a sample near a cdf knot.  Measured on an H100: rgb_map 2.7e-6 / 5.7e-5 (lego /
+        # fern), acc_map 2.0e-5 / 3.5e-5, w_fine 1.6e-4, z_fine 2.6e-5; gated at about 2.5-4x that.
+        assert st["rgb_map"] < 1.5e-4 and st["acc_map"] < 1e-4, st
         if "w_coarse" in st:
-            assert st["w_coarse"] < 1e-5 and st["w_fine"] < 2e-3 and st["z_fine"] < 2e-3, st
+            assert st["w_coarse"] < 1e-5 and st["w_fine"] < 5e-4 and st["z_fine"] < 1e-4, st
         assert st["disp_nan_mask_mismatch"] == 0.0, st
     else:
         assert st["rgb0"] < 3e-4 and st["acc0"] < 3e-4, st

@@ -72,16 +72,12 @@ def test_units_raw2outputs():
 
 def test_units_sample_pdf():
     fx = load_golden("units")
-    # A u that lands within 1 ulp of a cdf knot (notably u == 1 vs cdf[-1], SURVEY App. D quirk 5)
-    # flips the searchsorted bin when the cumsum rounds differently; with near-empty trailing
-    # bins that moves the sample to the neighbouring knot.  Budget: <= 1 % of samples.
+    # The oracle rounds the sum, cumsum and linspace as CPU torch does (oracle/resample.py), so even a u
+    # on a cdf knot (notably u == 1 vs cdf[-1], SURVEY App. D quirk 5) takes the reference's bin.
     det = O.sample_pdf(fx["spdf_bins"], fx["spdf_w"], 128, det=True)
-    bad = np.abs(det - fx["spdf_det"]) > 5e-6
-    assert bad.mean() <= 0.01, bad.mean()
-    assert not bad[:, 1:-1].any() or bad[:, 1:-1].mean() < 0.005
+    assert np.array_equal(det, fx["spdf_det"])
     rnd = O.sample_pdf(fx["spdf_bins"], fx["spdf_w"], 128, det=False, u=fx["spdf_u"])
-    bad = np.abs(rnd - fx["spdf_rand"]) > 5e-6
-    assert bad.mean() <= 0.01, bad.mean()
+    assert np.array_equal(rnd, fx["spdf_rand"])
 
 
 def test_units_rays():
@@ -142,13 +138,13 @@ def test_gradients_match_reference_autograd(name):
         for k, v in g.items():
             ref_norm = float(fx[f"g_{tag}_{k}_norm"])
             got_norm = float(np.linalg.norm(v.astype(np.float64)))
-            assert abs(got_norm - ref_norm) <= (3e-2 if bool(fx["sharpen"]) else 5e-3) * ref_norm + 1e-9, (tag, k, got_norm, ref_norm)
+            assert abs(got_norm - ref_norm) <= (1e-3 if bool(fx["sharpen"]) else 5e-3) * ref_norm + 1e-9, (tag, k, got_norm, ref_norm)
             idx = fx[f"g_{tag}_{k}_idx"]
             err = np.linalg.norm(v.reshape(-1)[idx] - fx[f"g_{tag}_{k}_val"]) / max(np.linalg.norm(fx[f"g_{tag}_{k}_val"]), 1e-12)
             worst = max(worst, err)
-            # sharpened heads: a knot flip in sample_pdf moves one fine sample (an fp64 run of the
-            # same algorithm is 1.2e-2 away from the reference's fp32 autograd on these tensors)
-            assert err < (3e-2 if bool(fx["sharpen"]) else 2e-3), (tag, k, err)
+            # sharpened heads amplify the MLP's fp32 summation order; the fine samples themselves are the
+            # reference's (sample_pdf rounds like CPU torch).  Measured worst: 5.6e-3 sampled, 2e-4 on the norms.
+            assert err < (1e-2 if bool(fx["sharpen"]) else 2e-3), (tag, k, err)
 
 
 def test_fp64_oracle_is_consistent():
