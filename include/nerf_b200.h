@@ -240,7 +240,14 @@ typedef struct NerfNetGrads {
   float* views_w;   float* views_b;   float* rgb_w;   float* rgb_b;
   float* output_w;  float* output_b;
 } NerfNetGrads;
-/* tensor-core backward (csrc/bwd_wg.cuh): compositing adjoint, wgmma dgrad chain with loss-scaled fp16
+/* Reproducibility of every backward entry point below (tensor-core and exact) and of mse_seed: no kernel adds floats
+ * atomically.  Sums that several blocks share are written as fp32 partials and added in a fixed order, so with the same
+ * build, GPU model and SM count, inputs, weights and seeds, the gradients (and the loss) are the same bits on every run,
+ * whatever else runs on the GPU and whatever the workspace and record buffers held before the call.  The order may
+ * depend on N, S, the network and the SM count (the tile plan does); results are not bit-equal across SM counts or GPU
+ * models, nor between the tensor-core and exact paths.
+ *
+ * tensor-core backward (csrc/bwd_wg.cuh): compositing adjoint, wgmma dgrad chain with loss-scaled fp16
  * activation gradients, layer-major wgmma weight gradient; consumes the records of the training-mode pass
  * and its raw [N,S,4].  Networks with view directions or with output_linear (output_ch >= 4; its rows >= 4 never
  * reach the loss and get no gradient). */
@@ -301,7 +308,8 @@ size_t nerf_b200_march_bwd_workspace_bytes(int64_t N, int S, const NerfNetParams
 
 /* ---- the two ends of the optimisation step (SURVEY 8f rank 2; csrc/train_step.cuh) ------------------------------
  *      mse_seed : img2mse (run_nerf_helpers.py:9; run_nerf.py:764-772): *loss_accum += mean((rgb - target)^2) and
- *                 g_rgb = 2 (rgb - target) / (3 N) * grad_scale  (grad_scale = 1 / world_size under data parallelism)
+ *                 g_rgb = 2 (rgb - target) / (3 N) * grad_scale  (grad_scale = 1 / world_size under data parallelism);
+ *                 the loss is summed by one block in a fixed order (the same bits on every run)
  *      adam_step: torch.optim.Adam(betas, eps) (run_nerf.py:207, :776) over one flat fp32 parameter buffer, with the
  *                 reference's learning-rate decay (run_nerf.py:778-783) evaluated on the device; state = float[4]:
  *                 [1] = steps taken so far, [2] = rate of the last step.  grads are multiplied by grad_mul first. ---- */

@@ -4,7 +4,8 @@
 // recomputed in fp32 with saved activations (mlp_simt_kernel, save mode), the compositing adjoint
 // (SURVEY App. E) gives dL/draw, and the MLP is walked backwards with two generic fp32 GEMMs
 // (dgrad: C = A B, wgrad: C += A^T B reduced over all sample rows), a ReLU-mask and a column-sum
-// kernel.  No gradient flows to rays / z (run_nerf.py:394, SURVEY 3.5).
+// kernel.  No gradient flows to rays / z (run_nerf.py:394, SURVEY 3.5).  Sums split over blocks are written as fp32 partials
+// and added in block order (sum_partials_kernel): no float atomics, the same bits on every run.
 // The tensor-core path (bwd_wg.cuh) is the default; this one serves exact mode and networks without view directions.
 #pragma once
 #include "common.cuh"
@@ -55,9 +56,11 @@ __global__ void __launch_bounds__(256) sgemm_nn_kernel(const float* __restrict__
 }
 
 // C[K1,N] (ldc) += A[M,K1]^T (lda) * B[M,N] (ldb), reduction over the M sample rows, split across
-// blockIdx.z slabs of `rows_per_slab` rows; partial tiles are combined with fp32 atomics.   -- wgrad
+// blockIdx.z slabs of `rows_per_slab` rows: with one slab the tile adds into C, else slab z writes part[z][K1][N]
+// (sum_partials_kernel adds the slabs in order).   -- wgrad
 __global__ void __launch_bounds__(256) sgemm_tn_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                      float* __restrict__ C, int ldc, long long M, int K1, int N, int rows_per_slab) {
+                                                      float* __restrict__ C, int ldc, long long M, int K1, int N, int rows_per_slab,
+                                                      float* __restrict__ part) {
   __shared__ float sA[GK][GT + 4], sB[GK][GT + 4];
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int i0 = blockIdx.x * GT, n0 = blockIdx.y * GT;
@@ -91,14 +94,17 @@ __global__ void __launch_bounds__(256) sgemm_tn_kernel(const float* __restrict__
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       int n = n0 + tx * 4 + j;
-      if (n < N) atomicAdd(C + (size_t)r * ldc + n, acc[i][j]);
+      if (n >= N) continue;
+      if (part) part[((size_t)blockIdx.z * K1 + r) * N + n] = acc[i][j];
+      else C[(size_t)r * ldc + n] += acc[i][j];
     }
   }
 }
 
-// d[m, c] *= (h[m, c] > 0)   (ReLU backward, in place), and colsum[c] += sum_m d[m, c]  (bias gradient)
+// d[m, c] *= (h[m, c] > 0)   (ReLU backward, in place), and colsum[c] += sum_m d[m, c]  (bias gradient): with one row block
+// straight into colsum, else block x writes part[x][C] (sum_partials_kernel adds the blocks in order)
 __global__ void relu_mask_colsum_kernel(float* __restrict__ d, int ldd, const float* __restrict__ h, int ldh,
-                                        long long M, int C, float* __restrict__ colsum, int rows_per_block) {
+                                        long long M, int C, float* __restrict__ colsum, int rows_per_block, float* __restrict__ part) {
   const int c = blockIdx.y * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const long long m0 = (long long)blockIdx.x * rows_per_block;
@@ -109,7 +115,17 @@ __global__ void relu_mask_colsum_kernel(float* __restrict__ d, int ldd, const fl
     if (h != nullptr) { v = (h[m * ldh + c] > 0.0f) ? v : 0.0f; d[m * ldd + c] = v; }
     s += v;
   }
-  if (colsum) atomicAdd(colsum + c, s);
+  if (part) part[(size_t)blockIdx.x * C + c] = s;
+  else if (colsum) colsum[c] += s;
+}
+
+// dst[r][c] (ld) += sum_p part[p][r][c], p = 0, 1, ... in order
+__global__ void sum_partials_kernel(const float* __restrict__ part, int nparts, int rows, int cols, float* __restrict__ dst, int ld) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= rows * cols) return;
+  float s = 0.f;
+  for (int q = 0; q < nparts; ++q) s += part[(size_t)q * rows * cols + idx];
+  dst[(size_t)(idx / cols) * ld + idx % cols] += s;
 }
 
 // activations saved by the exact forward (row-major fp32), all optional

@@ -18,14 +18,19 @@
 //                        CTAs are partitioned over 128-row blocks of the layers' dW so that each holds ONE block in registers
 //                        across all of its tiles and writes it once; bias gradients are the column sums of the dA tiles
 //                        while they sit in shared memory.
-//   wgrad_reduce_kernel  sums the per-CTA partial dW, un-scales, adds into the gradient tensors
-//                        (alpha_linear's gradient and the per-ray row sums of d_hv are computed by the wgrad kernel's MMA
-//                        warpgroups from the tiles it streams anyway)
+//   wgrad_reduce_kernel  sums the per-CTA partial dW, bias sums and head gradients in CTA order, un-scales, adds into the
+//                        gradient tensors (alpha_linear's gradient is computed by the wgrad kernel's MMA warpgroups from the
+//                        tiles it streams anyway)
+//   dhv_ray_sum_kernel   the per-ray row sums of d_hv, each ray's rows in order
 //   views_enc_wgrad_kernel  views_linears[0].weight[:, W:] from the per-ray sums and gamma(viewdir)
 //   views_feat_wgrad_kernel views_linears[0].weight[:, :W] = (d_hv^T h_{D-1}) W_feat^T + db_v b_feat^T (feature_linear's output is never stored)
 //
 // The weight gradient is layer-major because a layer's dW (256 x 256 fp32) is a whole register file: it cannot share a
 // kernel with the tile-major dgrad chain.  It streams the images once: 2 x 64 KB per tile-layer at 64 MAC/B -- HBM-bound.
+//
+// No kernel here adds floats atomically: every sum over rows that several blocks share is written as fp32 partials (one row
+// per block, CTA or warp quarter) and added up by a reduction in a fixed order, so that a pass's gradients are the same bits
+// on every run (for one tile plan, i.e. one N, S, network and SM count), whatever the scheduling.
 #pragma once
 #include "fused_tc.cuh"
 #include "fused_wg.cuh"
@@ -75,14 +80,16 @@ __global__ void encv_kernel(const float* __restrict__ dirs, int stride, long lon
 // rgb_linear's backward (run_nerf_helpers.py:114), both halves in one sweep over the rows:
 //   seed of the dgrad chain: d_hv[row][c] = scale * (hv[row][c] > 0) * sum_j d_rgb[row][j] W_rgb[j][c]   (c < 128), written as the
 //     first 32 KB of every tile's gradient record (rows beyond the CTA's range: zeros -- dgrad and wgrad rely on that);
-//   weight / bias gradient: dW_rgb[j][c] += sum_rows d_rgb[row][j] hv[row][c],  db_rgb[j] += sum_rows d_rgb[row][j]   (fp32)
+//   weight / bias gradient: block b's sums over its rows of d_rgb[row][j] hv[row][c] and d_rgb[row][j] (fp32) go to its partial row
+//     part[b][SEED_HEADS_PART] = (dW_rgb[3][128], db_rgb[3]); wgrad_reduce_kernel adds the rows in block order
 // One warp per row, lane = four columns: a row is 256 contiguous bytes of hv in and of d_hv out (two 128-byte lines each).
 // ---------------------------------------------------------------------------------------------------------------
+constexpr int SEED_HEADS_PART = 388;      // floats per block: 384 weights + 3 biases (+1: 16-byte rows)
 struct SeedParams {
   const float* d_raw; const uint8_t* mask; const uint8_t* act; uint8_t* grad; const float* rgb_w; const unsigned int* amax;
   long long N; int S, rays_per_cta, nst_plan, D;
   uint32_t rec_mask, rec_act, rec_grad; long long n_tiles;
-  float* g_rgb_w; float* g_rgb_b;
+  float* part;
 };
 
 __global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams p) {
@@ -151,10 +158,9 @@ __global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) v += s_acc[w][i];
-    if (i < 384) {                                      // i = (j * 4 + k) * 32 + lane  ->  weight[j][lane * 4 + k]
-      const int j = i / 128, k = (i / 32) & 3, ln = i & 31;
-      atomicAdd(p.g_rgb_w + j * 128 + ln * 4 + k, v);
-    } else atomicAdd(p.g_rgb_b + (i - 384), v);
+    int o = i;                                          // i = (j * 4 + k) * 32 + lane  ->  weight[j][lane * 4 + k]
+    if (i < 384) { const int j = i / 128, k = (i / 32) & 3, ln = i & 31; o = j * 128 + ln * 4 + k; }
+    p.part[(size_t)blockIdx.x * SEED_HEADS_PART + o] = v;
   }
 }
 
@@ -163,15 +169,17 @@ __global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams
 //   seed of the dgrad chain: dA_{D-1}[row][c] = (pre_{D-1}[row][c] > 0) * sum_{k<4} (scale d_raw[row][k]) W_out[k][c], written as
 //     the step-1 image of every tile's gradient record -- where the view-direction chain leaves dA_{D-1} too, so that dgrad and
 //     wgrad read one layout (rows beyond the CTA's range: zeros, they rely on that);
-//   weight / bias gradient: dW_out[k][c] += sum_rows d_raw[row][k] h_{D-1}[row][c],  db_out[k] += sum_rows d_raw[row][k]   (k < 4,
-//     fp32; rows >= 4 of a 5-output head never reach the loss (run_nerf.py:187) and keep their zero gradient)
+//   weight / bias gradient: block b's sums over its rows of d_raw[row][k] h_{D-1}[row][c] and d_raw[row][k] (k < 4, fp32) go to its
+//     partial row part[b][SEED_OUT_PART] = (dW_out[4][256], db_out[4]); wgrad_reduce_kernel adds the rows in block order (rows >= 4
+//     of a 5-output head never reach the loss (run_nerf.py:187) and keep their zero gradient)
 // One warp per row, lane = eight columns: a row is 512 contiguous bytes of h_{D-1} in and of dA_{D-1} out.
 // ---------------------------------------------------------------------------------------------------------------
+constexpr int SEED_OUT_PART = 1028;       // floats per block: 1024 weights + 4 biases
 struct SeedOutParams {
   const float* d_raw; const uint8_t* mask; const uint8_t* act; uint8_t* grad; const float* out_w; const unsigned int* amax;
   long long N; int S, rays_per_cta, nst_plan, D;
   uint32_t rec_mask, rec_act, rec_grad; long long n_tiles;
-  float* g_out_w; float* g_out_b;
+  float* part;
 };
 constexpr int SEED_OUT_BATCH = 4;         // rows of a warp whose loads are in flight together
 
@@ -251,10 +259,9 @@ __global__ void __launch_bounds__(256, 2) dA_seed_output_kernel(const SeedOutPar
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) v += s_acc[w][i];
-    if (i < 1024) {                                     // i = (k * 8 + e) * 32 + lane  ->  weight[k][lane * 8 + e]
-      const int k = i >> 8, e = (i >> 5) & 7, ln = i & 31;
-      atomicAdd(p.g_out_w + k * 256 + ln * 8 + e, v);
-    } else atomicAdd(p.g_out_b + (i - 1024), v);
+    int o = i;                                          // i = (k * 8 + e) * 32 + lane  ->  weight[k][lane * 8 + e]
+    if (i < 1024) { const int k = i >> 8, e = (i >> 5) & 7, ln = i & 31; o = k * 256 + ln * 8 + e; }
+    p.part[(size_t)blockIdx.x * SEED_OUT_PART + o] = v;
   }
 }
 
@@ -413,7 +420,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
 // tiles g, g + G, ...  Stage = one 64-row half tile of A's 128 columns and of B (one contiguous piece each in the record).
 // Warpgroup 0: one producer thread.  Warpgroups 1, 2: wgmma with both operands MN-major straight from the images, each on 64
 // of the block's rows (dW rows = A columns), the accumulator in registers for the whole launch; while the MMAs of a stage
-// run, the same threads form the bias gradient (column sums of A) and the job extras from the stage in shared memory.
+// run, the same threads form the bias gradient (column sums of A) and alpha_linear's gradient from the stage in shared memory.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int WG2_THREADS = 384, WG2_MAX_STAGES = 6, WG2_MAX_JOBS = 24;
 constexpr uint32_t WG2_RING = 196608,                  // ring: 4 stages of a 128 + 256 column job
@@ -424,16 +431,15 @@ struct WgradJob {
   int a_cols, m0;               // columns of the A image (128 | 256); first A column of this block (0 | 128)
   int Nc;                       // columns of B (64 | 128 | 256)
   int cta0, ncta;               // CTA range serving this job
-  float* db;                    // bias gradient of the whole layer (fp32, += scaled column sums of A; this block adds its 128) or NULL
   long long part_off;           // float offset of this job's partial blocks [ncta][128][Nc]
-  int aux;                      // 1: A = d_hv  -> per-ray row sums into aux_dst [N,128] (view columns of views_linears[0])
-                                // 2: B = h_{D-1} -> aux_dst[c] += sum_rows d_sigma[row] B[row][c]  (alpha_linear.weight), aux_b += sum d_sigma
-  float* aux_dst; float* aux_b;
+  long long db_off;             // -1, or float offset of the scaled column sums of A (bias gradient) [ncta][4][128]
+  long long alpha_off;          // -1, or (B = h_{D-1}) float offset of alpha_linear's partials: [ncta][2][256] weight
+                                // (sum_rows d_sigma[row] B[row][c]), then [ncta][2] bias (sum_rows d_sigma[row])
 };
 struct WgradParams {
   const uint8_t* act; const uint8_t* grad; uint32_t rec_act, rec_grad;
   long long N; int S, rays_per_cta, nst_plan; long long n_tiles;
-  const unsigned int* amax; float* partial; const float* d_raw; int njobs;
+  float* partial; const float* d_raw; int njobs;
   long long t0, t1;             // tiles [t0, t1) of the plan (a launch may cover part of a pass; the reduction adds up)
   WgradJob jobs[WG2_MAX_JOBS];
 };
@@ -453,9 +459,8 @@ __device__ __forceinline__ void wgrad_consumer(const WgradParams& p, const Wgrad
                                                uint32_t nstg, uint32_t bar_full, uint32_t bar_empty) {
   constexpr int R = NC / 2;
   const int w = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
-  const float inv = 1.0f / loss_scale_from_absmax(__uint_as_float(*p.amax));
   const int cp = t & 31;                                  // column pair of the bias sums: A columns m0 + 64 w + 2 cp, rows 16 wq ..
-  const int cp2 = t & 63, rh = t >> 6;                    // aux == 2: B columns 128 w + 2 cp2, rows 32 rh ..
+  const int cp2 = t & 63, rh = t >> 6;                    // alpha_linear: B columns 128 w + 2 cp2, rows 32 rh ..
   float acc[R];
 #pragma unroll
   for (int i = 0; i < R; ++i) acc[i] = 0.f;
@@ -471,7 +476,7 @@ __device__ __forceinline__ void wgrad_consumer(const WgradParams& p, const Wgrad
       const int lr0 = st * 256 + X * 128 + h * 64;
       const uint32_t xb = sb + s * stride, yb = xb + 16384u;
       float dsv = 0.f;
-      if (job.aux == 2) { const int lr = lr0 + 32 * rh + lane; dsv = lr < nrows ? p.d_raw[(row_begin + lr) * 4 + 3] : 0.f; }
+      if (job.alpha_off >= 0) { const int lr = lr0 + 32 * rh + lane; dsv = lr < nrows ? p.d_raw[(row_begin + lr) * 4 + 3] : 0.f; }
       ptx::mbar_wait(bar_full + 8 * s, ph);
       ptx::wgmma_fence();
 #pragma unroll
@@ -485,33 +490,16 @@ __device__ __forceinline__ void wgrad_consumer(const WgradParams& p, const Wgrad
       }
       ptx::wgmma_commit();
       any = true;
-      // while the MMAs run: column sums of this warpgroup's 64 A columns (bias gradient) and per-ray sums (views job)
-      if (job.db != nullptr || job.aux == 1) {
+      // while the MMAs run: column sums of this warpgroup's 64 A columns (bias gradient)
+      if (job.db_off >= 0) {
         const uint32_t abase = xb + (uint32_t)w * 8192u;
-        float r0s = 0.f, r1s = 0.f;
-        int ray = -1;
         for (int i = 0; i < 16; ++i) {
-          const int r = 16 * wq + i, lr = lr0 + r;
-          const uint32_t v = ptx::ld_shared_b32(abase + kblock_off(r, 2 * cp));
+          const uint32_t v = ptx::ld_shared_b32(abase + kblock_off(16 * wq + i, 2 * cp));
           const __half2 hh = *reinterpret_cast<const __half2*>(&v);
-          const float lo = __low2float(hh), hi = __high2float(hh);
-          s0 += lo; s1 += hi;
-          if (job.aux == 1 && lr < nrows) {                  // rows past the CTA's range are zero: skipped
-            const int rl = lr / p.S;
-            if (rl != ray && ray >= 0) {
-              float* d = job.aux_dst + ((long long)cta * p.rays_per_cta + ray) * 128 + job.m0 + 64 * w + 2 * cp;
-              atomicAdd(d, r0s * inv); atomicAdd(d + 1, r1s * inv);
-              r0s = r1s = 0.f;
-            }
-            ray = rl; r0s += lo; r1s += hi;
-          }
-        }
-        if (ray >= 0) {
-          float* d = job.aux_dst + ((long long)cta * p.rays_per_cta + ray) * 128 + job.m0 + 64 * w + 2 * cp;
-          atomicAdd(d, r0s * inv); atomicAdd(d + 1, r1s * inv);
+          s0 += __low2float(hh); s1 += __high2float(hh);
         }
       }
-      if (job.aux == 2) {                                  // alpha_linear.weight: sum_rows d_sigma[row] h_{D-1}[row][c]
+      if (job.alpha_off >= 0) {                                  // alpha_linear.weight: sum_rows d_sigma[row] h_{D-1}[row][c]
         const int c = 128 * w + 2 * cp2;
         const uint32_t bbase = yb + (uint32_t)(c >> 6) * 8192u;
 #pragma unroll 8
@@ -530,12 +518,12 @@ __device__ __forceinline__ void wgrad_consumer(const WgradParams& p, const Wgrad
       if (++s == nstg) { s = 0; ph ^= 1; }
     }
   }
-  if (any) {
-    if (job.db != nullptr) { float* d = job.db + job.m0 + 64 * w + 2 * cp; atomicAdd(d, s0 * inv); atomicAdd(d + 1, s1 * inv); }
-    if (job.aux == 2) {
-      atomicAdd(job.aux_dst + 128 * w + 2 * cp2, a0); atomicAdd(job.aux_dst + 128 * w + 2 * cp2 + 1, a1);
-      if (w == 0 && cp2 == 0) atomicAdd(job.aux_b, bsum);
-    }
+  // every CTA writes all of its partials (zeros when it had no tiles): the reduction reads them all
+  if (job.db_off >= 0)
+    *reinterpret_cast<float2*>(p.partial + job.db_off + ((size_t)g * 4 + wq) * 128 + 64 * w + 2 * cp) = make_float2(s0, s1);
+  if (job.alpha_off >= 0) {
+    *reinterpret_cast<float2*>(p.partial + job.alpha_off + ((size_t)g * 2 + rh) * 256 + 128 * w + 2 * cp2) = make_float2(a0, a1);
+    if (w == 0 && cp2 == 0) p.partial[job.alpha_off + (size_t)G * 512 + g * 2 + rh] = bsum;
   }
   float* part = p.partial + job.part_off + (size_t)g * 128 * NC;
   const int q4 = lane & 3, rr = 64 * w + 16 * wq + (lane >> 2);
@@ -592,9 +580,11 @@ __global__ void __launch_bounds__(WG2_THREADS, 1) wgrad_wg_kernel(const WgradPar
   else wgrad_consumer<64>(p, job, g, G, sb, stride, nstg, bar_full, bar_empty);
 }
 
-// dst[o][i] += inv_scale * sum_g partial[g][o][i]   (i < n_valid; dst row stride ldw)
-struct ReduceJob { long long part_off; int ncta, Mc, Nc, n_valid, ldw; float* dst; };   // Mc = 128: one block
-struct ReduceParams { const float* partial; const unsigned int* amax; int njobs; ReduceJob jobs[WG2_MAX_JOBS]; };
+// dst[o][i] += (scaled ? inv_scale : 1) * sum_g partial[g][o][i], g = 0, 1, ... in order   (i < n_valid; dst row stride ldw;
+// partial rows g are gstride floats apart).  A dW job has Mc = 128 (one block); the others are bias and head gradients.
+struct ReduceJob { long long part_off, gstride; int ncta, Mc, Nc, n_valid, ldw, scaled; float* dst; };
+constexpr int WG2_MAX_REDUCE = 56;        // dW blocks, their bias sums, alpha_linear and the seed kernels' heads
+struct ReduceParams { const float* partial; const unsigned int* amax; int njobs; ReduceJob jobs[WG2_MAX_REDUCE]; };
 
 __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams p) {
   const ReduceJob j = p.jobs[blockIdx.y];
@@ -604,28 +594,63 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams p)
   if (i >= j.n_valid) return;
   const float* src = p.partial + j.part_off + idx;
   float s = 0.f;
-  for (int g = 0; g < j.ncta; ++g) s += src[(size_t)g * j.Mc * j.Nc];
-  const float inv = 1.0f / loss_scale_from_absmax(__uint_as_float(*p.amax));
+  for (int g = 0; g < j.ncta; ++g) s += src[(size_t)g * j.gstride];
+  const float inv = j.scaled ? 1.0f / loss_scale_from_absmax(__uint_as_float(*p.amax)) : 1.0f;
   j.dst[(size_t)o * j.ldw + i] += s * inv;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// the view columns of views_linears[0] (alpha_linear and the per-ray sums of d_hv ride along in the wgrad kernel, whose tiles
-// already hold their operands; rgb_linear's gradient comes from dhv_seed_heads_kernel)
+// the view columns of views_linears[0] (alpha_linear rides along in the wgrad kernel, whose tiles already hold its operands;
+// rgb_linear's gradient comes from dhv_seed_heads_kernel)
 // ---------------------------------------------------------------------------------------------------------------
-// views_linears[0].weight[c][W + e] += sum_rays dsum[ray][c] * gamma(viewdir_ray)[e]      (run_nerf_helpers.py:108-110);
-// block e == ICV: dbv[c] += sum_rays dsum[ray][c]  (this pass's bias gradient of views_linears[0], for the kernel below)
+// dsum[ray][c] = inv_scale * sum over the ray's rows, in order, of d_hv[row][c]: one warp per ray, lane = four columns, walking the
+// ray's rows through the tile plan in the d_hv seed images (offset 0 of each gradient record).  A ray's rows may span tiles and
+// super-tiles but never CTAs (whole rays per CTA).
+constexpr int DSUM_BATCH = 8;             // rows of a warp whose loads are in flight together
+__global__ void __launch_bounds__(256) dhv_ray_sum_kernel(const uint8_t* __restrict__ grad, uint32_t rec_grad, long long N, int S,
+                                                        int rays_per_cta, int nst_plan, const unsigned int* __restrict__ amax,
+                                                        float* __restrict__ dsum) {
+  const long long n = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (n >= N) return;
+  const int c = (threadIdx.x & 31) * 4;
+  const int cta = (int)(n / rays_per_cta), lr0 = (int)(n - (long long)cta * rays_per_cta) * S;
+  const uint8_t* rec = grad + (size_t)cta * nst_plan * 2 * rec_grad;      // the CTA's tiles: local row lr is in tile lr >> 7
+  float s[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int k0 = 0; k0 < S; k0 += DSUM_BATCH) {
+    uint2 v[DSUM_BATCH];
+#pragma unroll
+    for (int k = 0; k < DSUM_BATCH; ++k) {
+      const int lr = lr0 + k0 + k;
+      v[k] = (k0 + k < S) ? *reinterpret_cast<const uint2*>(rec + (size_t)(lr >> 7) * rec_grad + img_off(lr & 127, c, 128)) : make_uint2(0u, 0u);
+    }
+#pragma unroll
+    for (int k = 0; k < DSUM_BATCH; ++k) {
+      if (k0 + k < S) {
+        const __half2 h01 = *reinterpret_cast<const __half2*>(&v[k].x), h23 = *reinterpret_cast<const __half2*>(&v[k].y);
+        s[0] += __low2float(h01); s[1] += __high2float(h01); s[2] += __low2float(h23); s[3] += __high2float(h23);
+      }
+    }
+  }
+  const float inv = 1.0f / loss_scale_from_absmax(__uint_as_float(*amax));
+  *reinterpret_cast<float4*>(dsum + n * 128 + c) = make_float4(s[0] * inv, s[1] * inv, s[2] * inv, s[3] * inv);
+}
+
+// Block (e, b) sums over the rays [b R, (b + 1) R): part[b][c][e] = sum dsum[ray][c] * gamma(viewdir_ray)[e] for e < ICV (the view
+// columns of views_linears[0].weight, run_nerf_helpers.py:108-110), and part[b][ICV][c] = sum dsum[ray][c] (this pass's bias
+// gradient of views_linears[0], for views_feat_wgrad_kernel).  gridDim.y is set by the SM count, not by N; wgrad_reduce_kernel
+// adds the blocks' rows in order.  part: [gridDim.y][(ICV + 1) * 128]
 __global__ void __launch_bounds__(128) views_enc_wgrad_kernel(const float* __restrict__ dsum, const float* __restrict__ encv, long long N, int ICV,
-                                                            float* __restrict__ views_w, int ld, int col0, float* __restrict__ dbv) {
+                                                            long long R, float* __restrict__ part) {
   const int e = blockIdx.x, c = threadIdx.x;
-  const long long n0 = (long long)blockIdx.y * 64, n1 = (n0 + 64 < N) ? n0 + 64 : N;
+  const long long n0 = (long long)blockIdx.y * R, n1 = (n0 + R < N) ? n0 + R : N;
+  float* row = part + (size_t)blockIdx.y * (ICV + 1) * 128;
   float s = 0.f;
   if (e < ICV) {
     for (long long n = n0; n < n1; ++n) s = fmaf(dsum[n * 128 + c], encv[n * ICV + e], s);
-    atomicAdd(views_w + (size_t)c * ld + col0 + e, s);
+    row[c * ICV + e] = s;
   } else {
     for (long long n = n0; n < n1; ++n) s += dsum[n * 128 + c];
-    atomicAdd(dbv + c, s);
+    row[ICV * 128 + c] = s;
   }
 }
 

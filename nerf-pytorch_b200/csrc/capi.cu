@@ -620,19 +620,36 @@ static int gemm_nn(const float* A, int lda, const float* B, int ldb, float* C, i
   NB_LAUNCH_OK("sgemm_nn_kernel");
   return 0;
 }
-static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, long long M, int K1, int N, cudaStream_t st) {
-  const int slab = 2048;
-  dim3 grid(cdiv(K1, GT), cdiv(N, GT), cdiv(M, slab));
-  sgemm_tn_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, K1, N, slab);
-  NB_LAUNCH_OK("sgemm_tn_kernel");
+// The two row-reductions below split M over slabs / blocks; with more than one, their partials go to `scratch` (one of the
+// pass's [M, W] buffers that is free at the call) and sum_partials_kernel adds them in order.  The partials fit: slabs need
+// cdiv(M, 2048) * K1 * N <= M * W floats (K1 <= W, and N <= 1024 <= M / cdiv(M, 2048) when M > 2048); blocks need
+// cdiv(M, 256) * C <= M * W floats (C <= W).
+static int sum_partials(const float* part, int nparts, int rows, int cols, float* dst, int ld, cudaStream_t st) {
+  sum_partials_kernel<<<cdiv((long long)rows * cols, 256), 256, 0, st>>>(part, nparts, rows, cols, dst, ld);
+  NB_LAUNCH_OK("sum_partials_kernel");
   return 0;
 }
-static int mask_colsum(float* d, int ldd, const float* h, int ldh, long long M, int C, float* colsum, cudaStream_t st) {
+static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, long long M, int K1, int N, float* scratch,
+                   long long scratch_floats, cudaStream_t st) {
+  const int slab = 2048;
+  const int nslab = cdiv(M, slab);
+  float* part = nslab > 1 ? scratch : nullptr;
+  NB_CHECK_ARG(nslab == 1 || (long long)nslab * K1 * N <= scratch_floats, "internal: wgrad partials do not fit the scratch buffer");
+  dim3 grid(cdiv(K1, GT), cdiv(N, GT), nslab);
+  sgemm_tn_kernel<<<grid, 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, K1, N, slab, part);
+  NB_LAUNCH_OK("sgemm_tn_kernel");
+  return part ? sum_partials(part, nslab, K1, N, C, ldc, st) : 0;
+}
+static int mask_colsum(float* d, int ldd, const float* h, int ldh, long long M, int C, float* colsum, float* scratch,
+                       long long scratch_floats, cudaStream_t st) {
   const int rpb = 256;
-  dim3 grid(cdiv(M, rpb), cdiv(C, 64));
-  relu_mask_colsum_kernel<<<grid, 64, 0, st>>>(d, ldd, h, ldh, M, C, colsum, rpb);
+  const int nblk = cdiv(M, rpb);
+  float* part = nblk > 1 ? scratch : nullptr;
+  NB_CHECK_ARG(nblk == 1 || (long long)nblk * C <= scratch_floats, "internal: column-sum partials do not fit the scratch buffer");
+  dim3 grid(nblk, cdiv(C, 64));
+  relu_mask_colsum_kernel<<<grid, 64, 0, st>>>(d, ldd, h, ldh, M, C, colsum, rpb, part);
   NB_LAUNCH_OK("relu_mask_colsum_kernel");
-  return 0;
+  return part ? sum_partials(part, nblk, 1, C, colsum, C, st) : 0;
 }
 #define NB_TRY(expr) do { if (int rc__ = (expr)) return rc__; } while (0)
 
@@ -679,43 +696,44 @@ static int march_bwd_impl(const float* rays, const float* z_vals, const float* n
     // 2. compositing adjoint -> dL/draw
     NB_TRY(raw2outputs_bwd_impl(raw, zz, ry + 3, rs, nz, nn, S, cfg->white_bkgd, seeds_at(g, n0, S), nullptr, d_raw, st));
     const float* h_last = sv.h + (size_t)(D - 1) * M * W;
+    const long long sc = M * W;                      // floats of each [M, W] buffer: the partials' scratch is one that is free
     if (net->use_viewdirs) {
       // 3. rgb_linear (run_nerf_helpers.py:114)
-      NB_TRY(gemm_tn(d_raw, 4, sv.hv, W2, grads->rgb_w, W2, M, 3, W2, st));
-      NB_TRY(mask_colsum(d_raw, 4, nullptr, 0, M, 3, grads->rgb_b, st));
+      NB_TRY(gemm_tn(d_raw, 4, sv.hv, W2, grads->rgb_w, W2, M, 3, W2, dh0, sc, st));
+      NB_TRY(mask_colsum(d_raw, 4, nullptr, 0, M, 3, grads->rgb_b, dh0, sc, st));
       NB_TRY(gemm_nn(d_raw, 4, net->rgb_w, W2, d_hv, W2, M, W2, 3, 0, st));
       // 4. views_linears[0] on cat([feature, input_views]) (:108-112)
-      NB_TRY(mask_colsum(d_hv, W2, sv.hv, W2, M, W2, grads->views_b, st));
-      NB_TRY(gemm_tn(d_hv, W2, sv.feat, W, grads->views_w, W + ICV, M, W2, W, st));
-      NB_TRY(gemm_tn(d_hv, W2, sv.encv, ICV, grads->views_w + W, W + ICV, M, W2, ICV, st));
+      NB_TRY(mask_colsum(d_hv, W2, sv.hv, W2, M, W2, grads->views_b, dh0, sc, st));
+      NB_TRY(gemm_tn(d_hv, W2, sv.feat, W, grads->views_w, W + ICV, M, W2, W, dh0, sc, st));
+      NB_TRY(gemm_tn(d_hv, W2, sv.encv, ICV, grads->views_w + W, W + ICV, M, W2, ICV, dh0, sc, st));
       NB_TRY(gemm_nn(d_hv, W2, net->views_w, W + ICV, dh0, W, M, W, W2, 0, st));                // d_feature
       // 5. feature_linear and alpha_linear both read the last hidden layer (:106-107)
-      NB_TRY(gemm_tn(dh0, W, h_last, W, grads->feature_w, W, M, W, W, st));
-      NB_TRY(mask_colsum(dh0, W, nullptr, 0, M, W, grads->feature_b, st));
-      NB_TRY(gemm_tn(d_raw + 3, 4, h_last, W, grads->alpha_w, W, M, 1, W, st));
-      NB_TRY(mask_colsum(d_raw + 3, 4, nullptr, 0, M, 1, grads->alpha_b, st));
+      NB_TRY(gemm_tn(dh0, W, h_last, W, grads->feature_w, W, M, W, W, dh1, sc, st));
+      NB_TRY(mask_colsum(dh0, W, nullptr, 0, M, W, grads->feature_b, dh1, sc, st));
+      NB_TRY(gemm_tn(d_raw + 3, 4, h_last, W, grads->alpha_w, W, M, 1, W, dh1, sc, st));
+      NB_TRY(mask_colsum(d_raw + 3, 4, nullptr, 0, M, 1, grads->alpha_b, dh1, sc, st));
       NB_TRY(gemm_nn(dh0, W, net->feature_w, W, dh1, W, M, W, W, 0, st));
       NB_TRY(gemm_nn(d_raw + 3, 4, net->alpha_w, W, dh1, W, M, W, 1, 1, st));
     } else {
       // 3'. output_linear (:117): only its first four rows ever reach the loss (run_nerf.py:187 note); rows >= 4 get zero gradient
-      NB_TRY(gemm_tn(d_raw, 4, h_last, W, grads->output_w, W, M, 4, W, st));
-      NB_TRY(mask_colsum(d_raw, 4, nullptr, 0, M, 4, grads->output_b, st));
+      NB_TRY(gemm_tn(d_raw, 4, h_last, W, grads->output_w, W, M, 4, W, dh0, sc, st));
+      NB_TRY(mask_colsum(d_raw, 4, nullptr, 0, M, 4, grads->output_b, dh0, sc, st));
       NB_TRY(gemm_nn(d_raw, 4, net->output_w, W, dh1, W, M, W, 4, 0, st));
     }
     // 6. pts_linears, last to first (:99-103); skip layer input = cat([input_pts, h])
     float* dcur = dh1;
     float* dnext = dh0;
     for (int l = D - 1; l >= 0; --l) {
-      NB_TRY(mask_colsum(dcur, W, sv.h + (size_t)l * M * W, W, M, W, grads->pts_b[l], st));
+      NB_TRY(mask_colsum(dcur, W, sv.h + (size_t)l * M * W, W, M, W, grads->pts_b[l], dnext, sc, st));
       const bool after_skip = (l > 0) && (l - 1 == net->skip);
       const int Kl = (l == 0) ? IC : (after_skip ? W + IC : W);
       if (l == 0) {
-        NB_TRY(gemm_tn(dcur, W, sv.enc, IC, grads->pts_w[0], Kl, M, W, IC, st));
+        NB_TRY(gemm_tn(dcur, W, sv.enc, IC, grads->pts_w[0], Kl, M, W, IC, dnext, sc, st));
       } else {
         const float* hprev = sv.h + (size_t)(l - 1) * M * W;
         const int off = after_skip ? IC : 0;
-        if (after_skip) NB_TRY(gemm_tn(dcur, W, sv.enc, IC, grads->pts_w[l], Kl, M, W, IC, st));
-        NB_TRY(gemm_tn(dcur, W, hprev, W, grads->pts_w[l] + off, Kl, M, W, W, st));
+        if (after_skip) NB_TRY(gemm_tn(dcur, W, sv.enc, IC, grads->pts_w[l], Kl, M, W, IC, dnext, sc, st));
+        NB_TRY(gemm_tn(dcur, W, hprev, W, grads->pts_w[l] + off, Kl, M, W, W, dnext, sc, st));
         NB_TRY(gemm_nn(dcur, W, net->pts_w[l] + off, Kl, dnext, W, M, W, W, 0, st));
         float* t = dcur; dcur = dnext; dnext = t;
       }
@@ -742,10 +760,20 @@ int nerf_b200_march_bwd_outs(const float* rays, const float* z_vals, const float
 // ---- tensor-core backward of one pass (bwd_wg.cuh) ------------------------------------------------
 namespace {
 struct BwdTcLayout { size_t off_amax, off_draw, off_encv, off_dsum, off_gv, off_partial, off_grad, total; long long part_floats; };
-struct BwdTcJobs { int n; bool overflow; WgradJob w[WG2_MAX_JOBS]; ReduceJob r[WG2_MAX_JOBS]; int total_ctas; long long part_floats; };
+// r[0, n): the dW blocks' reductions (r[i] belongs to w[i]); r[n, nr): the bias sums', alpha_linear's and the seed kernels'
+struct BwdTcJobs {
+  int n, nr; bool overflow; WgradJob w[WG2_MAX_JOBS]; float* db[WG2_MAX_JOBS]; ReduceJob r[WG2_MAX_REDUCE]; int total_ctas;
+  long long part_floats, extra_end;
+  void reduce(long long off, long long gstride, int nparts, int Nc, float* dst, int scaled) {   // dst[i] += sum of nparts rows
+    ReduceJob& q = r[nr++];
+    q.part_off = off; q.gstride = gstride; q.ncta = nparts; q.Mc = 1; q.Nc = Nc; q.n_valid = Nc; q.ldw = Nc; q.dst = dst; q.scaled = scaled;
+  }
+};
 
 // jobs of the weight gradient (128-row blocks of dW) and their CTA ranges (proportional to the bytes each job streams per tile).
 // Every job gets at least one CTA: the caller rejects `sms` < J.n (and J.overflow: more jobs than WG2_MAX_JOBS).
+// The dW blocks take the partial region's lower half (at most sms x 128 x 256 floats); the bias sums and alpha_linear's partials
+// follow from sms x 128 x 256 up to J.extra_end.
 BwdTcJobs make_bwd_jobs(const NerfNetParams& n, const NerfNetGrads* g, int sms) {
   BwdTcJobs J;
   memset(&J, 0, sizeof(J));
@@ -755,8 +783,9 @@ BwdTcJobs make_bwd_jobs(const NerfNetParams& n, const NerfNetGrads* g, int sms) 
       if (J.n == WG2_MAX_JOBS) { J.overflow = true; return; }
       WgradJob& w = J.w[J.n];
       ReduceJob& r = J.r[J.n];
-      w.a_off = a_off; w.a_cols = Mc; w.m0 = m0; w.b_off = b_off; w.Nc = Nc; w.db = db; w.aux = 0; w.aux_dst = nullptr; w.aux_b = nullptr;
-      r.Mc = 128; r.Nc = Nc; r.n_valid = n_valid; r.ldw = ldw; r.dst = dst ? dst + (size_t)m0 * ldw : nullptr;
+      w.a_off = a_off; w.a_cols = Mc; w.m0 = m0; w.b_off = b_off; w.Nc = Nc; w.db_off = -1; w.alpha_off = -1;
+      J.db[J.n] = db ? db + m0 : nullptr;
+      r.Mc = 128; r.Nc = Nc; r.scaled = 1; r.n_valid = n_valid; r.ldw = ldw; r.dst = dst ? dst + (size_t)m0 * ldw : nullptr;
       ++J.n;
     }
   };
@@ -802,10 +831,26 @@ BwdTcJobs make_bwd_jobs(const NerfNetParams& n, const NerfNetGrads* g, int sms) 
   long long pf = 0;
   for (int i = 0; i < J.n; ++i) {
     J.w[i].cta0 = cta; cta += J.w[i].ncta;
-    J.w[i].part_off = pf; J.r[i].part_off = pf; J.r[i].ncta = J.w[i].ncta;
+    J.w[i].part_off = pf; J.r[i].part_off = pf; J.r[i].gstride = 128LL * J.w[i].Nc; J.r[i].ncta = J.w[i].ncta;
     pf += (long long)J.w[i].ncta * 128 * J.w[i].Nc;
   }
   J.total_ctas = cta; J.part_floats = pf;
+  J.nr = J.n;
+  long long xf = (long long)sms * 128 * 256;
+  for (int i = 0; i < J.n; ++i) {
+    if (!J.db[i]) continue;
+    J.w[i].db_off = xf;                              // [ncta][4 warp quarters][128]
+    J.reduce(xf, 128, 4 * J.w[i].ncta, 128, J.db[i], 1);
+    xf += 512LL * J.w[i].ncta;
+  }
+  if (n.use_viewdirs && g) {                         // feature job, first block: alpha_linear
+    const int G = J.w[1].ncta;
+    J.w[1].alpha_off = xf;                           // [G][2 row halves][256] weight, then [G][2] bias
+    J.reduce(xf, 256, 2 * G, 256, g->alpha_w, 0);
+    J.reduce(xf + 512LL * G, 1, 2 * G, 1, g->alpha_b, 0);
+    xf += 514LL * G;
+  }
+  J.extra_end = xf;
   return J;
 }
 
@@ -857,8 +902,9 @@ namespace {
 struct BwdTcPass {
   const float* rays; const float* z; const float* noise; int64_t N; int S; const NerfNetParams* net; const void* packed;
   const NerfRenderCfg* cfg; const float* raw; const NerfTrainSave* save; NerfOutGrads seeds; const NerfNetGrads* grads;
-  DeviceState* ds; TilePlan plan; BwdTcLayout LY; PackLayout PL;
+  DeviceState* ds; TilePlan plan; BwdTcLayout LY; PackLayout PL; BwdTcJobs J;
   unsigned int* amax; float *d_raw, *encv, *dsum, *gv, *dbv, *partial; uint8_t* grec; const uint8_t *act, *mask;
+  int seed_grid; long long seed_off, views_rays;      // seed kernels: blocks, partial rows from `seed_off`; rays per views block
 
   int init(void* workspace, size_t workspace_bytes) {
     ds = device_state();
@@ -879,6 +925,19 @@ struct BwdTcPass {
     grec = ws + LY.off_grad;
     act = static_cast<const uint8_t*>(save->act);
     mask = static_cast<const uint8_t*>(save->mask);
+    // every partial sum lives in the partial region (sms x 256 x 256 floats): the dW blocks in its lower half, above them the bias
+    // and alpha_linear partials, then the seed kernels' rows; the views kernel's rows reuse the upper half once those are reduced
+    const int sms = ds->sms;
+    J = make_bwd_jobs(*net, grads, sms);
+    NB_CHECK_ARG(!J.overflow && J.n <= sms, "weight gradient: %d jobs need at least as many CTAs (have %d; at most %d jobs)", J.n, sms, WG2_MAX_JOBS);
+    const long long cap = (long long)sms * 256 * 256, upper = (long long)sms * 128 * 256;
+    seed_grid = (int)(plan.n_tiles < (net->use_viewdirs ? 3 : 2) * sms ? plan.n_tiles : (net->use_viewdirs ? 3 : 2) * sms);
+    seed_off = J.extra_end;
+    const long long seed_floats = (long long)seed_grid * (net->use_viewdirs ? SEED_HEADS_PART : SEED_OUT_PART);
+    views_rays = (N + sms - 1) / sms;
+    const long long views_floats = net->use_viewdirs ? (long long)sms * (net->input_ch_views + 1) * 128 : 0;
+    NB_CHECK_ARG(J.part_floats <= upper && seed_off + seed_floats <= cap && upper + views_floats <= cap,
+                 "internal: backward partials exceed the partial region");
     if (!ds->optin_bwd) {
       NB_TRY(smem_optin((const void*)dgrad_wg_kernel, SM_ALLOC));
       NB_TRY(smem_optin((const void*)wgrad_wg_kernel, WG2_TOTAL));
@@ -891,12 +950,9 @@ struct BwdTcPass {
   // is the only seed, else from the adjoint's max over all effective seeds;  2. seed of the chain: d_hv tiles, or
   // without view directions dA_{D-1} tiles (+ output_linear's gradient).  Both read amax after the adjoint, on the same stream.
   int prologue(cudaStream_t st) {
-    const int sms = ds->sms, D = net->D;
+    const int D = net->D;
     NB_CUDA(cudaMemsetAsync(amax, 0, 256, st));
-    if (net->use_viewdirs) {
-      NB_CUDA(cudaMemsetAsync(dsum, 0, (size_t)N * 128 * 4, st));
-      NB_CUDA(cudaMemsetAsync(gv, 0, (size_t)(128 * 256 + 128) * 4, st));
-    }
+    if (net->use_viewdirs) NB_CUDA(cudaMemsetAsync(gv, 0, (size_t)(128 * 256 + 128) * 4, st));
     if (seeds_rgb_only(seeds)) {
       absmax_kernel<<<cdiv(N * 3, 1024) < 64 ? cdiv(N * 3, 1024) : 64, 256, 0, st>>>(seeds.rgb_map, N * 3, amax);
       NB_LAUNCH_OK("absmax_kernel");
@@ -909,18 +965,22 @@ struct BwdTcPass {
       so.d_raw = d_raw; so.mask = mask; so.act = act; so.grad = grec; so.out_w = net->output_w; so.amax = amax;
       so.N = N; so.S = S; so.rays_per_cta = plan.rays_per_cta; so.nst_plan = plan.nst; so.D = D;
       so.rec_mask = rec_mask_bytes(D); so.rec_act = rec_act_bytes(D); so.rec_grad = rec_grad_bytes(D); so.n_tiles = plan.n_tiles;
-      so.g_out_w = grads->output_w; so.g_out_b = grads->output_b;
-      dA_seed_output_kernel<<<(int)(plan.n_tiles < 2 * sms ? plan.n_tiles : 2 * sms), 256, 0, st>>>(so);
+      so.part = partial + seed_off;
+      dA_seed_output_kernel<<<seed_grid, 256, 0, st>>>(so);
       NB_LAUNCH_OK("dA_seed_output_kernel");
+      J.reduce(seed_off, SEED_OUT_PART, seed_grid, 1024, grads->output_w, 0);
+      J.reduce(seed_off + 1024, SEED_OUT_PART, seed_grid, 4, grads->output_b, 0);
       return 0;
     }
     SeedParams sp;
     sp.d_raw = d_raw; sp.mask = mask; sp.act = act; sp.grad = grec; sp.rgb_w = net->rgb_w; sp.amax = amax;
     sp.N = N; sp.S = S; sp.rays_per_cta = plan.rays_per_cta; sp.nst_plan = plan.nst; sp.D = D;
     sp.rec_mask = rec_mask_bytes(D); sp.rec_act = rec_act_bytes(D); sp.rec_grad = rec_grad_bytes(D); sp.n_tiles = plan.n_tiles;
-    sp.g_rgb_w = grads->rgb_w; sp.g_rgb_b = grads->rgb_b;
-    dhv_seed_heads_kernel<<<(int)(plan.n_tiles < 3 * sms ? plan.n_tiles : 3 * sms), 256, 0, st>>>(sp);
+    sp.part = partial + seed_off;
+    dhv_seed_heads_kernel<<<seed_grid, 256, 0, st>>>(sp);
     NB_LAUNCH_OK("dhv_seed_heads_kernel");
+    J.reduce(seed_off, SEED_HEADS_PART, seed_grid, 384, grads->rgb_w, 0);
+    J.reduce(seed_off + 384, SEED_HEADS_PART, seed_grid, 3, grads->rgb_b, 0);
     return 0;
   }
 
@@ -955,24 +1015,18 @@ struct BwdTcPass {
     return 0;
   }
 
-  // 4. weight gradients (layer-major) + bias gradients on all SMs, then the reduction of the per-CTA partial blocks (adds into
-  // the gradient tensors)
+  // 4. weight gradients (layer-major) + bias gradients on all SMs, then the reduction of the per-CTA partials (and of the seed
+  // kernels' partial rows) in CTA order (adds into the gradient tensors)
   int wgrad(cudaStream_t st) {
-    const int ctas = ds->sms, vc0 = 0, vc1 = plan.grid;
+    const int vc0 = 0, vc1 = plan.grid;
     const int D = net->D;
-    BwdTcJobs J = make_bwd_jobs(*net, grads, ctas);
-    NB_CHECK_ARG(!J.overflow && J.n <= ctas, "weight gradient: %d jobs need at least as many CTAs (have %d; at most %d jobs)", J.n, ctas, WG2_MAX_JOBS);
     const bool views = net->use_viewdirs != 0;
-    if (views) {
-      J.w[0].aux = 1; J.w[0].aux_dst = dsum;            // views job: per-ray row sums of d_hv
-      J.w[1].aux = 2; J.w[1].aux_dst = grads->alpha_w; J.w[1].aux_b = grads->alpha_b;   // feature job, first block: alpha_linear gradients
-    }
     WgradParams wp;
     memset(&wp, 0, sizeof(wp));
     wp.act = act; wp.grad = grec; wp.rec_act = rec_act_bytes(D); wp.rec_grad = rec_grad_bytes(D);
     wp.N = N; wp.S = S; wp.rays_per_cta = plan.rays_per_cta; wp.nst_plan = plan.nst; wp.n_tiles = plan.n_tiles;
     wp.t0 = (long long)vc0 * plan.nst * 2; wp.t1 = (long long)vc1 * plan.nst * 2;
-    wp.amax = amax; wp.partial = partial; wp.d_raw = d_raw; wp.njobs = J.n;
+    wp.partial = partial; wp.d_raw = d_raw; wp.njobs = J.n;
     for (int i = 0; i < J.n; ++i) wp.jobs[i] = J.w[i];
     TimedLaunch* tl = nullptr;
     if (g_timing && g_ntimed < 4096) {
@@ -989,10 +1043,10 @@ struct BwdTcPass {
     NB_LAUNCH_OK("wgrad_wg_kernel");
     ReduceParams rp;
     memset(&rp, 0, sizeof(rp));
-    rp.partial = partial; rp.amax = amax; rp.njobs = J.n;
+    rp.partial = partial; rp.amax = amax; rp.njobs = J.nr;
     if (views) J.r[0].dst = gv;                       // job 0 reduces into the scratch block G
-    for (int i = 0; i < J.n; ++i) rp.jobs[i] = J.r[i];
-    dim3 rg(128, J.n);
+    for (int i = 0; i < J.nr; ++i) rp.jobs[i] = J.r[i];
+    dim3 rg(128, J.nr);
     wgrad_reduce_kernel<<<rg, 256, 0, st>>>(rp);
     NB_LAUNCH_OK("wgrad_reduce_kernel");
     return 0;
@@ -1004,9 +1058,21 @@ struct BwdTcPass {
     const int ICV = net->input_ch_views;
     encv_kernel<<<cdiv(N * ICV, 256), 256, 0, st>>>(rays + 8, cfg->ray_stride, N, ICV, encv);
     NB_LAUNCH_OK("encv_kernel");
-    dim3 vg(ICV + 1, cdiv(N, 64));
-    views_enc_wgrad_kernel<<<vg, 128, 0, st>>>(dsum, encv, N, ICV, grads->views_w, net->W + ICV, net->W, dbv);
+    dhv_ray_sum_kernel<<<cdiv(N, 8), 256, 0, st>>>(grec, rec_grad_bytes(net->D), N, S, plan.rays_per_cta, plan.nst, amax, dsum);
+    NB_LAUNCH_OK("dhv_ray_sum_kernel");
+    const int sms = ds->sms;
+    const long long voff = (long long)sms * 128 * 256;  // the upper half of the partial region: reduced already (stream order)
+    dim3 vg(ICV + 1, sms);
+    views_enc_wgrad_kernel<<<vg, 128, 0, st>>>(dsum, encv, N, ICV, views_rays, partial + voff);
     NB_LAUNCH_OK("views_enc_wgrad_kernel");
+    ReduceParams rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.partial = partial; rp.amax = amax; rp.njobs = 2;
+    const long long vrow = (long long)(ICV + 1) * 128;
+    rp.jobs[0] = ReduceJob{voff, vrow, sms, 128, ICV, ICV, net->W + ICV, 0, grads->views_w + net->W};   // [c][e] -> weight[c][W + e]
+    rp.jobs[1] = ReduceJob{voff + (long long)ICV * 128, vrow, sms, 1, 128, 128, 128, 0, dbv};
+    wgrad_reduce_kernel<<<dim3(cdiv(128 * ICV, 256), 2), 256, 0, st>>>(rp);
+    NB_LAUNCH_OK("wgrad_reduce_kernel");
     views_feat_wgrad_kernel<<<128, 256, 0, st>>>(gv, dbv, net->feature_w, net->feature_b, grads->views_w, net->W + ICV);
     NB_LAUNCH_OK("views_feat_wgrad_kernel");
     return 0;
@@ -1114,7 +1180,7 @@ int nerf_b200_mse_seed(const float* rgb, const float* target, int64_t N, float g
   NB_CHECK_ARG(rgb && target && g_rgb && loss_accum, "NULL pointer");
   if (N == 0) return 0;
   const long long n3 = N * 3;
-  mse_seed_kernel<<<cdiv(n3, 256) < 64 ? cdiv(n3, 256) : 64, 256, 0, (cudaStream_t)stream>>>(rgb, target, n3, 1.0f / (float)n3, grad_scale, g_rgb, loss_accum);
+  mse_seed_kernel<<<1, MSE_THREADS, 0, (cudaStream_t)stream>>>(rgb, target, n3, 1.0f / (float)n3, grad_scale, g_rgb, loss_accum);
   NB_LAUNCH_OK("mse_seed_kernel");
   return 0;
 }

@@ -10,16 +10,26 @@
 namespace nb {
 
 // state[0] = loss accumulator (fp32), state[1] = optimizer step count (as float), state[2] = learning rate used last
-__global__ void mse_seed_kernel(const float* __restrict__ rgb, const float* __restrict__ target, long long n3, float inv_n3,
-                                float grad_scale, float* __restrict__ g, float* __restrict__ loss) {
+// ONE block: each thread sums its strided elements in order, then the warps and the block add up in a fixed order, so that the
+// loss is the same bits on every run (no atomics).  A batch is a few thousand rays: one block streams it in microseconds.
+constexpr int MSE_THREADS = 1024;
+__global__ void __launch_bounds__(MSE_THREADS) mse_seed_kernel(const float* __restrict__ rgb, const float* __restrict__ target, long long n3,
+                                                             float inv_n3, float grad_scale, float* __restrict__ g, float* __restrict__ loss) {
+  __shared__ float s_warp[MSE_THREADS / 32];
   float s = 0.f;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n3; i += (long long)gridDim.x * blockDim.x) {
+  for (long long i = threadIdx.x; i < n3; i += MSE_THREADS) {
     const float d = rgb[i] - target[i];
     s = fmaf(d, d, s);
     g[i] = 2.0f * d * inv_n3 * grad_scale;
   }
   s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) atomicAdd(loss, s * inv_n3);
+  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < MSE_THREADS / 32; ++w) t += s_warp[w];
+    *loss += t * inv_n3;
+  }
 }
 
 // Adam step t = state[1] + 1 on n parameters.  lr_t = lr0 * decay_rate^((t - 2) / decay_steps) for t >= 2, lr0 for t = 1:
