@@ -946,6 +946,8 @@ class DeviceRayBatcher:
         self.poses = torch.as_tensor(poses, dtype=torch.float32)                        # host: one [3,4] pose per step goes into kernel arguments
         self.i_train = list(range(self.images.shape[0])) if i_train is None else [int(i) for i in i_train]
         self.rays_rgb = None if rays_rgb is None else torch.as_tensor(rays_rgb, dtype=torch.float32, device=self.dev)
+        # self.rays_rgb == the constructor's rays_rgb[self.perm]: the order to restore, without saving the shuffled rays
+        self.perm = None if rays_rgb is None else torch.arange(self.rays_rgb.shape[0], device=self.dev)
         self.i_batch, self.step = 0, 0
         self.precrop_iters, self.precrop_frac = int(precrop_iters), float(precrop_frac)
 
@@ -955,7 +957,8 @@ class DeviceRayBatcher:
             b = self.rays_rgb[self.i_batch:self.i_batch + self.B].transpose(0, 1)
             self.i_batch += self.B
             if self.i_batch >= self.rays_rgb.shape[0]:
-                self.rays_rgb = self.rays_rgb[torch.randperm(self.rays_rgb.shape[0], device=self.dev)]
+                idx = torch.randperm(self.rays_rgb.shape[0], device=self.dev)
+                self.rays_rgb, self.perm = self.rays_rgb[idx], self.perm[idx]
                 self.i_batch = 0
             return b[:2].contiguous(), b[2].contiguous()
         img_i = self.i_train[int(torch.randint(len(self.i_train), (1,)).item())]
@@ -968,6 +971,34 @@ class DeviceRayBatcher:
             pix = torch.randperm(self.H * self.W, device=self.dev)[:self.B]             # np.random.choice(..., replace=False), :741
         target = self.images[img_i].reshape(-1, self.images.shape[-1])[pix][:, :3].contiguous()
         return self.poses[img_i][:3, :4], pix, target
+
+    def state_dict(self):
+        """The batcher's position: `step` (which decides the centre crop), `i_batch`, the state of the host's torch generator (the
+        image draw of no_batching) and, with use_batching, the current order of rays_rgb as an int64 permutation of the
+        constructor's rays_rgb (8 bytes per ray instead of the 36 of the shuffled rays).  The device draws (the epoch-end
+        randperm, the pixel ids) come from the CUDA generator, which FusedTrainStep.state_dict() holds."""
+        return {"step": self.step, "i_batch": self.i_batch, "cpu_rng_state": torch.get_rng_state(),
+                "perm": None if self.perm is None else self.perm.cpu()}
+
+    def load_state_dict(self, sd):
+        """The inverse of state_dict(), on a batcher constructed with the same images, poses, rays_rgb and settings.  It also
+        sets the host's torch generator (torch.set_rng_state), from which next() draws the image of no_batching."""
+        perm = sd["perm"]
+        if (perm is None) != (self.rays_rgb is None):
+            raise RuntimeError("DeviceRayBatcher.load_state_dict: the state is of the other batching mode (use_batching differs)")
+        if perm is not None:
+            n = self.rays_rgb.shape[0]
+            perm = perm.to(self.dev)
+            if perm.dtype != torch.int64 or tuple(perm.shape) != (n,) or \
+                    not torch.equal(torch.sort(perm).values, torch.arange(n, device=self.dev)):
+                raise RuntimeError(f"DeviceRayBatcher.load_state_dict: 'perm' is not an int64 permutation of this batcher's {n} rays")
+            if not 0 <= int(sd["i_batch"]) < n:
+                raise RuntimeError(f"DeviceRayBatcher.load_state_dict: i_batch {int(sd['i_batch'])} is outside [0, {n})")
+            inv = torch.empty_like(self.perm)
+            inv[self.perm] = torch.arange(n, device=self.dev)
+            self.rays_rgb, self.perm = self.rays_rgb[inv[perm]], perm
+        self.step, self.i_batch = int(sd["step"]), int(sd["i_batch"])
+        torch.set_rng_state(sd["cpu_rng_state"].cpu())
 
 
 # ------------------------------------------------------------------------------------------------

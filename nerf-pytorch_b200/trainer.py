@@ -12,7 +12,9 @@ no autograd graph and no per-tensor optimizer:
 
 captured once for a fixed ray count and replayed.  The parameters stay the SAME `nn.Parameter` objects (re-pointed at
 slices of one flat buffer), so `state_dict()` / checkpoints / `render()` keep working; `attach_optimizer()` exposes the
-moments to a `torch.optim.Adam` so that the reference's checkpoint format (run_nerf.py:792-800) is unchanged.
+moments to a `torch.optim.Adam` so that the reference's checkpoint format (run_nerf.py:792-800) is unchanged, and
+`load_optimizer()` takes them back from one (run_nerf.py:215-233 reloads it).  `state_dict()` / `load_state_dict()` add what
+a bit-exact continuation needs on top, stored under `RESUME_KEY` of the same checkpoint dict (INTEGRATION §5a).
 No reference counterpart; nothing here is needed by the drop-in path.
 """
 from __future__ import annotations
@@ -25,6 +27,60 @@ import torch
 from . import _lib
 from . import api
 from ._lib import NerfPassOut, NerfTrainSave, check
+
+# The key of the reference's checkpoint dict under which a continuation's extra state goes: {"train_step":
+# FusedTrainStep.state_dict(), "batcher": DeviceRayBatcher.state_dict()}.  The reference's create_nerf reads only its own four
+# keys (run_nerf.py:225-233), so it still reloads such a file.
+RESUME_KEY = "nerf_b200_resume"
+
+
+def adam_moments(named_params, optimizer, betas, eps):
+    """The Adam state that `optimizer` holds for `named_params` ((name, Parameter) pairs in the order of the flat buffer), matched
+    by parameter identity, not by position in its param_groups.  -> None when it holds state for none of them, else
+    (step, [(offset in the flat buffer, exp_avg, exp_avg_sq) per parameter]).  `step` may be a tensor (current torch) or an int
+    (torch 1.11, which the reference pins and its published checkpoints were written with).  Raises RuntimeError for a parameter
+    the optimizer does not hold, hyper-parameters the flat Adam does not share (betas, eps, weight decay, amsgrad, maximize),
+    state for some parameters only, a moment whose shape is not its parameter's, or step counts that differ."""
+    named_params = list(named_params)
+    group_of = {id(q): g for g in optimizer.param_groups for q in g["params"]}
+    offsets, off = [], 0
+    for name, p in named_params:
+        g = group_of.get(id(p))
+        if g is None:
+            raise RuntimeError(f"load_optimizer: parameter {name} is not in the optimizer")
+        if tuple(float(b) for b in g["betas"]) != tuple(float(b) for b in betas) or float(g["eps"]) != float(eps):
+            raise RuntimeError(f"load_optimizer: the optimizer's betas {tuple(g['betas'])} / eps {g['eps']} for {name} differ from the "
+                               f"step's own {tuple(betas)} / {eps}")
+        if g.get("weight_decay", 0) or g.get("amsgrad", False) or g.get("maximize", False):
+            raise RuntimeError(f"load_optimizer: {name} is in a param group with weight_decay, amsgrad or maximize, which the flat Adam "
+                               "does not implement")
+        offsets.append(off)
+        off += p.numel()
+    states = [optimizer.state.get(p) for _, p in named_params]
+    given = [bool(s) for s in states]
+    if not any(given):
+        return None
+    if not all(given):
+        missing = [name for (name, _), h in zip(named_params, given) if not h]
+        raise RuntimeError(f"load_optimizer: the optimizer holds Adam state for {sum(given)} of {len(given)} parameters; "
+                           f"none for {', '.join(missing[:4])}{' ...' if len(missing) > 4 else ''}")
+    steps, out = {}, []
+    for (name, p), s, o in zip(named_params, states, offsets):
+        for k in ("step", "exp_avg", "exp_avg_sq"):
+            if k not in s:
+                raise RuntimeError(f"load_optimizer: the optimizer's state for {name} has no '{k}'")
+        for k in ("exp_avg", "exp_avg_sq"):
+            if tuple(s[k].shape) != tuple(p.shape):
+                raise RuntimeError(f"load_optimizer: {k} of {name} has shape {tuple(s[k].shape)}, the parameter {tuple(p.shape)}")
+        steps.setdefault(float(s["step"]), name)
+        out.append((o, s["exp_avg"], s["exp_avg_sq"]))
+    if len(steps) != 1:
+        raise RuntimeError("load_optimizer: the parameters' Adam step counts differ: " +
+                           ", ".join(f"{t:g} ({name})" for t, name in sorted(steps.items())))
+    step = next(iter(steps))
+    if step != int(step) or not 0 <= step < 2 ** 24:          # the flat Adam counts steps in a float32
+        raise RuntimeError(f"load_optimizer: Adam step count {step} is not a whole number in [0, 2^24)")
+    return int(step), out
 
 
 class FusedTrainStep:
@@ -248,3 +304,44 @@ class FusedTrainStep:
         for g in optimizer.param_groups:                # the rate the NEXT step will use, as run_nerf.py:779-783 leaves it
             g["lr"] = self.lr0 * self.decay_rate ** ((t - 1.0) / self.decay_steps) if (t >= 1.0 and self.decay_steps > 0) else self.lr0
         return optimizer
+
+    def _named_params(self):
+        return [(f"{tag}.{k}", p) for tag, n in zip(("network_fn", "network_fine"), self._nets) for k, p in n.named_parameters()]
+
+    def load_optimizer(self, optimizer: torch.optim.Adam):
+        """The inverse of attach_optimizer: continue from the Adam state `optimizer` holds, e.g. after create_nerf() reloaded a
+        checkpoint (run_nerf.py:225-228).  Each parameter's exp_avg / exp_avg_sq is found by parameter identity and copied into
+        the flat moments, and the step count goes to state[1], from which the device derives the decayed rate and the bias
+        correction.  The count is Adam's `step`, the number of updates applied; the checkpoint's `global_step` is not read (the
+        reference writes it before its increment, run_nerf.py:794 / :872, so in its own checkpoints it is one less).  An
+        optimizer without state (a fresh run) leaves the step as it is.  Afterwards the optimizer's state aliases the flat
+        moments, as after attach_optimizer.  The learning rate comes from the step's own lrate / lrate_decay, not from the
+        optimizer's param_groups.  See adam_moments for what is refused."""
+        found = adam_moments(self._named_params(), optimizer, (self.b1, self.b2), self.eps)
+        if found is not None:
+            step, moments = found
+            with torch.no_grad():
+                for off, m, v in moments:
+                    self.m[off:off + m.numel()].copy_(m.reshape(-1))
+                    self.v[off:off + v.numel()].copy_(v.reshape(-1))
+                self.state[1] = float(step)
+        return self.attach_optimizer(optimizer)
+
+    def state_dict(self):
+        """What a bit-exact continuation needs besides the networks and the optimizer: the flat moments, the step state (loss,
+        step count, rate) and the state of this device's CUDA generator, from which the step's draws (t_rand, σ noise, u) and
+        DeviceRayBatcher's device draws come.  m / v / state are this step's own buffers, as nn.Module.state_dict returns the
+        parameters themselves, so torch.save stores them once together with the optimizer state that attach_optimizer aliased
+        to them."""
+        return {"m": self.m, "v": self.v, "state": self.state, "cuda_rng_state": torch.cuda.get_rng_state(self.dev)}
+
+    def load_state_dict(self, sd):
+        """The inverse of state_dict().  Call it after construction: the constructor's warm-up steps draw from the generator.
+        The captured graph reads the generator's seed and offset at every replay, so its replays then draw what the
+        interrupted run would have drawn.  In a data-parallel run every rank loads the same dict (INTEGRATION §5a)."""
+        with torch.no_grad():
+            for k, dst in (("m", self.m), ("v", self.v), ("state", self.state)):
+                if tuple(sd[k].shape) != tuple(dst.shape):
+                    raise RuntimeError(f"FusedTrainStep.load_state_dict: '{k}' has shape {tuple(sd[k].shape)}, this step's {tuple(dst.shape)}")
+                dst.copy_(sd[k])
+        torch.cuda.set_rng_state(sd["cuda_rng_state"].cpu(), self.dev)
