@@ -934,7 +934,10 @@ class DeviceRayBatcher:
     """The two ray-batching modes of train() (run_nerf.py:677-757) with the data resident on the device (SURVEY 8f rank 3).
 
     use_batching=True : `rays_rgb` [(N_img*H*W), 3, 3] (ro, rd, rgb) lives on the device, is shuffled with torch.randperm at every
-                        epoch end (:746-750) and sliced; next() -> (batch_rays [2,B,3], target [B,3]).
+                        epoch end (:746-750) and sliced; next() -> (batch_rays [2,B,3], target [B,3]).  As in the reference's
+                        slicing (:717-726), the last batch of an epoch is shorter when the ray count is not a multiple of B:
+                        it holds the remaining n < B rays.  FusedTrainStep takes it on the first n rows of its buffers
+                        (step.rays[:, :n], step.target[:n], step_device(n_rays=n); INTEGRATION §5a).
     use_batching=False: per step one random training image; pixel ids are drawn on the device (inside the centre crop while
                         i < precrop_iters, :731-744) and the targets gathered there; next() -> (c2w [3,4], pixel_index [B] int64,
                         target [B,3]) for FusedTrainStep.step_device(c2w, pixel_index) / nerf_b200_pack_rays_pixels."""
@@ -1057,42 +1060,71 @@ def create_nerf(args, device=None):
 
 
 # ------------------------------------------------------------------------------------------------
-# CUDA-graph replay of render() for a fixed ray count (no reference counterpart)
+# CUDA-graph replay of render() for up to a fixed ray count (no reference counterpart)
 # ------------------------------------------------------------------------------------------------
 
+def _capture_graph(dev, warm_up, body, pool=None, keep_rng=False):
+    """Run `warm_up()` on a side stream, so that one-time work (weight packing, opt-ins, caches, lazy initialisations) stays
+    out of the capture, then capture `body()` into a new CUDA graph -> (graph, what body returned).  `pool`: the memory pool
+    of an earlier graph (`graph.pool()`) to allocate from, for graphs that never run concurrently.  `keep_rng`: put the
+    device's CUDA generator back to its state before the warm-up, so that a capture made in the middle of a run leaves every
+    later random draw as it would have been without it (the capture itself draws nothing)."""
+    rng = torch.cuda.get_rng_state(dev) if keep_rng else None
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side):
+        warm_up()
+    torch.cuda.current_stream(dev).wait_stream(side)
+    torch.cuda.synchronize(dev)
+    if rng is not None:
+        torch.cuda.set_rng_state(rng, dev)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph, pool=pool):
+        out = body()
+    return graph, out
+
+
 class GraphedRender:
-    """`render(H, W, K, rays=..., **render_kwargs)` under `torch.no_grad()`, captured once into a CUDA graph for a
-    fixed number of rays and replayed per call: host -> device copy of the rays, one graph launch (ray packing,
-    z sampling, both fused passes, resampling), one device -> host copy of `[rgb(3), disp, acc]`.
+    """`render(H, W, K, rays=..., **render_kwargs)` under `torch.no_grad()`, captured into a CUDA graph and replayed per
+    call: host -> device copy of the rays, one graph launch (ray packing, z sampling, both fused passes, resampling), one
+    device -> host copy of `[rgb(3), disp, acc]`.
+
+    `n_rays` is the capacity: a call takes any n <= n_rays rays, such as the tail chunk of a frame that is not a whole number
+    of chunks.  The constructor captures n_rays; every other n is captured on its first call, as
+    `render(H, W, K, rays=self.rays[:, :n], ...)` in the first graph's memory pool, and kept.
 
     After the fusion a 4096-ray render is ~1 ms of GPU time, so the ~10 Python-level launches and allocations of
     `render()` (the reference's structure, run_nerf.py:69-134 -> :54-66 -> :308-418) cost as much as the kernels
     when the GPU starts idle; render_only / test-time callers (run_nerf.py:668,:805,:823 iterate `render` over
     poses under no_grad) can use this instead.  Deterministic settings only (perturb = 0, raw_noise_std = 0:
     the graph would replay the same random draws).  Weight updates are picked up by `refresh()` (re-packs into
-    the same device buffer the graph reads)."""
+    the same device buffer the graphs read)."""
 
     def __init__(self, H, W, K, n_rays, **render_kwargs):
         if render_kwargs.get("perturb", 0.) or render_kwargs.get("raw_noise_std", 0.):
             raise ValueError("GraphedRender supports deterministic rendering only (perturb = 0, raw_noise_std = 0)")
         self._nets = [n for n in (render_kwargs.get("network_fn"), render_kwargs.get("network_fine")) if isinstance(n, NeRF)]
-        dev = _render_device(render_kwargs)
         self.n_rays = int(n_rays)
-        self.rays = torch.zeros((2, self.n_rays, 3), device=dev, dtype=torch.float32)
+        self.rays = torch.zeros((2, self.n_rays, 3), device=_render_device(render_kwargs), dtype=torch.float32)
         self.rays[1, :, 2] = -1.0                                       # any non-degenerate direction for the warm-up
         self.host_out = torch.empty((self.n_rays, 5), dtype=torch.float32, device="cpu").pin_memory()
-        call = lambda: render(H, W, K, rays=self.rays, **render_kwargs)
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.no_grad(), torch.cuda.stream(side):
-            for _ in range(2):                                          # one-time work (packing, opt-ins, caches) outside the capture
-                call()
-        torch.cuda.current_stream(dev).wait_stream(side)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.no_grad(), torch.cuda.graph(self.graph):
-            rgb, disp, acc, extras = call()
-            self.packed_out = torch.cat([rgb, disp[:, None], acc[:, None]], -1)
-        self.device_out = (rgb, disp, acc, extras)
+        self._render = lambda rays: render(H, W, K, rays=rays, **render_kwargs)
+        self.graph = None
+        self._graphs = {}                       # n -> (graph, packed_out, device_out, self.rays[:, :n], self.host_out[:n])
+        self.graph, self.packed_out, self.device_out = self._graph(self.n_rays)[:3]
+
+    def _graph(self, n):
+        if n not in self._graphs:
+            rays = self.rays[:, :n]
+
+            def body():
+                rgb, disp, acc, extras = self._render(rays)
+                return torch.cat([rgb, disp[:, None], acc[:, None]], -1), (rgb, disp, acc, extras)
+            with torch.no_grad():
+                graph, (packed, dev_out) = _capture_graph(self.rays.device, lambda: [self._render(rays) for _ in range(2)], body,
+                                                          pool=None if self.graph is None else self.graph.pool())
+            self._graphs[n] = (graph, packed, dev_out, rays, self.host_out[:n])
+        return self._graphs[n]
 
     def refresh(self):
         """Call after the networks' parameters changed (optimizer step, load_state_dict)."""
@@ -1101,11 +1133,15 @@ class GraphedRender:
                 n.packed()
 
     def __call__(self, rays_host):
-        """rays_host: [2, n_rays, 3] fp32 (pinned memory makes the copy asynchronous).  Returns the pinned host
-        tensor [n_rays, 5] = rgb_map (3), disp_map, acc_map; the device tensors of the last call stay available
-        in `.device_out`.  Synchronises the current stream before returning."""
-        self.rays.copy_(rays_host, non_blocking=True)
-        self.graph.replay()
-        self.host_out.copy_(self.packed_out, non_blocking=True)
+        """rays_host: [2, n, 3] fp32 with 0 < n <= n_rays (pinned memory makes the copy asynchronous).  Returns the first n
+        rows of the pinned host tensor `host_out` [n_rays, 5] = rgb_map (3), disp_map, acc_map; the device tensors of the
+        last call stay available in `.device_out`.  Synchronises the current stream before returning."""
+        sh = tuple(rays_host.shape)
+        if len(sh) != 3 or sh[0] != 2 or sh[2] != 3 or not 0 < sh[1] <= self.n_rays:
+            raise RuntimeError(f"GraphedRender: rays of shape {sh}; expected [2, n, 3] with 0 < n <= {self.n_rays}")
+        graph, self.packed_out, self.device_out, rays, out = self._graph(sh[1])
+        rays.copy_(rays_host, non_blocking=True)
+        graph.replay()
+        out.copy_(self.packed_out, non_blocking=True)
         torch.cuda.current_stream(self.rays.device).synchronize()
-        return self.host_out
+        return out

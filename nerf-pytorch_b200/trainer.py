@@ -10,7 +10,9 @@ no autograd graph and no per-tensor optimizer:
     -> fused MSE + gradient seed (both terms) -> tensor-core backward of both passes into ONE flat gradient buffer
     -> [one all-reduce of that buffer when data parallel] -> flat Adam with the decayed rate computed on the device
 
-captured once for a fixed ray count and replayed.  The parameters stay the SAME `nn.Parameter` objects (re-pointed at
+captured once per ray count and replayed.  The constructor's `n_rays` is the capacity: the buffers hold that many rays and
+its graph is captured at once; a step of fewer rays (the short last batch of an epoch) runs on the first rows of the same
+buffers under a graph of its own, captured on first use.  The parameters stay the SAME `nn.Parameter` objects (re-pointed at
 slices of one flat buffer), so `state_dict()` / checkpoints / `render()` keep working; `attach_optimizer()` exposes the
 moments to a `torch.optim.Adam` so that the reference's checkpoint format (run_nerf.py:792-800) is unchanged, and
 `load_optimizer()` takes them back from one (run_nerf.py:215-233 reloads it).  `state_dict()` / `load_state_dict()` add what
@@ -87,6 +89,7 @@ class FusedTrainStep:
     def __init__(self, H, W, K, n_rays, render_kwargs, lrate=5e-4, lrate_decay=250, betas=(0.9, 0.999), eps=1e-8,
                  process_group=None, use_graph=True, data_parallel=True):
         """render_kwargs: the `render_kwargs_train` dict of create_nerf() plus near / far (run_nerf.py:643-648).
+        n_rays: the most rays a step takes (N_rand); the graph of an n_rays step is captured here.
         lrate_decay is in units of 1000 steps like the reference's --lrate_decay (run_nerf.py:779-780)."""
         import torch.distributed as dist
         self.lib = _lib.load()
@@ -160,94 +163,127 @@ class FusedTrainStep:
         self._pk_c = torch.empty(lib.nerf_b200_packed_bytes(C.byref(self._np_c)), dtype=torch.uint8, device=self.dev)
         self._pk_f = self._pk_c if (self.Ni == 0 or self.net_f is self.net_c) else \
             torch.empty(lib.nerf_b200_packed_bytes(C.byref(self._np_f)), dtype=torch.uint8, device=self.dev)
-        with api._on(self.rays):
-            self._sv_c, self._act_c, self._mask_c = api._train_save(lib, N, Sc, self._np_c, self.dev)
-            if self.Ni > 0:
-                self._sv_f, self._act_f, self._mask_f = api._train_save(lib, N, Sf, self._np_f, self.dev)
-            self._ws = torch.empty(lib.nerf_b200_march_workspace_bytes(N, Sf), dtype=torch.uint8, device=self.dev)
-            bw = lib.nerf_b200_render_rays_bwd_tc_workspace_bytes(N, Sc, C.byref(self._np_c), Sf if self.Ni > 0 else 0,
-                                                                  C.byref(self._np_f) if self.Ni > 0 else None)
-            self._bws = torch.empty(bw + 1024, dtype=torch.uint8, device=self.dev)
-        o = self.out
-        self._bp_c = _lib.NerfBwdPass(api._ptr(self.z_c), api._ptr(self.noise0), Sc, C.pointer(self._np_c), api._ptr(self._pk_c), api._ptr(o["raw0"]),
-                                      C.pointer(self._sv_c), api._ptr(o["g_rgb0"]), C.pointer(self._gs[0]))
-        self._bp_f = _lib.NerfBwdPass(api._ptr(self.z_f), api._ptr(self.noise1), Sf, C.pointer(self._np_f), api._ptr(self._pk_f), api._ptr(o["raw"]),
-                                      C.pointer(self._sv_f), api._ptr(o["g_rgb"]), C.pointer(self._gs[-1])) if self.Ni > 0 else None
+        # every buffer above has the rays as its leading dimension, so an n-ray step (n <= N) runs on their first n rows, which
+        # start at the same pointers; the records and workspaces follow the tile plan of n (see _size_buffers)
+        self._sized = {}
+        self._sized[N] = self._size_buffers(N)
         self._cam = api._camera(self.H, self.W, self.K)
         self._cfg = api._cfg_struct(self.cfgd, self.ray_stride)
         self.host_loss = torch.zeros(4, dtype=torch.float32, device="cpu").pin_memory()
         # ---- capture ----
         self.graph = self.graph_adam = None
+        self._graphs = {}                               # n -> the graph of an n-ray step; other sizes are captured on first use
         if use_graph:
-            side = torch.cuda.Stream(device=self.dev)
-            side.wait_stream(torch.cuda.current_stream(self.dev))
-            snap = (self.flat_p.clone(), self.m.clone(), self.v.clone(), self.state.clone())
-            with torch.cuda.stream(side):
-                for _ in range(2):                      # opt-ins, caches, lazy initialisations outside the capture
-                    self._pack_rays(); self._fwd_bwd(); self._adam()
-            torch.cuda.current_stream(self.dev).wait_stream(side)
-            torch.cuda.synchronize(self.dev)
-            with torch.no_grad():                       # the warm-up steps must not count: restore parameters and moments
-                self.flat_p.copy_(snap[0]); self.m.copy_(snap[1]); self.v.copy_(snap[2]); self.state.copy_(snap[3])
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self._fwd_bwd()
-                if self.world == 1:
-                    self._adam()
+            self.graph = self._graphs[N] = self._capture(N)
             if self.world > 1:
                 self.graph_adam = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(self.graph_adam):
                     self._adam()
 
-    # ---- the step, as library calls on the current stream ----
-    def _pack_rays(self, c2w=None, pixel_index=None):
-        """The ray batch -> packed [N,11] rows ([N,8] without view directions).  Outside the graph (one launch): the camera travels
+    def _size_buffers(self, n):
+        """The training records, the workspaces and the backward-pass descriptors of an n-ray step.  Their sizes follow the
+        tile plan the library derives from n, which can need more for some n < N than for N, so each is the capacity's
+        where the library's size query for n fits in it, and a new buffer of the queried size otherwise."""
+        lib, dev, fine, Sf = self.lib, self.dev, self.Ni > 0, self.Sc + self.Ni
+        cap = self._sized.get(self.N)
+
+        def buf(key, nbytes):
+            t = None if cap is None else cap[key]
+            return t if (t is not None and t.numel() >= nbytes) else torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        b = {}
+        with api._on(self.rays):
+            for tag, S, np_ in (("c", self.Sc, self._np_c), ("f", Sf, self._np_f))[:1 + fine]:
+                ab, mb = C.c_size_t(0), C.c_size_t(0)
+                check(lib.nerf_b200_train_record_bytes(n, S, C.byref(np_), C.byref(ab), C.byref(mb)), "train_record_bytes")
+                b["act_" + tag], b["mask_" + tag] = buf("act_" + tag, ab.value), buf("mask_" + tag, mb.value)
+            b["ws"] = buf("ws", lib.nerf_b200_march_workspace_bytes(n, Sf))
+            bw = lib.nerf_b200_render_rays_bwd_tc_workspace_bytes(n, self.Sc, C.byref(self._np_c), Sf if fine else 0,
+                                                                  C.byref(self._np_f) if fine else None)
+            b["bws"] = buf("bws", bw + 1024)
+        if cap is not None and all(b[k] is cap[k] for k in b):
+            return cap
+        o = self.out
+        b["sv_c"] = NerfTrainSave(api._ptr(b["act_c"]), b["act_c"].numel(), api._ptr(b["mask_c"]), b["mask_c"].numel())
+        b["bp_c"] = _lib.NerfBwdPass(api._ptr(self.z_c), api._ptr(self.noise0), self.Sc, C.pointer(self._np_c), api._ptr(self._pk_c),
+                                     api._ptr(o["raw0"]), C.pointer(b["sv_c"]), api._ptr(o["g_rgb0"]), C.pointer(self._gs[0]))
+        b["sv_f"] = b["bp_f"] = None
+        if fine:
+            b["sv_f"] = NerfTrainSave(api._ptr(b["act_f"]), b["act_f"].numel(), api._ptr(b["mask_f"]), b["mask_f"].numel())
+            b["bp_f"] = _lib.NerfBwdPass(api._ptr(self.z_f), api._ptr(self.noise1), Sf, C.pointer(self._np_f), api._ptr(self._pk_f),
+                                         api._ptr(o["raw"]), C.pointer(b["sv_f"]), api._ptr(o["g_rgb"]), C.pointer(self._gs[-1]))
+        return b
+
+    def _capture(self, n, pool=None, keep_rng=False):
+        """The CUDA graph of an n-ray step: everything after the ray packing (before Adam when data parallel), captured after
+        two eager warm-up steps whose changes to the parameters, moments and state are undone."""
+        snap = (self.flat_p.clone(), self.m.clone(), self.v.clone(), self.state.clone())
+
+        def warm_up():                                  # opt-ins, caches, lazy initialisations outside the capture
+            for _ in range(2):
+                self._pack_rays(n=n); self._fwd_bwd(n); self._adam()
+
+        def body():
+            self._fwd_bwd(n)
+            if self.world == 1:
+                self._adam()
+        graph, _ = api._capture_graph(self.dev, warm_up, body, pool=pool, keep_rng=keep_rng)
+        with torch.no_grad():                           # the warm-up steps must not count: restore parameters and moments
+            self.flat_p.copy_(snap[0]); self.m.copy_(snap[1]); self.v.copy_(snap[2]); self.state.copy_(snap[3])
+        return graph
+
+    # ---- the step, as library calls on the current stream; n rays (default: the capacity N) ----
+    def _pack_rays(self, c2w=None, pixel_index=None, n=None):
+        """The ray batch -> packed [n,11] rows ([n,8] without view directions).  Outside the graph (one launch): the camera travels
         in the kernel arguments, so a per-step pose could not be replayed.  Given rays (self.rays) or -- SURVEY 8f rank 3 -- pixels of
         one posed image."""
+        n = self.N if n is None else n
         vd = int(self.use_viewdirs)
         with api._on(self.rays):
             if pixel_index is None:
-                check(self.lib.nerf_b200_pack_rays(api._ptr(self.rays[0]), api._ptr(self.rays[1]), None, C.byref(self._cam), self.N, 0, self.ndc, self.near,
+                check(self.lib.nerf_b200_pack_rays(api._ptr(self.rays[0]), api._ptr(self.rays[1]), None, C.byref(self._cam), n, 0, self.ndc, self.near,
                                                    self.far, vd, api._ptr(self.packed_rays), api._stream(self.rays)), "pack_rays")
             else:
                 cam = api._camera(self.H, self.W, self.K, c2w)
-                check(self.lib.nerf_b200_pack_rays_pixels(C.byref(cam), api._ptr(pixel_index), self.N, self.ndc, self.near, self.far, vd,
+                check(self.lib.nerf_b200_pack_rays_pixels(C.byref(cam), api._ptr(pixel_index), n, self.ndc, self.near, self.far, vd,
                                                           api._ptr(self.packed_rays), api._stream(self.rays)), "pack_rays_pixels")
 
-    def _fwd_bwd(self):
-        lib, N, cfg = self.lib, self.N, self._cfg
+    def _fwd_bwd(self, n=None):
+        lib, cfg = self.lib, self._cfg
+        n = self.N if n is None else n
+        b = self._sized[n]
         st = api._stream(self.rays)
         with api._on(self.rays):
             check(lib.nerf_b200_pack_weights(C.byref(self._np_c), api._ptr(self._pk_c), self._pk_c.numel(), st), "pack_weights")
             if self._pk_f is not self._pk_c:
                 check(lib.nerf_b200_pack_weights(C.byref(self._np_f), api._ptr(self._pk_f), self._pk_f.numel(), st), "pack_weights")
+            # the draws of an n-ray step fill the first n rows only: the generator advances as in a step built for n rays
             if self.t_rand is not None:                                 # (the reference's draw order)
-                self.t_rand.uniform_()                                  # run_nerf.py:371
+                self.t_rand[:n].uniform_()                              # run_nerf.py:371
             if self.noise0 is not None:
-                self.noise0.normal_().mul_(self.noise_std)              # run_nerf.py:285
+                self.noise0[:n].normal_().mul_(self.noise_std)          # run_nerf.py:285
             if self.u_rand is not None:
-                self.u_rand.uniform_()                                  # run_nerf_helpers.py:208
+                self.u_rand[:n].uniform_()                              # run_nerf_helpers.py:208
             if self.noise1 is not None:
-                self.noise1.normal_().mul_(self.noise_std)
+                self.noise1[:n].normal_().mul_(self.noise_std)
             fine = self.Ni > 0
             check(lib.nerf_b200_render_rays_fwd_train(
-                api._ptr(self.packed_rays), N, C.byref(cfg), C.byref(self._np_c), api._ptr(self._pk_c),
+                api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(self._np_c), api._ptr(self._pk_c),
                 C.byref(self._np_f) if fine else None, api._ptr(self._pk_f) if fine else None,
                 api._ptr(self.t_vals), api._ptr(self.u_det), api._ptr(self.t_rand), api._ptr(self.u_rand), api._ptr(self.noise0), api._ptr(self.noise1),
                 api._ptr(self.z_c), C.byref(self._out_c), api._ptr(self.z_f) if fine else None, api._ptr(self.z_std) if fine else None,
-                C.byref(self._out_f) if fine else None, api._ptr(self._ws), self._ws.numel(),
-                C.byref(self._sv_c), C.byref(self._sv_f) if fine else None, st), "render_rays_fwd_train")
-            # loss = img2mse(rgb, target) + img2mse(rgb0, target)  (run_nerf.py:764-772) and its gradient seeds
+                C.byref(self._out_f) if fine else None, api._ptr(b["ws"]), b["ws"].numel(),
+                C.byref(b["sv_c"]), C.byref(b["sv_f"]) if fine else None, st), "render_rays_fwd_train")
+            # loss = img2mse(rgb, target) + img2mse(rgb0, target)  (run_nerf.py:764-772), means over the n rays, and its gradient seeds
             self.state[0:1].zero_()
             self.flat_g.zero_()
             gscale = 1.0 / self.world
             o = self.out
             if fine:
-                check(lib.nerf_b200_mse_seed(api._ptr(o["rgb"]), api._ptr(self.target), N, gscale, api._ptr(o["g_rgb"]), api._ptr(self.state), st), "mse_seed")
-            check(lib.nerf_b200_mse_seed(api._ptr(o["rgb0"]), api._ptr(self.target), N, gscale, api._ptr(o["g_rgb0"]), api._ptr(self.state), st), "mse_seed")
+                check(lib.nerf_b200_mse_seed(api._ptr(o["rgb"]), api._ptr(self.target), n, gscale, api._ptr(o["g_rgb"]), api._ptr(self.state), st), "mse_seed")
+            check(lib.nerf_b200_mse_seed(api._ptr(o["rgb0"]), api._ptr(self.target), n, gscale, api._ptr(o["g_rgb0"]), api._ptr(self.state), st), "mse_seed")
             # backward of both passes into the flat gradient buffer (one call)
-            check(lib.nerf_b200_render_rays_bwd_tc(api._ptr(self.packed_rays), N, C.byref(cfg), C.byref(self._bp_c),
-                                                   C.byref(self._bp_f) if fine else None, api._ptr(self._bws), self._bws.numel(), st), "render_rays_bwd_tc")
+            check(lib.nerf_b200_render_rays_bwd_tc(api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(b["bp_c"]),
+                                                   C.byref(b["bp_f"]) if fine else None, api._ptr(b["bws"]), b["bws"].numel(), st), "render_rays_bwd_tc")
 
     def _adam(self):
         with api._on(self.rays):
@@ -255,17 +291,39 @@ class FusedTrainStep:
                                                api._ptr(self.state), self.lr0, self.decay_rate, self.decay_steps, self.b1, self.b2, self.eps, 1.0,
                                                api._stream(self.rays)), "adam_step")
 
+    def _prepare(self, n):
+        """The buffers of an n-ray step and, with graphs, its graph: made on the first step of that size.  A new size is
+        captured in the first graph's memory pool (the graphs never run concurrently), and the capture's warm-up leaves the
+        device's generator where it was, so the step draws what it would have drawn without the capture."""
+        if n not in self._sized:
+            self._sized[n] = self._size_buffers(n)
+        if self.graph is not None and n not in self._graphs:
+            self._graphs[n] = self._capture(n, pool=self.graph.pool(), keep_rng=True)
+        return self._graphs.get(n)
+
+    def _check_size(self, n):
+        if not 0 < n <= self.N:
+            raise RuntimeError(f"FusedTrainStep: a step of {n} rays; this step takes 1 to {self.N} (its n_rays)")
+        return n
+
     # ---- public ----
-    def step_device(self, c2w=None, pixel_index=None):
-        """One step on the rays / target already in `self.rays` ([2,N,3]) and `self.target` ([N,3]); no host sync.
-        With `c2w` [3,4] and `pixel_index` (int64 CUDA tensor [N] of row-major pixel ids) the rays are generated on the device
-        for those pixels of that pose instead (run_nerf.py:728-757 without get_rays' [H,W,3] tensors)."""
+    def step_device(self, c2w=None, pixel_index=None, n_rays=None):
+        """One step on the first n rows of the rays / target already in `self.rays` ([2,N,3]) and `self.target` ([N,3]); no
+        host sync.  With `c2w` [3,4] and `pixel_index` (int64 CUDA tensor [n] of row-major pixel ids) the rays are generated on
+        the device for those pixels of that pose instead (run_nerf.py:728-757 without get_rays' [H,W,3] tensors).
+        n is `n_rays`, else `pixel_index.numel()`, else the capacity N; 0 < n <= N.  The loss is the mean over the n rays, as
+        img2mse takes it, and the random draws are those of a step built for n rays.  The first step of a size other than N
+        captures its graph (see _prepare)."""
         import torch.distributed as dist
-        self._pack_rays(c2w, pixel_index)
-        if self.graph is not None:
-            self.graph.replay()
+        n = self._check_size(int(n_rays) if n_rays is not None else (pixel_index.numel() if pixel_index is not None else self.N))
+        if pixel_index is not None and pixel_index.numel() != n:
+            raise RuntimeError(f"FusedTrainStep: pixel_index has {pixel_index.numel()} entries for a step of {n} rays")
+        graph = self._prepare(n)                        # before the packing: a capture's warm-up packs self.rays
+        self._pack_rays(c2w, pixel_index, n)
+        if graph is not None:
+            graph.replay()
         else:
-            self._fwd_bwd()
+            self._fwd_bwd(n)
         if self.world > 1:
             dist.all_reduce(self.flat_g, op=dist.ReduceOp.SUM, group=self.group)     # ONE collective: every gradient, 4.77 MB
             if self.graph_adam is not None:
@@ -278,11 +336,15 @@ class FusedTrainStep:
             n.invalidate_pack()                         # parameters changed behind autograd's version counters
 
     def __call__(self, rays_host, target_host):
-        """rays_host [2,N,3], target_host [N,3] (pinned host memory makes the copies asynchronous) -> loss (python float).
-        Copies the batch in, runs the step, copies the loss out and synchronises the stream."""
-        self.rays.copy_(rays_host, non_blocking=True)
-        self.target.copy_(target_host, non_blocking=True)
-        self.step_device()
+        """rays_host [2,n,3], target_host [n,3] with 0 < n <= N (pinned host memory makes the copies asynchronous) -> loss
+        (python float).  Copies the batch into the first n rows, runs the step, copies the loss out and synchronises the stream."""
+        sr, st = tuple(rays_host.shape), tuple(target_host.shape)
+        if len(sr) != 3 or sr[0] != 2 or sr[2] != 3 or st != (sr[1], 3):
+            raise RuntimeError(f"FusedTrainStep: rays {sr} and target {st}; expected [2, n, 3] and [n, 3]")
+        n = self._check_size(sr[1])
+        self.rays[:, :n].copy_(rays_host, non_blocking=True)
+        self.target[:n].copy_(target_host, non_blocking=True)
+        self.step_device(n_rays=n)
         self.host_loss.copy_(self.state, non_blocking=True)
         torch.cuda.current_stream(self.dev).synchronize()
         return float(self.host_loss[0])
