@@ -203,6 +203,8 @@ class NeRF(nn.Module):
         return p.device
 
     def net_params(self) -> NerfNetParams:
+        if not 1 <= self.D <= _lib.MAX_D:
+            raise RuntimeError(f"nerf_b200: netdepth must be in [1, {_lib.MAX_D}] (got {self.D})")
         self._check_device()
         n = NerfNetParams()
         n.D, n.W, n.input_ch = self.D, self.W, self.input_ch
@@ -843,6 +845,11 @@ def render(H, W, K, chunk=1024 * 32, rays=None, c2w=None, ndc=True, near=0., far
     every mode, `c2w_staticcam` (rays from one camera, view directions from another, :104-107) included; per-ray
     near/far arrays are written into their two columns afterwards."""
     lib = _lib.load()
+    if get_precision() == "fp32":                  # refuse a net the exact path cannot run before the batch is built
+        nets = [kwargs.get("network_fn")] + ([kwargs.get("network_fine")] if kwargs.get("N_importance", 0) > 0 else [])
+        for net in nets:
+            if isinstance(net, NeRF) and lib.nerf_b200_march_bwd_workspace_bytes(1, 1, C.byref(net.net_params())) == 0:
+                raise RuntimeError("nerf_b200: " + lib.nerf_b200_last_error().decode())
     ndc = int(bool(ndc))
     if c2w is not None:
         dev = _render_device(kwargs)

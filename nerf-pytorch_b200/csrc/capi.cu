@@ -38,11 +38,24 @@ static double net_macs_per_row(const NerfNetParams& n) {
 
 static int check_tc_net(const NerfNetParams* net) {
   NB_CHECK_ARG(net != nullptr, "net is NULL");
-  NB_CHECK_ARG(net->W == TC_W, "tensor-core path supports netwidth == 256 (got %d); use precision=FP32", net->W);
+  NB_CHECK_ARG(net->W == TC_W, "tensor-core path supports netwidth == 256 (got %d); other widths run on the exact path "
+               "(precision FP32, set_precision('fp32'))", net->W);
   NB_CHECK_ARG(net->D >= 2 && net->D <= TC_MAXD, "tensor-core path supports 2 <= netdepth <= %d (got %d)", TC_MAXD, net->D);
   NB_CHECK_ARG(net->input_ch >= 3 && net->input_ch <= 63, "input_ch must be in [3,63] (got %d)", net->input_ch);
   NB_CHECK_ARG(net->skip < net->D - 1, "skip layer must be < D-1");
   if (net->use_viewdirs) NB_CHECK_ARG(net->input_ch_views >= 3 && net->input_ch_views <= 63, "input_ch_views must be in [3,63]");
+  return 0;
+}
+
+// the exact path (mlp_simt_kernel forward, bwd_simt.cuh backward): one thread per output column, so W <= SIMT_THREADS, and
+// W a multiple of 4.  A skip after the last layer is refused as the reference fails on it: its heads would receive W + input_ch
+// columns, and mlp_simt_kernel never reaches that concatenation.
+static int check_exact_net(const NerfNetParams* net) {
+  NB_CHECK_ARG(net != nullptr, "net is NULL");
+  NB_CHECK_ARG(net->W >= 4 && net->W <= SIMT_THREADS && net->W % 4 == 0,
+               "exact path supports netwidth <= %d and a multiple of 4 (got %d)", SIMT_THREADS, net->W);
+  NB_CHECK_ARG(net->D >= 1 && net->D <= NERF_B200_MAX_D, "exact path supports 1 <= netdepth <= %d (got %d)", NERF_B200_MAX_D, net->D);
+  NB_CHECK_ARG(net->skip < net->D - 1, "skip layer must be < netdepth - 1 (got skip %d, netdepth %d)", net->skip, net->D);
   return 0;
 }
 
@@ -258,7 +271,7 @@ int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, in
   if (N == 0 || S == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (precision == NERF_B200_PREC_FP32) {
-    NB_CHECK_ARG(net->W <= SIMT_THREADS && net->W % 4 == 0, "exact path supports netwidth <= 256");
+    if (int rc = check_exact_net(net)) return rc;
     NB_CHECK_ARG(!net->use_viewdirs || viewdirs, "viewdirs required");
     const long long M = N * (long long)S;
     const size_t sm = simt_smem_bytes(*net);
@@ -452,12 +465,12 @@ static int march_impl(const float* rays, const float* z_vals, const float* noise
   if (cfg->precision == NERF_B200_PREC_FP32) {
     // exact mode (validation path): materialise pts -> fp32 CUDA-core MLP -> raw2outputs kernel
     NB_CHECK_ARG(save == nullptr, "training-mode records belong to the tensor-core path");
+    if (int rc = check_exact_net(net)) return rc;
     const long long M = N * (long long)S;
     // mlp_simt_kernel stores raw as float4: its scratch starts on a 16-byte boundary whatever M is
     const size_t pts_floats = ((size_t)M * 3 + 3) & ~(size_t)3;
     const size_t need = pts_floats * 4 + (out->raw ? 0 : (size_t)M * 16);
     NB_CHECK_ARG(workspace && workspace_bytes >= need, "exact-mode workspace too small: need %zu bytes", need);
-    NB_CHECK_ARG(net->W <= SIMT_THREADS && net->W % 4 == 0, "exact path supports netwidth <= 256");
     float* pts = static_cast<float*>(workspace);
     float* raw = out->raw ? out->raw : pts + pts_floats;
     pts_kernel<<<cdiv(M, 256), 256, 0, st>>>(rays, cfg->ray_stride, z_vals, M, S, pts);
@@ -516,6 +529,10 @@ static int render_rays_fwd_impl(const float* rays, int64_t N, const NerfRenderCf
   }
   const int Sc = cfg->N_samples, Ni = cfg->N_importance;
   NB_CHECK_ARG(Sc >= 1 && Ni >= 0, "bad sample counts");
+  if (cfg->precision == NERF_B200_PREC_FP32) {          // both nets are checked before the first launch
+    if (int rc = check_exact_net(net_coarse)) return rc;
+    if (Ni > 0 && net_fine) { if (int rc = check_exact_net(net_fine)) return rc; }
+  }
   NB_CHECK_ARG(!cfg->perturb || t_rand, "perturb > 0 needs t_rand");
   // per-ray prologue: z sampling (run_nerf.py:357-379) and, on the tensor-core path, the view-bias tables of both networks
   // -- one launch (ray_setup_kernel); the exact path keeps the stand-alone z kernel
@@ -608,8 +625,12 @@ int nerf_b200_render_rays_fwd_train(const float* rays, int64_t N, const NerfRend
 // ---- exact-mode backward of one pass (see bwd_simt.cuh) -------------------------------------------
 static const int BWD_RAYS_PER_SLAB = 512;     // rays recomputed + back-propagated per slab (bounds the workspace)
 
+// march_bwd_impl carves BWD_BUFFERS buffers per slab, each rounded up to 4 floats: the 1024 spare bytes cover the rounding
+static const int BWD_BUFFERS = 11;
+static_assert(BWD_BUFFERS * 3 * sizeof(float) <= 1024, "the workspace's spare bytes must cover the 16-byte rounding");
+
 size_t nerf_b200_march_bwd_workspace_bytes(int64_t N, int S, const NerfNetParams* net) {
-  if (!net) return 0;
+  if (check_exact_net(net)) return 0;
   const long long rows = (long long)(N < BWD_RAYS_PER_SLAB ? N : BWD_RAYS_PER_SLAB) * S;
   return (size_t)rows * (3 + bwd_floats_per_row(*net)) * 4 + 1024;
 }
@@ -658,7 +679,7 @@ static int march_bwd_impl(const float* rays, const float* z_vals, const float* n
                           void* workspace, size_t workspace_bytes, void* stream) {
   NB_CHECK_ARG(rays && z_vals && net && cfg && grads, "NULL pointer");
   NB_CHECK_ARG(!seeds_none(g), "no output gradient given (every NerfOutGrads member is NULL)");
-  NB_CHECK_ARG(net->W <= SIMT_THREADS && net->W % 4 == 0 && net->D <= NERF_B200_MAX_D, "unsupported network shape");
+  if (int rc = check_exact_net(net)) return rc;
   if (N == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int W = net->W, W2 = W / 2, IC = net->input_ch, ICV = net->input_ch_views, D = net->D, rs = cfg->ray_stride;
@@ -669,22 +690,23 @@ static int march_bwd_impl(const float* rays, const float* z_vals, const float* n
     const float* ry = rays + n0 * rs;
     const float* zz = z_vals + n0 * S;
     const float* nz = noise ? noise + n0 * S : nullptr;
-    // every buffer starts on a 16-byte boundary: mlp_simt_kernel stores raw as float4, and M * (3 + IC + ICV) need not be a
-    // multiple of 4 (the rounding takes at most 24 of the workspace's 1024 spare bytes)
+    // every one of the BWD_BUFFERS buffers starts on a 16-byte boundary: mlp_simt_kernel stores raw as float4 and
+    // raw2outputs_bwd_kernel loads it so, and neither M * (3 + IC + ICV) nor M * W / 2 need be a multiple of 4 (odd M, W = 4k
+    // with k odd).  The rounding takes at most BWD_BUFFERS * 12 of the workspace's 1024 spare bytes.
     float* p = static_cast<float*>(workspace);
     auto q4 = [](long long n) { return (n + 3) & ~3ll; };
     float* pts = p;        p += q4(M * 3);
     SimtSave sv;
     sv.enc = p;            p += q4(M * IC);
     sv.encv = p;           p += q4(M * ICV);
-    sv.h = p;              p += (size_t)D * M * W;
-    sv.feat = p;           p += M * W;
-    sv.hv = p;             p += M * W2;
-    float* raw = p;        p += M * 4;
-    float* d_raw = p;      p += M * 4;
-    float* dh0 = p;        p += M * W;
-    float* dh1 = p;        p += M * W;
-    float* d_hv = p;       p += M * W2;
+    sv.h = p;              p += q4((long long)D * M * W);
+    sv.feat = p;           p += q4(M * W);
+    sv.hv = p;             p += q4(M * W2);
+    float* raw = p;        p += q4(M * 4);
+    float* d_raw = p;      p += q4(M * 4);
+    float* dh0 = p;        p += q4(M * W);
+    float* dh1 = p;        p += q4(M * W);
+    float* d_hv = p;       p += q4(M * W2);
     if (!net->use_viewdirs) { sv.encv = nullptr; sv.feat = nullptr; sv.hv = nullptr; }
     // 1. recompute the pass in fp32 with saved activations
     pts_kernel<<<cdiv(M, 256), 256, 0, st>>>(ry, rs, zz, M, S, pts);

@@ -1,6 +1,8 @@
-"""Generate tests/golden/shapes.npz by running the UNMODIFIED reference on CPU  --  build container only.
+"""Generate tests/golden/shapes.npz and tests/golden/exact_shapes.npz by running the UNMODIFIED reference on CPU  --  build
+container only.
 
-    python oracle/gen_shapes_golden.py        # needs the reference checkout (oracle/ref_import.py); writes tests/golden/
+    python oracle/gen_shapes_golden.py [shapes | exact_shapes]   # needs the reference checkout (oracle/ref_import.py); writes
+                                                                 # tests/golden/ (both files without an argument)
 
 Networks other than the default 8 x 256 with 63 + 27 input channels, built by the reference's create_nerf (skips = [4]):
 
@@ -9,6 +11,14 @@ Networks other than the default 8 x 256 with 63 + 27 input channels, built by th
     noenc_d2   : --i_embed -1 (input_ch 3) --netdepth 2, no view directions, 64 samples, N_importance 0 (output_ch 4), 32 lego rays
     nv_d6_S316 : --netdepth 6 --netdepth_fine 6, no view directions, 16 + 300 samples (one fine ray spans two 256-row
                  super-tiles), 16 fern NDC rays
+
+exact_shapes.npz: create_nerf-shaped nets only the exact path (fp32 CUDA cores) runs -- the tensor-core path takes netwidth 256
+and input_ch <= 63 only:
+
+    w128_d10     : --netwidth 128 --netdepth 10 --netwidth_fine 64 --netdepth_fine 4, view directions, 32 + 64 samples, 32 lego rays
+    L14_Lv8      : --multires 14 --multires_views 8 (input_ch 87 + 51), view directions, 64 + 64 samples, 16 lego rays
+    w100_nv_odd  : --netwidth 100 --netwidth_fine 100, no view directions, 33 + 32 samples, 33 fern NDC rays: N * S is odd in both
+                   passes (33 x 33, 33 x 65) and W / 2 = 50 is not a multiple of 4
 
 Stored per case `x` (keys prefixed `x_`): the inputs and settings, the target, rgb_map / disp_map / acc_map, the loss
 img2mse(rgb) (+ img2mse(rgb0)), and per net (c, f) 64 sampled entries of every parameter gradient (g_{c,f}_{names,count,idx,val}),
@@ -40,6 +50,17 @@ CASES = {
                        N_samples=16, N_importance=300, seed_w=4),
 }
 
+EXACT_CASES = {
+    "w128_d10": dict(scene="lego", N=32, netwidth=128, netdepth=10, netwidth_fine=64, netdepth_fine=4, multires=10, multires_views=4,
+                     i_embed=0, use_viewdirs=True, N_samples=32, N_importance=64, seed_w=2),
+    "L14_Lv8": dict(scene="lego", N=16, netdepth=8, netdepth_fine=8, multires=14, multires_views=8, i_embed=0, use_viewdirs=True,
+                    N_samples=64, N_importance=64, seed_w=2),
+    "w100_nv_odd": dict(scene="fern", N=33, netwidth=100, netdepth=8, netwidth_fine=100, netdepth_fine=8, multires=10,
+                        multires_views=4, i_embed=0, use_viewdirs=False, N_samples=33, N_importance=32, seed_w=0),
+}
+
+TABLES = {"shapes": CASES, "exact_shapes": EXACT_CASES}
+
 
 def input_ch(L, i_embed):
     return 3 if i_embed == -1 else 3 + 6 * L
@@ -49,11 +70,11 @@ def states(c, output_ch):
     ic = input_ch(c["multires"], c["i_embed"])
     icv = input_ch(c["multires_views"], c["i_embed"])
     out = []
-    for k, D in enumerate((c["netdepth"], c["netdepth_fine"])):
+    for k, (D, W) in enumerate(((c["netdepth"], c.get("netwidth", 256)), (c["netdepth_fine"], c.get("netwidth_fine", 256)))):
         if c["use_viewdirs"]:
-            out.append(synth.nerf_state(c["seed_w"] + k, False, D=D, input_ch=ic, input_ch_views=icv, skips=(4,)))
+            out.append(synth.nerf_state(c["seed_w"] + k, False, D=D, W=W, input_ch=ic, input_ch_views=icv, skips=(4,)))
         else:
-            out.append(noviews.nerf_state_noviews(c["seed_w"] + k, output_ch=output_ch, D=D, input_ch=ic, skips=(4,)))
+            out.append(noviews.nerf_state_noviews(c["seed_w"] + k, output_ch=output_ch, D=D, W=W, input_ch=ic, skips=(4,)))
     return out
 
 
@@ -71,8 +92,9 @@ def run_case(rn, fx, tag, c):
     with tempfile.TemporaryDirectory() as tmp:
         args = make_args(tmp, N_importance=c["N_importance"], N_samples=c["N_samples"], use_viewdirs=c["use_viewdirs"],
                          white_bkgd=sb["white_bkgd"], dataset_type="llff" if sb["ndc"] else "blender", perturb=0.0)
-        for k in ("netdepth", "netdepth_fine", "multires", "multires_views", "i_embed"):
-            setattr(args, k, c[k])
+        for k in ("netdepth", "netdepth_fine", "multires", "multires_views", "i_embed", "netwidth", "netwidth_fine"):
+            if k in c:
+                setattr(args, k, c[k])
         kw, _, _, _, _ = rn.create_nerf(args)
     nets = [kw["network_fn"], kw["network_fine"]]
     output_ch = 5 if c["N_importance"] > 0 else 4
@@ -131,12 +153,13 @@ def main():
     torch.manual_seed(0)
     torch.set_num_threads(8)                      # fixed: CPU reductions are then reproducible bit for bit
     rn, _ = ref_import.load()
-    fx = {}
-    for tag, c in CASES.items():
-        run_case(rn, fx, tag, c)
     os.makedirs(OUT, exist_ok=True)
-    np.savez_compressed(os.path.join(OUT, "shapes.npz"), **fx)
-    print("wrote shapes", len(fx), "arrays in", round(time.time() - t0, 1), "s")
+    for name in sys.argv[1:] or list(TABLES):
+        fx = {}
+        for tag, c in TABLES[name].items():
+            run_case(rn, fx, tag, c)
+        np.savez_compressed(os.path.join(OUT, name + ".npz"), **fx)
+        print("wrote", name, len(fx), "arrays in", round(time.time() - t0, 1), "s")
 
 
 if __name__ == "__main__":

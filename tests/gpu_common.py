@@ -18,8 +18,8 @@ def dev(a):
     return torch.from_numpy(np.ascontiguousarray(a)).to(DEV)
 
 
-def make_net(state, use_viewdirs=True, output_ch=5, D=8, skips=(4,), input_ch=63, input_ch_views=27):
-    m = nb.NeRF(D=D, W=256, input_ch=input_ch, input_ch_views=input_ch_views if use_viewdirs else 0, output_ch=output_ch,
+def make_net(state, use_viewdirs=True, output_ch=5, D=8, skips=(4,), input_ch=63, input_ch_views=27, W=256):
+    m = nb.NeRF(D=D, W=W, input_ch=input_ch, input_ch_views=input_ch_views if use_viewdirs else 0, output_ch=output_ch,
                 skips=list(skips), use_viewdirs=use_viewdirs)
     m.load_state_dict({k: torch.from_numpy(v) for k, v in state.items()})
     return m.to(DEV)
@@ -114,8 +114,20 @@ def march_bwd_tc(net, rays, z, raw, act, mask, seeds, L=10, Lv=4, white=True):
     return {k: v.cpu().numpy() for k, v in grads.items()}, ws.cpu().numpy()[base:]
 
 
-def march_bwd_exact(net, rays, z, seeds, L=10, Lv=4, white=True):
-    """nerf_b200_march_bwd / nerf_b200_march_bwd_outs (fp32 recompute of the pass) -> grads dict name -> np"""
+def run_network_exact(net, pts, viewdirs, S, L=10, Lv=4):
+    """nerf_b200_run_network in fp32: pts [N * S, 3], viewdirs [N, 3] or None -> raw [N * S, 4]"""
+    lib = _lib.load()
+    N = pts.shape[0] // S
+    raw = torch.zeros((N * S, 4), device=DEV)
+    _lib.check(lib.nerf_b200_run_network(ptr(pts), ptr(viewdirs), N, S, C.byref(net.net_params()), None, L, Lv, _lib.PREC_FP32,
+                                         ptr(raw), None, 0, stream()), "run_network")
+    torch.cuda.synchronize()
+    return raw
+
+
+def march_bwd_exact(net, rays, z, seeds, L=10, Lv=4, white=True, fill=None):
+    """nerf_b200_march_bwd / nerf_b200_march_bwd_outs (fp32 recompute of the pass) -> grads dict name -> np.  fill: byte the
+    workspace is set to before the call (None: left as allocated)"""
     lib = _lib.load()
     N, S = z.shape
     n = net.net_params()
@@ -125,6 +137,8 @@ def march_bwd_exact(net, rays, z, seeds, L=10, Lv=4, white=True):
     ws_bytes = lib.nerf_b200_march_bwd_workspace_bytes(N, S, C.byref(n))
     assert ws_bytes > 0
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=DEV)
+    if fill is not None:
+        ws.fill_(fill)
     rgb_only, s = _seed_args(seeds)
     args = (ptr(rays), ptr(z), None, N, S, C.byref(n), None, C.byref(c))
     tail = (C.byref(gs), ptr(ws), ws_bytes, stream())

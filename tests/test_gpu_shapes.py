@@ -10,12 +10,17 @@
 (c) the backward's limit S <= 1024 (the forward accepts up to 4096).
 (d) create_nerf-shaped nets (netdepth 4 with skips = [4], i_embed = -1) through render() + loss.backward() against the
     reference's autograd (tests/golden/shapes.npz) and through FusedTrainStep.
+(e) shapes only the exact path serves (netwidth 4 .. 252 other than 256, netdepth 1 and 9 .. 16, multires 11 .. 16): forward,
+    run_network and both backward entry points against float64 autograd kernel by kernel, on workspaces whose contents must
+    not matter; create_nerf-shaped nets through render() against the reference (tests/golden/exact_shapes.npz); and the
+    refusals through render().
 
 conftest.rel_l2 ignores non-finite entries, so every comparison first asserts that the kernel's tensors are finite (disp and its
 NaN pattern excepted).  Measured deviations go to parity_shapes.json in $NERF_B200_PARITY_DIR (default: a nerf_b200_parity
 directory under the system's temporary directory)."""
 import json
 import os
+import re
 import tempfile
 import types
 
@@ -60,18 +65,18 @@ class Shape(types.SimpleNamespace):
     """one network: state dict, the library's NeRF and what the restatements need"""
 
 
-def _shape(G, sid, D, skips, L, Lv, out_ch, seed=0, sharpen=False):
+def _shape(G, sid, D, skips, L, Lv, out_ch, seed=0, sharpen=False, W=256):
     from nerf_pytorch_b200.api import effective_skip
     from oracle import noviews, tc_emul
     ic = tc_emul.input_ch(L)
     views = Lv is not None
     icv = tc_emul.input_ch(Lv) if views else 0
     if views:
-        state = G.synth.nerf_state(seed, sharpen, D=D, input_ch=ic, input_ch_views=icv, skips=skips)
+        state = G.synth.nerf_state(seed, sharpen, D=D, W=W, input_ch=ic, input_ch_views=icv, skips=skips)
     else:
-        state = noviews.nerf_state_noviews(seed, sharpen, output_ch=out_ch, D=D, input_ch=ic, skips=skips)
-    net = G.make_net(state, use_viewdirs=views, output_ch=out_ch, D=D, skips=skips, input_ch=ic, input_ch_views=icv)
-    return Shape(id=sid, D=D, skip=effective_skip(skips, D), L=L, Lv=Lv if views else 0, views=views, ic=ic, icv=icv,
+        state = noviews.nerf_state_noviews(seed, sharpen, output_ch=out_ch, D=D, W=W, input_ch=ic, skips=skips)
+    net = G.make_net(state, use_viewdirs=views, output_ch=out_ch, D=D, skips=skips, input_ch=ic, input_ch_views=icv, W=W)
+    return Shape(id=sid, W=W, D=D, skip=effective_skip(skips, D), L=L, Lv=Lv if views else 0, views=views, ic=ic, icv=icv,
                  state=state, net=net)
 
 
@@ -216,9 +221,12 @@ def _check_bwd_stages(G, sh, packed, z, o, plan, rec, grads, ws, g_rgb, stats, s
 
 # ---- (a) network shapes ---------------------------------------------------------------------------------------------------
 
-def _exact_reference(sh, packed, z, g_rgb, dtype=torch.float64):
+def _exact_reference(sh, packed, z, g_rgb, dtype=torch.float64, seeds=None):
     """autograd of the reference's network (oracle/torch_ref.mlp) and raw2outputs on the kernels' fp32 samples, in float64 (the
-    reference) or float32 (how far fp32 arithmetic itself is from it) -> (raw [M,4], maps, grads by state_dict key)"""
+    reference) or float32 (how far fp32 arithmetic itself is from it) -> (raw [M,4], maps, grads by state_dict key).  The loss
+    is sum(rgb_map * g_rgb), or with `seeds` (rgb_map, disp_map, acc_map, raw -> gradient) the sum of each output times its seed,
+    whose float64 dL/draw tests/test_outgrads_cpu.py pins oracle/outgrads.adjoint to.  disp is NaN on empty rays: a zero seed
+    keeps it off the loss there."""
     from oracle import torch_ref as T
     N, S = z.shape
     sd = {k: torch.from_numpy(v).to(dtype).requires_grad_(True) for k, v in sh.state.items()}
@@ -227,7 +235,13 @@ def _exact_reference(sh, packed, z, g_rgb, dtype=torch.float64):
         x = torch.cat([x, T.embed(_vd_rows(packed, S).to(dtype), sh.Lv)], -1)
     raw = T.mlp(sd, x, ic=sh.ic, icv=sh.icv, skip=sh.skip, D=sh.D)
     rgb, disp, acc, w = T.composite(raw.reshape(N, S, 4), torch.from_numpy(z).to(dtype), torch.from_numpy(packed[:, 3:6]).to(dtype), True)
-    (rgb * torch.from_numpy(g_rgb).to(dtype)).sum().backward()
+    if seeds is None:
+        (rgb * torch.from_numpy(g_rgb).to(dtype)).sum().backward()
+    else:
+        sd_ = {k: v.to(dtype) for k, v in seeds.items()}
+        disp_on = torch.where(sd_["disp_map"] != 0, disp, torch.zeros_like(disp))
+        ((rgb * sd_["rgb_map"]).sum() + (disp_on * sd_["disp_map"]).sum() + (acc * sd_["acc_map"]).sum() +
+         (raw.reshape(N, S, 4) * sd_["raw"]).sum()).backward()
     grads = {k: (v.grad if v.grad is not None else torch.zeros_like(v)).numpy() for k, v in sd.items()}
     maps = {"rgb": rgb.detach().numpy(), "disp": disp.detach().numpy(), "acc": acc.detach().numpy(), "w": w.detach().numpy()}
     return raw.detach().numpy(), maps, grads
@@ -432,17 +446,18 @@ def _fixture_nets(G, fx, case):
     L, Lv = (0, 0) if no_enc else (int(fx[p + "multires"]), int(fx[p + "multires_views"]))
     ic, icv = tc_emul.input_ch(L), (tc_emul.input_ch(Lv) if views else 0)
     nets = []
-    for k, D in enumerate((int(fx[p + "netdepth"]), int(fx[p + "netdepth_fine"]))):
+    for k, tag in enumerate(("", "_fine")):
         if k == 1 and int(fx[p + "N_importance"]) == 0:
             nets.append(None)
             continue
+        D, W = int(fx[p + "netdepth" + tag]), (int(fx[p + "netwidth" + tag]) if p + "netwidth" + tag in fx else 256)
         seed = int(fx[p + "seed_w"]) + k
         if views:
-            st = G.synth.nerf_state(seed, False, D=D, input_ch=ic, input_ch_views=icv, skips=(4,))
+            st = G.synth.nerf_state(seed, False, D=D, W=W, input_ch=ic, input_ch_views=icv, skips=(4,))
         else:
-            st = noviews.nerf_state_noviews(seed, output_ch=int(fx[p + "output_ch"]), D=D, input_ch=ic, skips=(4,))
+            st = noviews.nerf_state_noviews(seed, output_ch=int(fx[p + "output_ch"]), D=D, W=W, input_ch=ic, skips=(4,))
         nets.append(G.make_net(st, use_viewdirs=views, output_ch=int(fx[p + "output_ch"]), D=D, skips=[4], input_ch=ic,
-                               input_ch_views=icv))
+                               input_ch_views=icv, W=W))
     return nets
 
 
@@ -488,10 +503,14 @@ def test_render_against_reference(G, case):
     """render() + img2mse + loss.backward() on the exact and the tensor-core path against the reference's autograd on the same
     nets (tests/golden/shapes.npz): exact path within 3e-3 plus twice the fp32 conditioning per tensor; tensor-core path
     within the forward and end-to-end budgets of the other files."""
-    fx = load_golden("shapes")
+    _check_render_against_reference(G, "shapes", case, (("fp32", "exact"), ("tc_fp16", "tc")))
+
+
+def _check_render_against_reference(G, fixture, case, arms):
+    fx = load_golden(fixture)
     p = f"{case}_"
     stats = {}
-    for prec, bwd in (("fp32", "exact"), ("tc_fp16", "tc")):
+    for prec, bwd in arms:
         loss, maps, nets = _fixture_render(G, fx, case, prec, bwd)
         ref_loss = float(fx[p + "loss"])
         stats[f"{bwd}_loss_rel"] = abs(loss - ref_loss) / ref_loss
@@ -528,6 +547,7 @@ def test_render_against_reference(G, case):
         if bwd == "tc":
             assert med < 3e-2 and worst < 1.5e-1, (med, worst, errs)
     _record(f"golden_{case}", stats)
+    return stats
 
 
 def test_fused_step_netdepth4(G):
@@ -571,3 +591,148 @@ def test_fused_step_netdepth4(G):
         worst = max(worst, rel_l2(db, da))
     _record("fused_step_netdepth4", {"losses_autograd": losses_a, "losses_fused": losses_b, "update_worst": worst})
     assert worst < 5e-2, worst
+
+
+# ---- (e) shapes only the exact path serves -------------------------------------------------------------------------------------
+# The exact path (mlp_simt_kernel forward, bwd_simt.cuh backward) takes any netwidth <= 256 that is a multiple of 4, netdepth
+# 1 .. 16 and any encoding width; the tensor-core path only netwidth 256, netdepth 2 .. 8 and input_ch <= 63.  march_bwd_impl
+# recomputes the pass in slabs of up to 512 rays; a slab of M = rays x samples rows with M odd and netwidth / 2 not a multiple of
+# 4 is where its buffers after hv would lose their 16-byte alignment (raw is stored and loaded as float4).
+
+# id, W, D, skips, multires, multires_views (None: no view directions), output_ch, N, S, parameter seed (seeds whose rays are not
+# all empty: an empty batch has no gradient)
+EXACT_SHAPES = [
+    ("w100_d3_s0", 100, 3, [0], 10, 4, 5, 37, 65, 0),      # W / 2 = 50, odd M; GEMM tiles with remainders; several wgrad slabs
+    ("w252_d9_s7", 252, 9, [7], 10, 4, 5, 37, 65, 0),      # the widest odd-k width, D > 8, skip D - 2
+    ("w4_d1", 4, 1, [], 0, 0, 5, 7, 9, 0),                 # smallest net (i_embed = -1): one wgrad slab, one column-sum block
+    ("w128_d10", 128, 10, [4], 10, 4, 5, 37, 64, 1),       # --netwidth 128 --netdepth 10
+    ("w256_L16", 256, 8, [4], 16, 16, 5, 21, 64, 0),       # octaves up to 2^15, input_ch 99 + 99: the largest shared memory
+    ("w64_d16_nv", 64, 16, [14], 11, None, 4, 33, 33, 0),  # D = 16, the no-view head
+    ("w200_d12_s0", 200, 12, [0], 13, 5, 5, 600, 33, 1),   # > 512 rays: two ray slabs in march_bwd_impl
+    ("w36_d2_nv", 36, 2, [], 6, None, 5, 513, 3, 1),       # odd M in the last ray slab only (1 ray x 3 samples); output_ch 5
+]
+
+
+def _check_exact_grads(sh, grads, g_ref, g32, stats, tag):
+    """every gradient tensor against float64 autograd: gated at 1e-4 plus twice the float32 autograd's own distance where that
+    is <= 1e-4, recorded elsewhere; tensors off the loss's graph exactly 0 -> names of the gated tensors"""
+    gated = []
+    for name, ref in g_ref.items():
+        _finite(f"{tag} {name}", grads[name])
+        if not ref.any():
+            assert not grads[name].any(), (tag, name)
+            continue
+        e, cond = rel_l2(grads[name], ref), rel_l2(g32[name], ref)
+        stats[f"{tag}_g_{name}"], stats[f"{tag}_cond_g_{name}"] = e, cond
+        if cond <= 1e-4:
+            assert e < 1e-4 + 2 * cond, (tag, name, e, cond)
+            gated.append(name)
+    if "output_linear.weight" in grads:          # rows >= 4 of output_linear never reach raw2outputs
+        assert not grads["output_linear.weight"][4:].any() and not grads["output_linear.bias"][4:].any(), tag
+    return gated
+
+
+@pytest.mark.parametrize("sid,W,D,skips,L,Lv,out_ch,N,S,seed", EXACT_SHAPES, ids=[s[0] for s in EXACT_SHAPES])
+def test_exact_path_shape(G, sid, W, D, skips, L, Lv, out_ch, N, S, seed):
+    sh = _shape(G, sid, D, skips, L, Lv, out_ch, seed=seed, W=W)
+    packed, z = _rays(G, sh, N, S, seed=5)
+    rays, zd = G.dev(packed), G.dev(z)
+    slab_rows = [min(512, N - n0) * S for n0 in range(0, N, 512)]
+    stats = {"odd_slab": any(m % 2 for m in slab_rows), "hv_unaligned": (W // 2) % 4 != 0}
+    # forward: nerf_b200_march and nerf_b200_run_network in fp32
+    g_rgb = _g_rgb(N)
+    raw_ref, maps_ref, g_ref = _exact_reference(sh, packed, z, g_rgb)
+    raw32, maps32, g32 = _exact_reference(sh, packed, z, g_rgb, torch.float32)
+    stats["cond_raw"] = rel_l2(raw32, raw_ref)
+    o, _, _ = G.march(sh.net, rays, zd, train=False, L=sh.L, Lv=sh.Lv, precision=G._lib.PREC_FP32)
+    vd = G.dev(packed[:, 8:11]) if sh.views else None
+    raw_rn = G.run_network_exact(sh.net, _pts(packed, z).to(G.DEV), vd, S, L=sh.L, Lv=sh.Lv)
+    for tag, r in (("march", o["raw"]), ("run_network", raw_rn)):
+        r = r.cpu().numpy().reshape(-1, 4)
+        _finite(f"{tag} raw", r)
+        stats[f"{tag}_raw_rel"] = rel_l2(r, raw_ref)
+        assert stats[f"{tag}_raw_rel"] <= 2e-5 + 2 * stats["cond_raw"], (tag, stats)
+    for k in ("rgb", "disp", "acc", "w"):
+        v = o[k].cpu().numpy()
+        stats[f"{k}_rel"] = _same_nan("disp", v, maps_ref[k]) if k == "disp" else (_finite(k, v) or rel_l2(v, maps_ref[k]))
+        stats[f"cond_{k}"] = rel_l2(maps32[k], maps_ref[k])
+        assert stats[f"{k}_rel"] <= 2e-5 + 2 * stats[f"cond_{k}"], (k, stats)
+    # backward, rgb seed: the workspace's contents must not matter (0xFF bytes are NaNs)
+    g_nan = G.march_bwd_exact(sh.net, rays, zd, G.dev(g_rgb), L=sh.L, Lv=sh.Lv, fill=0xFF)
+    g_zero = G.march_bwd_exact(sh.net, rays, zd, G.dev(g_rgb), L=sh.L, Lv=sh.Lv, fill=0)
+    for name in g_zero:
+        assert np.array_equal(g_nan[name].view(np.uint32), g_zero[name].view(np.uint32)), name
+    gated = _check_exact_grads(sh, g_nan, g_ref, g32, stats, "rgb")
+    # backward, rgb + disp + acc + raw seeds (nerf_b200_march_bwd_outs).  disp is seeded on rays with acc > 1e-4 only: on emptier
+    # rays disp = acc / depth is all rounding.  The raw seed is positive: a zero-mean seed on every sample makes the bias gradients
+    # (plain sums of dL/draw over all rows) cancel 40 to 1000-fold, and then the order of the fp32 sums decides their last digits
+    rng = np.random.default_rng(4)
+    seeds = {"rgb_map": rng.standard_normal((N, 3)) * 1e-3, "disp_map": rng.standard_normal(N) * 1e-2 * (maps_ref["acc"] > 1e-4),
+             "acc_map": rng.standard_normal(N) * 1e-2, "raw": rng.random((N, S, 4)) * 1e-4}
+    seeds = {k: v.astype(np.float32) for k, v in seeds.items()}
+    seeds64 = {k: torch.from_numpy(v).double() for k, v in seeds.items()}
+    _, _, go_ref = _exact_reference(sh, packed, z, None, seeds=seeds64)
+    _, _, go32 = _exact_reference(sh, packed, z, None, torch.float32, seeds=seeds64)
+    go_nan = G.march_bwd_exact(sh.net, rays, zd, {k: G.dev(v) for k, v in seeds.items()}, L=sh.L, Lv=sh.Lv, fill=0xFF)
+    go_zero = G.march_bwd_exact(sh.net, rays, zd, {k: G.dev(v) for k, v in seeds.items()}, L=sh.L, Lv=sh.Lv, fill=0)
+    for name in go_zero:
+        assert np.array_equal(go_nan[name].view(np.uint32), go_zero[name].view(np.uint32)), name
+    gated_outs = _check_exact_grads(sh, go_nan, go_ref, go32, stats, "outs")
+    stats.update(gated_rgb=len(gated), gated_outs=len(gated_outs))
+    _record(f"exact_{sid}", stats)
+    assert gated and gated_outs, ("the loss has no well-conditioned gradient", stats)
+
+
+EXACT_GOLDEN_CASES = ["w128_d10", "L14_Lv8", "w100_nv_odd"]
+
+
+@pytest.mark.parametrize("case", EXACT_GOLDEN_CASES)
+def test_exact_shapes_render_against_reference(G, case):
+    """render() + img2mse + loss.backward() in fp32 on create_nerf-shaped nets the tensor-core path refuses, against the
+    reference's autograd (tests/golden/exact_shapes.npz), with test_render_against_reference's exact-path gates.  w100_nv_odd:
+    netwidth 100 and 33 rays x 33 / 65 samples, odd in both passes."""
+    _check_render_against_reference(G, "exact_shapes", case, (("fp32", "exact"),))
+
+
+# id -> (NeRF arguments, what the message names); skips = [3] with netdepth 4 is a skip after the last layer
+RENDER_REFUSED = {"skip_D_minus_1": (dict(D=4, W=64, skips=[3]), "skip layer must be < netdepth - 1"),
+                  "W50": (dict(D=2, W=50, skips=[]), "a multiple of 4"),
+                  "W260": (dict(D=2, W=260, skips=[]), "netwidth <= 256"),
+                  "D17": (dict(D=17, W=16, skips=[]), "netdepth must be in [1, 16]")}
+
+
+@pytest.mark.parametrize("case", list(RENDER_REFUSED))
+def test_exact_path_refusals_through_render(G, case):
+    """render() in fp32 refuses the net before it launches anything and leaves every .grad as it was; the coarse net is a
+    good one that already holds a gradient."""
+    kw_net, msg = RENDER_REFUSED[case]
+    sb = G.synth.ray_batch("lego", 16, seed=2)
+    good = G.nb.NeRF(D=2, W=64, input_ch=63, input_ch_views=27, output_ch=5, skips=[], use_viewdirs=True).to(G.DEV)
+    bad = G.nb.NeRF(input_ch=63, input_ch_views=27, output_ch=5, use_viewdirs=True, **kw_net).to(G.DEV)
+    for p in list(good.parameters()) + list(bad.parameters()):
+        p.grad = torch.full_like(p, 0.5)
+    before = [p.grad.clone() for p in list(good.parameters()) + list(bad.parameters())]
+    G.nb.set_precision("fp32")
+    try:
+        for nets in ((bad, None), (good, bad)):
+            n0 = G.nb.launch_count()
+            with pytest.raises(RuntimeError, match=re.escape(msg)):
+                G.nb.render(400, 400, sb["K"], rays=G.dev(sb["rays"]), **_render_kw(G, nets, N_samples=8, N_importance=8))
+            assert G.nb.launch_count() == n0, case
+    finally:
+        G.nb.set_precision("tc_fp16")
+    for p, g in zip(list(good.parameters()) + list(bad.parameters()), before):
+        assert torch.equal(p.grad, g)
+
+
+def test_tensor_core_refusal_of_another_width_points_to_the_exact_path(G):
+    sb = G.synth.ray_batch("lego", 16, seed=2)
+    net = G.nb.NeRF(D=8, W=128, input_ch=63, input_ch_views=27, output_ch=5, skips=[4], use_viewdirs=True).to(G.DEV)
+    with pytest.raises(RuntimeError, match=re.escape("set_precision('fp32')")):
+        G.nb.render(400, 400, sb["K"], rays=G.dev(sb["rays"]), **_render_kw(G, (net, net), N_samples=8, N_importance=8))
+    G.nb.set_precision("fp32")
+    try:
+        rgb, _, _, _ = G.nb.render(400, 400, sb["K"], rays=G.dev(sb["rays"]), **_render_kw(G, (net, net), N_samples=8, N_importance=8))
+    finally:
+        G.nb.set_precision("tc_fp16")
+    _finite("rgb", rgb.detach().cpu().numpy())
