@@ -21,6 +21,8 @@ int nerf_b200_selftest_gemm_tn(const float* X, const float* Y, float* out, int l
 /* one CTA per SM streams its own bytes_per_cta of `buf`: mode 0 cp.async.bulk g2s ring, 1 cp.async 16 B ring, 2 cp.async.bulk s2g,
  * 3 st.global.v4, 4 ld.global.v4; scatter != 0: the chunks of a region are visited in a strided order; out[nblocks + 1] int64 = cycles per CTA */
 int nerf_b200_debug_dram_stream(void* buf, size_t bytes_per_cta, int chunk, int stages, int mode, int nblocks, int scatter, void* out_i64, void* stream);
+/* the same; shared_bytes != 0 (mode 0): every CTA streams the first shared_bytes of buf cyclically (L2-resident), bytes_per_cta in all */
+int nerf_b200_debug_l2_stream(void* buf, size_t bytes_per_cta, size_t shared_bytes, int chunk, int stages, int mode, int nblocks, int scatter, void* out_i64, void* stream);
 int nerf_b200_debug_hbm_stream(const void* src, void* dst, size_t bytes, int mode, int nblocks, void* stream);
 #ifdef __cplusplus
 }

@@ -142,6 +142,7 @@ SIGNATURES = {
 DEV_SIGNATURES = {
     "nerf_b200_dev_last_error": (C.c_char_p, []),
     "nerf_b200_debug_dram_stream": (C.c_int, [c_fp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_fp, c_fp]),
+    "nerf_b200_debug_l2_stream": (C.c_int, [c_fp, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_fp, c_fp]),
     "nerf_b200_debug_hbm_stream": (C.c_int, [c_fp, c_fp, C.c_size_t, C.c_int, C.c_int, c_fp]),
     "nerf_b200_selftest_gemm": (C.c_int, [c_fp, c_fp, C.c_int, C.c_int, c_fp, c_fp, C.c_size_t, c_fp]),
     "nerf_b200_selftest_gemm_tn": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, C.c_int, c_fp]),

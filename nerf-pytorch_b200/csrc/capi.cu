@@ -11,6 +11,9 @@
 #include <stdlib.h>
 
 namespace nb {
+#ifdef NERF_B200_PHASE_PROBE
+static long long g_phase_launches = 0;      // forward launches since the last nerf_b200_phase_probe_reset
+#endif
 thread_local char g_err[512] = {0};
 long long g_launches = 0;
 int set_error(int code, const char* fmt, ...) {
@@ -125,8 +128,8 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
   p.rays_per_cta = plan.rays_per_cta;
   NB_CHECK_ARG((long long)p.rays_per_cta * S < (1ll << 30), "rays_per_cta * S overflows");
   if (!ds->optin_fwd) {
-    if (int rc = smem_optin((const void*)march_wg_kernel<false>, SM_ALLOC)) return rc;
-    if (int rc = smem_optin((const void*)march_wg_kernel<true>, SM_ALLOC)) return rc;
+    if (int rc = smem_optin((const void*)march_wg_kernel<false>, FWD_ALLOC)) return rc;
+    if (int rc = smem_optin((const void*)march_wg_kernel<true>, FWD_ALLOC)) return rc;
     ds->optin_fwd = true;
   }
   TrainSaveDev sv;
@@ -148,8 +151,14 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
     cudaEventRecord(tl->a, st);
   }
   p.chunks = pk + PL.off_chunks;
-  if (save) march_wg_kernel<true><<<plan.grid, TC_THREADS, SM_ALLOC, st>>>(p, sv);
-  else march_wg_kernel<false><<<plan.grid, TC_THREADS, SM_ALLOC, st>>>(p, sv);
+#ifdef NERF_B200_PHASE_PROBE
+  {
+    const int slot = (int)(g_phase_launches++ % PH_SLOTS);
+    NB_CUDA(cudaMemcpyToSymbolAsync(g_fwd_phase_slot, &slot, sizeof(int), 0, cudaMemcpyHostToDevice, st));
+  }
+#endif
+  if (save) march_wg_kernel<true><<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, sv);
+  else march_wg_kernel<false><<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, sv);
   if (tl) cudaEventRecord(tl->b, st);
   NB_LAUNCH_OK("march_wg_kernel");
   return 0;
@@ -1219,5 +1228,27 @@ int nerf_b200_adam_step(float* params, const float* grads, float* exp_avg, float
   NB_LAUNCH_OK("adam_advance_kernel");
   return 0;
 }
+
+#ifdef NERF_B200_PHASE_PROBE
+// Experiments build only (tools/forward_phase_probe.py): zero the forward's phase counters (fused_wg.cuh: Phases) and the
+// launch count that picks their slot; copy them out as uint64 [PH_SLOTS][PH_MAX_CTAS][2][PH_N].
+int nerf_b200_phase_probe_reset(void) {
+  static unsigned long long zeros[PH_SLOTS][PH_MAX_CTAS][2][PH_N];
+  NB_CUDA(cudaDeviceSynchronize());
+  NB_CUDA(cudaMemcpyToSymbol(g_fwd_phase, zeros, sizeof(zeros)));
+  g_phase_launches = 0;
+  return 0;
+}
+int nerf_b200_phase_probe_read(void* out, size_t bytes) {
+  NB_CHECK_ARG(out && bytes == sizeof(g_fwd_phase), "out must hold the whole counter table");
+  NB_CUDA(cudaDeviceSynchronize());
+  NB_CUDA(cudaMemcpyFromSymbol(out, g_fwd_phase, bytes));
+  return 0;
+}
+int nerf_b200_phase_probe_shape(int* slots, int* max_ctas, int* phases) {
+  *slots = PH_SLOTS; *max_ctas = PH_MAX_CTAS; *phases = PH_N;
+  return 0;
+}
+#endif
 
 }  // extern "C"

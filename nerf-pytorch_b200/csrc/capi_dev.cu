@@ -68,13 +68,18 @@ int nerf_b200_debug_hbm_stream(const void* src, void* dst, size_t bytes, int mod
 }
 
 int nerf_b200_debug_dram_stream(void* buf, size_t bytes_per_cta, int chunk, int stages, int mode, int nblocks, int scatter, void* out_i64, void* stream) {
+  return nerf_b200_debug_l2_stream(buf, bytes_per_cta, 0, chunk, stages, mode, nblocks, scatter, out_i64, stream);
+}
+
+int nerf_b200_debug_l2_stream(void* buf, size_t bytes_per_cta, size_t shared_bytes, int chunk, int stages, int mode, int nblocks, int scatter, void* out_i64, void* stream) {
   NB_CHECK_ARG(buf && out_i64 && nblocks > 0 && mode >= 0 && mode <= 4, "bad arguments");
   NB_CHECK_ARG(chunk >= 1024 && chunk % 1024 == 0 && stages >= 1 && stages <= 8 && (size_t)stages * chunk <= 196608, "ring too large");
   NB_CHECK_ARG(bytes_per_cta % (size_t)chunk == 0, "bytes_per_cta must be a multiple of chunk");
+  NB_CHECK_ARG(shared_bytes == 0 || (mode == 0 && shared_bytes % (size_t)chunk == 0), "a shared region is streamed by mode 0, in whole chunks");
   const size_t sm = (size_t)stages * chunk + 512 + 1024;
   if (int rc = smem_optin((const void*)dram_stream_probe_kernel, sm)) return rc;
   dram_stream_probe_kernel<<<nblocks, DSP_THREADS, sm, (cudaStream_t)stream>>>(static_cast<uint8_t*>(buf), (unsigned long long)bytes_per_cta, chunk, stages, mode,
-                                                                              static_cast<long long*>(out_i64), scatter);
+                                                                              static_cast<long long*>(out_i64), scatter, (unsigned long long)shared_bytes);
   NB_LAUNCH_OK("dram_stream_probe_kernel");
   return 0;
 }

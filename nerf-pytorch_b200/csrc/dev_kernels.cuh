@@ -142,20 +142,25 @@ __global__ void __launch_bounds__(512) hbm_stream_kernel(const uint4* __restrict
 //           cp.async.mbarrier.arrive.noinc
 //   mode 2: cp.async.bulk shared->global of `chunk` bytes, at most `stages` bulk groups pending (wait_group.read)
 //   mode 3: st.global.v4 by 512 threads          mode 4: ld.global.v4 by 512 threads (8 loads in flight per thread)
+// shared_bytes != 0 (mode 0 only): every CTA streams the SAME first `shared_bytes` of `buf`, cyclically, for bytes_per_cta in
+// all -- an L2-resident stream, as the weight chunks of the fused forward (every CTA walks one 1 179 648-byte chunk sequence).
 // out[blockIdx.x] = clock cycles of the CTA's stream.
 constexpr int DSP_THREADS = 512;
 __global__ void __launch_bounds__(DSP_THREADS, 1) dram_stream_probe_kernel(uint8_t* __restrict__ buf, unsigned long long bytes_per_cta, int chunk, int stages,
-                                                                           int mode, long long* out, int scatter) {
+                                                                           int mode, long long* out, int scatter, unsigned long long shared_bytes) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t sb = ptx::smem_u32(smem);
   const uint32_t BAR = (uint32_t)stages * (uint32_t)chunk;
   const int warp = threadIdx.x >> 5;
-  uint8_t* base = buf + (size_t)blockIdx.x * bytes_per_cta;
+  uint8_t* base = shared_bytes ? buf : buf + (size_t)blockIdx.x * bytes_per_cta;
   const int n = (int)(bytes_per_cta / (unsigned)chunk);
   // scatter: chunk i of the CTA's region is visited in a strided order (i * 37 mod n: successive chunks ~600 KB apart for 16 KB
   // chunks), like the per-tile records of the training kernels, instead of front to back
-  auto at = [&](int i) -> size_t { return (size_t)(scatter ? (int)(((long long)i * 37) % n) : i) * (size_t)chunk; };
+  auto at = [&](int i) -> size_t {
+    if (shared_bytes) return ((size_t)i * (size_t)chunk) % (size_t)shared_bytes;
+    return (size_t)(scatter ? (int)(((long long)i * 37) % n) : i) * (size_t)chunk;
+  };
   if (threadIdx.x == 0) {
     for (int i = 0; i < stages; ++i) { ptx::mbar_init(sb + BAR + 8 * i, mode == 1 ? 128 : 1); ptx::mbar_init(sb + BAR + 128 + 8 * i, 1); }
     ptx::fence_mbar_init();

@@ -36,6 +36,20 @@ constexpr uint32_t SM_MISC = SM_BARS + 256;                     // 212256: compo
 constexpr uint32_t SM_ALLOC = SM_MISC + 128;                    // 212384 (dynamic smem base is 1024-aligned: checked at run time)
 static_assert(SM_ALLOC <= 227 * 1024, "shared-memory map exceeds the per-block limit");
 
+// The forward's own map (march_wg_kernel).  Its encodings are one 8 KB K-block per warpgroup (dgrad's seed tiles need 16 KB),
+// so packing them frees 16 KB, and with the slack under the limit the ring gets two more stages: the producer keeps streaming
+// while both MMA warpgroups run a tile's sampler and compositor, which take longer than six stages' worth of the stream.
+constexpr int FWD_NST = 8;                                      // weight ring stages of the forward (16 KB each)
+constexpr uint32_t FWD_ENC = 65536;                             // 2 x 8 KB   encoded inputs (1 K-block), one per warpgroup
+constexpr uint32_t FWD_WRING = 81920;                           // 8 x 16 KB  weight ring
+constexpr uint32_t FWD_HEADS = FWD_WRING + FWD_NST * TC_STAGE_BYTES;   // 212992: head weights, 4128 B
+constexpr uint32_t FWD_BIAS = FWD_HEADS + 4128;                 // 217120: fp32 biases [TC_MAXD + 1][256]
+constexpr uint32_t FWD_RAW = FWD_BIAS + (TC_MAXD + 1) * 1024;   // 226336: 128 x float4 raw rows of the tile
+constexpr uint32_t FWD_BARS = FWD_RAW + 2048;                   // 228384: mbarriers full, empty [FWD_NST]
+constexpr uint32_t FWD_MISC = FWD_BARS + 16 * FWD_NST;          // 228512: compositing carry
+constexpr uint32_t FWD_ALLOC = FWD_MISC + 128;                  // 228640
+static_assert(FWD_ALLOC <= 227 * 1024, "the forward's shared-memory map exceeds the per-block limit");
+
 // heads region (floats): viewdirs: alpha_w[256] rgb_w[3][128] alpha_b rgb_b[3]; else output_w[4][256] output_b[4]
 constexpr int HEADS_FLOATS = 1032;
 

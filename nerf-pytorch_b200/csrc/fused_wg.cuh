@@ -33,11 +33,50 @@ __device__ __forceinline__ uint32_t half_off(int r, int c) {
 __device__ __forceinline__ uint64_t desc_act(uint32_t addr) { return ptx::gmma_desc(addr, 16, 1024, ptx::GMMA_SW128); }
 __device__ __forceinline__ uint64_t desc_w(uint32_t addr) { return ptx::gmma_desc(addr, 16, 512, ptx::GMMA_SW64); }
 
-// Weight ring shared by the producer and both MMA warpgroups: every party walks the same chunk sequence.
-struct Ring {
-  uint32_t full, empty, stage, phase;
-  __device__ __forceinline__ void advance() { if (++stage == TC_NST) { stage = 0; phase ^= 1; } }
+// Phase counters of an experiments build (-DNERF_B200_PHASE_PROBE, tools/forward_phase_probe.py): thread 0 of each MMA
+// warpgroup adds the clock64 time it spends in each phase to g_fwd_phase[slot][CTA][warpgroup][phase], slot = the launch
+// count modulo PH_SLOTS (coarse, fine).  PH_FULL: waits on a ring stage's full barrier; PH_GAP: from the end of a layer's
+// MMAs (wgmma_wait<0>) to the next layer's first full-barrier wait, inside a tile; PH_SAMPLER / PH_COMPOSITOR: from the
+// tile's start to its first layer / from its last layer's epilogue to its end; PH_TOTAL: the warpgroup's whole run.  The
+// product build compiles all of it to nothing.
+enum { PH_FULL, PH_GAP, PH_SAMPLER, PH_COMPOSITOR, PH_TOTAL, PH_N };
+#ifdef NERF_B200_PHASE_PROBE
+constexpr int PH_SLOTS = 2, PH_MAX_CTAS = 1024;
+__device__ unsigned long long g_fwd_phase[PH_SLOTS][PH_MAX_CTAS][2][PH_N];
+__device__ int g_fwd_phase_slot;
+struct Phases {
+  long long acc[PH_N] = {0, 0, 0, 0, 0}, t0 = 0, tb = 0;
+  __device__ __forceinline__ void begin() { tb = clock64(); }
+  __device__ __forceinline__ void start() { t0 = clock64(); }
+  __device__ __forceinline__ void stop(int k) { acc[k] += clock64() - t0; }
+  __device__ __forceinline__ void wait_full(uint32_t bar, uint32_t parity) {
+    const long long a = clock64();
+    ptx::mbar_wait(bar, parity);
+    acc[PH_FULL] += clock64() - a;
+  }
+  __device__ __forceinline__ void flush(int w, int t) {
+    acc[PH_TOTAL] = clock64() - tb;
+    if (t == 0 && blockIdx.x < PH_MAX_CTAS)
+      for (int k = 0; k < PH_N; ++k) atomicAdd(&g_fwd_phase[g_fwd_phase_slot][blockIdx.x][w][k], (unsigned long long)acc[k]);
+  }
 };
+#else
+struct Phases {
+  __device__ __forceinline__ void begin() {}
+  __device__ __forceinline__ void start() {}
+  __device__ __forceinline__ void stop(int) {}
+  __device__ __forceinline__ void wait_full(uint32_t bar, uint32_t parity) { ptx::mbar_wait(bar, parity); }
+  __device__ __forceinline__ void flush(int, int) {}
+};
+#endif
+
+// Weight ring shared by the producer and both MMA warpgroups: every party walks the same chunk sequence.
+template <int NST>
+struct RingN {
+  uint32_t full, empty, stage, phase;
+  __device__ __forceinline__ void advance() { if (++stage == NST) { stage = 0; phase ^= 1; } }
+};
+using Ring = RingN<TC_NST>;
 
 // One K = 32 chunk into a 64 x N accumulator (two K = 16 instructions); `acc0` = 0 overwrites the accumulator
 template <int R>
@@ -53,13 +92,13 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[R], uint64_t ad, uint64_t
 
 // All chunks of one layer: `a_of(c)` gives chunk c's A descriptor.  The previous chunk's stage is released as soon as the
 // wgmma group of the next one is in flight; on return the accumulator is complete.
-template <int R, typename AOf>
-__device__ __forceinline__ void mma_layer(float (&acc)[R], Ring& rg, uint32_t ring_base, int nch, bool from_zero, AOf a_of) {
+template <int R, typename RG, typename AOf>
+__device__ __forceinline__ void mma_layer(float (&acc)[R], RG& rg, uint32_t ring_base, int nch, bool from_zero, AOf a_of, Phases& ph) {
   ptx::wgmma_fence();
   int pending = -1;
   for (int c = 0; c < nch; ++c) {
     const uint32_t s = rg.stage;
-    ptx::mbar_wait(rg.full + 8 * s, rg.phase);
+    ph.wait_full(rg.full + 8 * s, rg.phase);
     mma_chunk(acc, a_of(c), desc_w(ring_base + s * TC_STAGE_BYTES), (from_zero && c == 0) ? 0u : 1u);
     ptx::wgmma_commit();
     if (pending >= 0) { ptx::wgmma_wait<1>(); ptx::mbar_arrive(rg.empty + 8 * pending); }
@@ -69,6 +108,11 @@ __device__ __forceinline__ void mma_layer(float (&acc)[R], Ring& rg, uint32_t ri
   ptx::wgmma_wait<0>();
   ptx::fence_regs(acc);
   if (pending >= 0) ptx::mbar_arrive(rg.empty + 8 * pending);
+}
+template <int R, typename AOf>
+__device__ __forceinline__ void mma_layer(float (&acc)[R], Ring& rg, uint32_t ring_base, int nch, bool from_zero, AOf a_of) {
+  Phases none;
+  mma_layer(acc, rg, ring_base, nch, from_zero, a_of, none);
 }
 
 // OR of a value over the four lanes that share an accumulator row
@@ -86,9 +130,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
   uint8_t* smem = tc_smem;
   const uint32_t sb = ptx::smem_u32(smem);
   if ((sb & 1023u) != 0) __trap();
-  float* s_heads = reinterpret_cast<float*>(smem + SM_HEADS);
-  float* s_bias = reinterpret_cast<float*>(smem + SM_BIAS);
-  const uint32_t a_heads = sb + SM_HEADS, a_carry = sb + SM_MISC;
+  float* s_heads = reinterpret_cast<float*>(smem + FWD_HEADS);
+  float* s_bias = reinterpret_cast<float*>(smem + FWD_BIAS);
+  const uint32_t a_heads = sb + FWD_HEADS, a_carry = sb + FWD_MISC;
   const int D = p.D, NL = p.D + (p.use_viewdirs ? 2 : 0);
 
   // this CTA's rays / rows; the number of super-tiles is the tile plan's (train_common.cuh: plan_cta_nst)
@@ -99,9 +143,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
 
   for (int i = threadIdx.x; i < HEADS_FLOATS; i += TC_THREADS) s_heads[i] = p.heads[i];
   for (int i = threadIdx.x; i < (TC_MAXD + 1) * 256; i += TC_THREADS) s_bias[i] = p.bias[i];
-  Ring rg{sb + SM_BARS, sb + SM_BARS + 8 * TC_NST, 0, 0};
+  RingN<FWD_NST> rg{sb + FWD_BARS, sb + FWD_BARS + 8 * FWD_NST, 0, 0};
   if (threadIdx.x == 0) {
-    for (int i = 0; i < TC_NST; ++i) { ptx::mbar_init(rg.full + 8 * i, 1); ptx::mbar_init(rg.empty + 8 * i, 256); }
+    for (int i = 0; i < FWD_NST; ++i) { ptx::mbar_init(rg.full + 8 * i, 1); ptx::mbar_init(rg.empty + 8 * i, 256); }
     sts32(a_carry + CARRY_T, 1.0f); sts32(a_carry + CARRY_R, 0.f); sts32(a_carry + CARRY_G, 0.f); sts32(a_carry + CARRY_B, 0.f);
     sts32(a_carry + CARRY_D, 0.f); sts32(a_carry + CARRY_A, 0.f); st_release_shared(a_carry + CARRY_TURN, 0u);
     ptx::fence_mbar_init();
@@ -120,7 +164,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
           for (int c = 0; c < nch; ++c) {
             ptx::mbar_wait(rg.empty + 8 * rg.stage, rg.phase ^ 1);
             ptx::mbar_arrive_expect_tx(rg.full + 8 * rg.stage, bytes);
-            ptx::bulk_g2s(sb + SM_WRING + rg.stage * TC_STAGE_BYTES, src, bytes, rg.full + 8 * rg.stage);
+            ptx::bulk_g2s(sb + FWD_WRING + rg.stage * TC_STAGE_BYTES, src, bytes, rg.full + 8 * rg.stage);
             src += bytes;
             rg.advance();
           }
@@ -135,17 +179,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
   const int w = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
   const int q4 = lane & 3;
   const int r0 = 16 * wq + (lane >> 2), r1 = r0 + 8;              // this thread's two accumulator rows (of the warpgroup's 64)
-  const uint32_t act = sb + SM_ACT + (uint32_t)w * 32768u, enc = sb + SM_ENC + (uint32_t)w * 16384u;
-  const uint32_t ring = sb + SM_WRING;
+  const uint32_t act = sb + SM_ACT + (uint32_t)w * 32768u, enc = sb + FWD_ENC + (uint32_t)w * 8192u;
+  const uint32_t ring = sb + FWD_WRING;
   const uint64_t l2_first = EMIT ? ptx::l2_policy_evict_first() : 0ull;
   auto wg_sync = [&]() { ptx::named_bar_sync(1 + w, 128); };
   // row-dependent parts of the swizzled addresses of this thread's pairs: column pair (8 j + 2 q4) of row r sits at
   // rowoff(r) + (j >> 3) * 8192 + (((j & 7) ^ (r & 7)) << 4) + 4 q4
   const uint32_t ro0 = (uint32_t)((r0 >> 3) * 1024 + (r0 & 7) * 128 + 4 * q4), ro1 = (uint32_t)((r1 >> 3) * 1024 + (r1 & 7) * 128 + 4 * q4);
   auto pair_addr = [&](uint32_t base, uint32_t ro, int r, int j) { return base + ro + (uint32_t)(j >> 3) * 8192u + (uint32_t)(((j & 7) ^ (r & 7)) << 4); };
+  // stmatrix row address of this lane: row 16 wq + 8 ((lane >> 3) & 1) + (lane & 7), column group j + (lane >> 4) for even j,
+  // whose swizzled 16-byte chunk is (j & 7) ^ sm_key
+  const int sm_r = 16 * wq + 8 * ((lane >> 3) & 1) + (lane & 7);
+  const uint32_t sm_row = act + act_row_off(sm_r), sm_key = (uint32_t)((lane >> 4) ^ (lane & 7));
 
   float acc[128];
+  Phases ph;
+  ph.begin();
   for (int tile = 0; tile < 2 * nst; ++tile) {
+    ph.start();
     const int st = tile >> 1, X = tile & 1;
     uint8_t* const arec = EMIT ? sv.act + (size_t)((blockIdx.x * sv.nst_plan + st) * 2 + X) * sv.rec_act : nullptr;
     uint8_t* const mrec = EMIT ? sv.mask + (size_t)((blockIdx.x * sv.nst_plan + st) * 2 + X) * sv.rec_mask : nullptr;
@@ -183,6 +234,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
     if (EMIT && t == 0) { ptx::bulk_s2g_hint(arec + (uint32_t)w * 8192u, enc, 8192u, l2_first); ptx::bulk_commit(); }
 
     float hp[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};   // head partial sums of this thread's columns, per row
+    ph.stop(PH_SAMPLER);
     for (int l = 0; l < NL; ++l) {
       const int nch = tc_layer_chunks(l, D, p.skip);
       const bool skip_layer = (l < D && p.skip >= 0 && l == p.skip + 1);
@@ -199,7 +251,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
           const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
           acc[4 * j] = b.x; acc[4 * j + 1] = b.y; acc[4 * j + 2] = b.x; acc[4 * j + 3] = b.y;
         }
-        mma_layer(acc, rg, ring, nch, false, a_of);
+        if (l > 0) ph.stop(PH_GAP);
+        mma_layer(acc, rg, ring, nch, false, a_of, ph);
+        ph.start();
         if (EMIT && t == 0) ptx::bulk_wait_read0();
         wg_sync();                                                // the whole warpgroup's MMAs and copies are done with the operand
         const bool last_pts = (l == D - 1);
@@ -250,12 +304,18 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
         // records it (output_linear's weight gradient reads it, dA_seed_output_kernel in bwd_wg.cuh)
         if (EMIT || !(last_pts && !p.use_viewdirs)) {
           const bool relu = l < D;
+          // column groups j, j + 1 of the warp's 16 rows as four 8 x 8 matrices (the accumulator fragment is stmatrix's):
+          // matrix m = (group j + (m >> 1), rows + 8 (m & 1)); this lane addresses row (lane & 7) of matrix lane >> 3
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const uint32_t h0 = relu ? ptx::cvt_relu_f16x2(acc[4 * j], acc[4 * j + 1]) : ptx::cvt_f16x2(acc[4 * j], acc[4 * j + 1]);
-            const uint32_t h1 = relu ? ptx::cvt_relu_f16x2(acc[4 * j + 2], acc[4 * j + 3]) : ptx::cvt_f16x2(acc[4 * j + 2], acc[4 * j + 3]);
-            ptx::st_shared_b32(pair_addr(act, ro0, r0, j), h0);
-            ptx::st_shared_b32(pair_addr(act, ro1, r1, j), h1);
+          for (int j = 0; j < 32; j += 2) {
+            uint32_t h[4];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int g = j + e;
+              h[2 * e] = relu ? ptx::cvt_relu_f16x2(acc[4 * g], acc[4 * g + 1]) : ptx::cvt_f16x2(acc[4 * g], acc[4 * g + 1]);
+              h[2 * e + 1] = relu ? ptx::cvt_relu_f16x2(acc[4 * g + 2], acc[4 * g + 3]) : ptx::cvt_f16x2(acc[4 * g + 2], acc[4 * g + 3]);
+            }
+            ptx::stmatrix_x4(sm_row + (uint32_t)(j >> 3) * 8192u + ((uint32_t)((j & 7) ^ sm_key) << 4), h[0], h[1], h[2], h[3]);
           }
           ptx::fence_proxy_async_smem();
           wg_sync();
@@ -267,7 +327,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
       } else {
         // ---- views_linears[0] (N = 128) + per-ray view bias, ReLU, rgb_linear ----
         float* accv = acc;                                        // the first 64 accumulators
-        mma_layer(*reinterpret_cast<float(*)[64]>(accv), rg, ring, nch, true, a_of);
+        ph.stop(PH_GAP);
+        mma_layer(*reinterpret_cast<float(*)[64]>(accv), rg, ring, nch, true, a_of, ph);
+        ph.start();
         wg_sync();
         const float* vb0 = p.vb + nray[0] * 128;
         const float* vb1 = p.vb + nray[1] * 128;
@@ -312,12 +374,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
     }
 
     // ---- heads: full row sums over the quad -> raw rows of the tile -> compositing ----
+    ph.start();
     float raw[2][4];
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
       for (int k = 0; k < 4; ++k) raw[h][k] = quad_sum(hp[h][k]);
-    const uint32_t a_raw = sb + SM_RAW + (uint32_t)(64 * w) * 16u;
+    const uint32_t a_raw = sb + FWD_RAW + (uint32_t)(64 * w) * 16u;
     if (q4 == 0) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -338,8 +401,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
       if (n_ray < 0) n_ray = 0;
       composite_rows(p, lds128(a_raw + (uint32_t)tr * 16u), valid, lr, rl, n_ray, row_begin, st, X, 2 * w + wq, lane, a_carry);
     }
+    ph.stop(PH_COMPOSITOR);
   }
   if (EMIT && t == 0) ptx::bulk_wait_all();
+  ph.flush(w, t);
 }
 
 }  // namespace nb

@@ -122,6 +122,10 @@ __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t
 __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t a) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
 }
+// four 8 x 8 fp16 matrices, register i of every lane into matrix i; lanes 8 i .. 8 i + 7 give the addresses of its 8 rows
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
 __device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
   uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory"); return v;
 }
