@@ -64,6 +64,9 @@ typedef struct NerfRenderCfg {
 
 #define NERF_B200_PREC_TC_FP16 0   /* wgmma f16, fp16 operands, fp32 accumulate (fast path)        */
 #define NERF_B200_PREC_FP32    1   /* CUDA-core fp32 FMA chain (exact mode, validation)             */
+#define NERF_B200_PREC_TC_SPLIT 2  /* wgmma f16, each operand split into hi + lo fp16 halves, three  */
+                                   /* MMAs per K-step, fp32 accumulate: fp32-class inference; packed */
+                                   /* by nerf_b200_pack_weights_split; no training-mode records      */
 
 /* Outputs of one network pass over N rays x S samples.  NULL pointers are skipped. */
 typedef struct NerfPassOut {
@@ -85,10 +88,15 @@ int nerf_b200_embed(const float* x, int64_t M, int L, float* out, void* stream);
 /* (replaces nothing in the reference; it is the analogue of `.to(device)` at run_nerf.py:191)     */
 size_t nerf_b200_packed_bytes(const NerfNetParams* net);
 int    nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t packed_bytes, void* stream);
+/* the split image of precision TC_SPLIT: per-layer power-of-two weight scales, hi | lo fp16 chunks of */
+/* the scaled weights, the same fp32 tables; no backward stream                                      */
+size_t nerf_b200_packed_bytes_split(const NerfNetParams* net);
+int    nerf_b200_pack_weights_split(const NerfNetParams* net, void* packed, size_t packed_bytes, void* stream);
 
 /* ---- run_network + batchify + NeRF.forward (run_nerf.py:27-51, run_nerf_helpers.py:96-119) --- */
 /* pts [N*S,3], viewdirs [N,3] (NULL when the net has no view input) -> raw [N*S,4].               */
-/* precision TC_FP16 needs `packed` (from nerf_b200_pack_weights); FP32 needs `net`.               */
+/* precision TC_FP16 needs `packed` (from nerf_b200_pack_weights), TC_SPLIT the split image        */
+/* (nerf_b200_pack_weights_split); FP32 needs `net`.                                                */
 int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, int S,
                           const NerfNetParams* net, const void* packed, int multires,
                           int multires_views, int precision, float* raw,

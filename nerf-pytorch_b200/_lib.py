@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libnerf_b200.so")
 MAX_D = 16
-PREC_TC_FP16, PREC_FP32 = 0, 1
+PREC_TC_FP16, PREC_FP32, PREC_TC_SPLIT = 0, 1, 2
 
 c_fp = C.c_void_p     # device pointers travel as integers
 
@@ -74,6 +74,8 @@ SIGNATURES = {
     "nerf_b200_embed": (C.c_int, [c_fp, C.c_int64, C.c_int, c_fp, c_fp]),
     "nerf_b200_packed_bytes": (C.c_size_t, [C.POINTER(NerfNetParams)]),
     "nerf_b200_pack_weights": (C.c_int, [C.POINTER(NerfNetParams), c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_packed_bytes_split": (C.c_size_t, [C.POINTER(NerfNetParams)]),
+    "nerf_b200_pack_weights_split": (C.c_int, [C.POINTER(NerfNetParams), c_fp, C.c_size_t, c_fp]),
     "nerf_b200_run_network": (C.c_int, [c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp, C.c_int,
                                         C.c_int, C.c_int, c_fp, c_fp, C.c_size_t, c_fp]),
     "nerf_b200_raw2outputs": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, c_fp, C.c_int64, C.c_int, C.c_int,

@@ -24,7 +24,7 @@ import torch.nn.functional as F
 
 from . import _lib
 from ._lib import (NerfCamera, NerfNetGrads, NerfNetParams, NerfPassOut, NerfRenderCfg, NerfTrainSave, PREC_FP32, PREC_TC_FP16,
-                   check)
+                   PREC_TC_SPLIT, check)
 
 __all__ = ["NeRF", "Embedder", "get_embedder", "sample_pdf", "raw2outputs", "run_network", "batchify",
            "batchify_rays", "render_rays", "render", "create_nerf",
@@ -39,18 +39,24 @@ mse2psnr = lambda x: -10. * torch.log(x) / torch.log(torch.tensor([10.], device=
 to8b = lambda x: (255 * np.clip(x, 0, 1)).astype(np.uint8)                          # :11
 
 
+_PRECISIONS = {"tc_fp16": PREC_TC_FP16, "fp32": PREC_FP32, "tc_split": PREC_TC_SPLIT}
+
+
 def set_precision(mode: str):
-    """'tc_fp16' (wgmma fp16 operands / fp32 accumulate, default) or 'fp32' (CUDA-core exact mode)."""
-    _PRECISION["mode"] = {"tc_fp16": PREC_TC_FP16, "fp32": PREC_FP32}[mode]
+    """'tc_fp16' (wgmma fp16 operands / fp32 accumulate, default), 'fp32' (CUDA-core exact mode) or 'tc_split' (wgmma with
+    every operand split into hi + lo fp16 halves, three MMAs per K-step into an fp32 accumulator: the fp32 path's accuracy on
+    tensor cores, for the forward; netwidth 256 only, like tc_fp16)."""
+    _PRECISION["mode"] = _PRECISIONS[mode]
 
 
 def get_precision() -> str:
-    return "tc_fp16" if _PRECISION["mode"] == PREC_TC_FP16 else "fp32"
+    return {v: k for k, v in _PRECISIONS.items()}[_PRECISION["mode"]]
 
 
 def set_backward(mode: str):
     """'tc' (default in tc_fp16 precision: wgmma backward from the forward's saved tile records, with or without view
-    directions) or 'exact' (fp32 CUDA-core recompute backward; always used in fp32 precision)."""
+    directions) or 'exact' (fp32 CUDA-core recompute backward; always used in fp32 and tc_split precision: tc_split's forward
+    is the split tensor-core pass, its backward recomputes the pass in fp32 on CUDA cores)."""
     if mode not in ("tc", "exact"):
         raise ValueError(mode)
     _PRECISION["backward"] = mode
@@ -159,6 +165,7 @@ class NeRF(nn.Module):
         else:
             self.output_linear = nn.Linear(W, output_ch)
         self._pack = None           # (key, packed fp16 weight stream) for the tensor-core path
+        self._pack_split = None     # (key, split hi | lo image) for precision tc_split
 
     def forward(self, x):
         """Evaluate on ALREADY-EMBEDDED rows [M, input_ch + input_ch_views] (run_nerf_helpers.py:96-119).
@@ -262,20 +269,29 @@ class NeRF(nn.Module):
         """fp16 UMMA-swizzled weight streams (forward chunks + the transposed chunks of the backward), re-packed
         whenever a parameter changed in place (optimizer.step bumps Parameter._version; load_state_dict / .to()
         change data_ptr) or invalidate_pack() was called."""
+        return self._packed_image("_pack", "")
+
+    def packed_split(self):
+        """The split image of precision tc_split (hi | lo fp16 halves of the scaled forward weights), cached apart from
+        packed() and re-packed on the same conditions."""
+        return self._packed_image("_pack_split", "_split")
+
+    def _packed_image(self, attr, kind):
         dev = self._check_device()
         key = (getattr(self, "_pack_epoch", 0),) + tuple((q.data_ptr(), q._version) for _, _, _, q in self._named_params())
-        if self._pack is not None and self._pack[0] == key:
-            return self._pack[1]
+        cached = getattr(self, attr, None)
+        if cached is not None and cached[0] == key:
+            return cached[1]
         lib = _lib.load()
         n = self.net_params()
-        nbytes = lib.nerf_b200_packed_bytes(C.byref(n))
+        nbytes = getattr(lib, "nerf_b200_packed_bytes" + kind)(C.byref(n))
         if nbytes == 0:
             raise RuntimeError("nerf_b200: " + lib.nerf_b200_last_error().decode())
-        buf = self._pack[1] if (self._pack is not None and self._pack[1].numel() == nbytes and self._pack[1].device == dev) \
+        buf = cached[1] if (cached is not None and cached[1].numel() == nbytes and cached[1].device == dev) \
             else torch.empty(nbytes, dtype=torch.uint8, device=dev)
         with _on(buf):
-            check(lib.nerf_b200_pack_weights(C.byref(n), _ptr(buf), nbytes, _stream(buf)), "pack_weights")
-        self._pack = (key, buf)
+            check(getattr(lib, "nerf_b200_pack_weights" + kind)(C.byref(n), _ptr(buf), nbytes, _stream(buf)), "pack_weights" + kind)
+        setattr(self, attr, (key, buf))
         return buf
 
 
@@ -397,6 +413,13 @@ def _freqs_of(embed_fn, out_dim_hint=None):
     return int(L)
 
 
+def _packed_for(net, prec):
+    """The packed image a precision reads: packed() for tc_fp16, packed_split() for tc_split, None for fp32."""
+    if prec == PREC_TC_FP16:
+        return net.packed()
+    return net.packed_split() if prec == PREC_TC_SPLIT else None
+
+
 def run_network(inputs, viewdirs, fn, embed_fn, embeddirs_fn, netchunk=1024 * 64):
     """inputs [N,S,3] (+ viewdirs [N,3]) -> raw [N,S,4] in ONE fused kernel: encode + MLP.
     `netchunk` is accepted and ignored ("does not affect final results", run_nerf.py:78-79)."""
@@ -409,7 +432,7 @@ def run_network(inputs, viewdirs, fn, embed_fn, embeddirs_fn, netchunk=1024 * 64
     lib = _lib.load()
     n = fn.net_params()
     prec = _PRECISION["mode"]
-    packed = fn.packed() if prec == PREC_TC_FP16 else None
+    packed = _packed_for(fn, prec)
     raw = torch.empty((N * S, 4), device=inputs.device, dtype=torch.float32)
     ws_bytes = lib.nerf_b200_march_workspace_bytes(N, S)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=inputs.device)
@@ -531,10 +554,10 @@ class _RenderRays(torch.autograd.Function):
         Sc, Ni = cfgd["N_samples"], cfgd["N_importance"]
         Sf = Sc + Ni
         cfg = _cfg_struct(cfgd, ray_batch.shape[1])
-        tc = cfg.precision == PREC_TC_FP16
+        tc = cfg.precision == PREC_TC_FP16          # tc_split runs like fp32 here: no training-mode records, raw kept
         pc, pf = net_c.net_params(), (net_f.net_params() if net_f is not None else None)
-        pk_c = net_c.packed() if tc else None
-        pk_f = net_f.packed() if (tc and net_f is not None) else None
+        pk_c = _packed_for(net_c, cfg.precision)
+        pk_f = _packed_for(net_f, cfg.precision) if net_f is not None else None
         f32 = dict(device=dev, dtype=torch.float32)
         t_vals = _linspace01(Sc, dev)                                             # run_nerf.py:357
         u_det = _linspace01(Ni, dev) if Ni > 0 else None                          # run_nerf_helpers.py:205
@@ -865,7 +888,7 @@ def render(H, W, K, chunk=1024 * 32, rays=None, c2w=None, ndc=True, near=0., far
     packed = torch.empty((N, 11 if use_viewdirs else 8), device=dev, dtype=torch.float32)
 
     # one chunk, scalar bounds, one camera: the batch is built by render_rays' own prologue launch (see _DEFERRED_PACK)
-    defer = scalar_bounds and c2w_staticcam is None and N <= chunk and get_precision() == "tc_fp16"
+    defer = scalar_bounds and c2w_staticcam is None and N <= chunk and get_precision() in ("tc_fp16", "tc_split")
 
     def pack(o, d, view_src, cam, out, ndc_, viewdirs_):
         global _DEFERRED_PACK
@@ -1135,9 +1158,8 @@ class GraphedRender:
 
     def refresh(self):
         """Call after the networks' parameters changed (optimizer step, load_state_dict)."""
-        if _PRECISION["mode"] == PREC_TC_FP16:
-            for n in self._nets:
-                n.packed()
+        for n in self._nets:
+            _packed_for(n, _PRECISION["mode"])
 
     def __call__(self, rays_host):
         """rays_host: [2, n, 3] fp32 with 0 < n <= n_rays (pinned memory makes the copy asynchronous).  Returns the first n

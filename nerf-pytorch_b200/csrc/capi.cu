@@ -69,7 +69,7 @@ static int smem_optin(const void* fn, size_t bytes) {
 
 // per-device facts (SM count; which kernels already have their > 48 KB shared-memory opt-in): the library may be used
 // on several devices of one process, and cudaFuncSetAttribute is per device
-struct DeviceState { int sms; bool optin_fwd, optin_bwd; };
+struct DeviceState { int sms; bool optin_fwd, optin_bwd, optin_split; };
 static DeviceState* device_state() {
   static DeviceState st[64];
   static bool init[64] = {false};
@@ -80,7 +80,7 @@ static DeviceState* device_state() {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     st[dev].sms = n > 0 ? n : 132;
-    st[dev].optin_fwd = st[dev].optin_bwd = false;
+    st[dev].optin_fwd = st[dev].optin_bwd = st[dev].optin_split = false;
     cudaGetLastError();
     init[dev] = true;
   }
@@ -88,18 +88,27 @@ static DeviceState* device_state() {
 }
 static int num_sms() { return device_state()->sms; }
 
-// shared launcher of the fused tensor-core pass; `save` != NULL selects the training-mode kernel (EMIT)
+static bool is_tc(int precision) { return precision == NERF_B200_PREC_TC_FP16 || precision == NERF_B200_PREC_TC_SPLIT; }
+static PackLayout pack_layout_for(const NerfNetParams& net, int precision) {
+  return precision == NERF_B200_PREC_TC_SPLIT ? make_pack_layout_split(net) : make_pack_layout(net);
+}
+#define NB_SPLIT_TRAIN_MSG "precision TC_SPLIT has no training-mode records: it trains through the exact backward (nerf_b200_march_bwd)"
+
+// shared launcher of the fused tensor-core pass; `save` != NULL selects the training-mode kernel (EMIT); precision TC_SPLIT runs
+// march_split_kernel on the split packed image (nerf_b200_pack_weights_split)
 static int launch_march(const float* rays, int ray_stride, const float* z_vals, const float* pts,
                         const float* dirs, int dir_stride, const float* noise, long long N, int S,
                         const NerfNetParams* net, const void* packed, int L, int Lv, int white_bkgd, int do_composite,
                         const NerfPassOut* out, void* workspace, size_t workspace_bytes, const NerfTrainSave* save, const float* vb_pre,
-                        cudaStream_t st) {
+                        cudaStream_t st, int precision = NERF_B200_PREC_TC_FP16) {
   if (int rc = check_tc_net(net)) return rc;
-  NB_CHECK_ARG(packed != nullptr, "packed weights are NULL (call nerf_b200_pack_weights)");
+  const bool split = precision == NERF_B200_PREC_TC_SPLIT;
+  NB_CHECK_ARG(!(split && save), NB_SPLIT_TRAIN_MSG);
+  NB_CHECK_ARG(packed != nullptr, split ? "packed weights are NULL (call nerf_b200_pack_weights_split)" : "packed weights are NULL (call nerf_b200_pack_weights)");
   NB_CHECK_ARG(N > 0 && S > 0, "empty ray batch must be handled by the caller (N=%lld S=%d)", N, S);
   NB_CHECK_ARG((long long)N * S < (1ll << 40), "batch too large");
   NB_CHECK_ARG(3 + 6 * L == net->input_ch || (L == 0 && net->input_ch == 3), "multires %d does not match input_ch %d", L, net->input_ch);
-  const PackLayout PL = make_pack_layout(*net);
+  const PackLayout PL = pack_layout_for(*net, precision);
   const uint8_t* pk = static_cast<const uint8_t*>(packed);
   MarchParams p;
   memset(&p, 0, sizeof(p));
@@ -127,7 +136,11 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
   const TilePlan plan = make_tile_plan(N, S, ds->sms);
   p.rays_per_cta = plan.rays_per_cta;
   NB_CHECK_ARG((long long)p.rays_per_cta * S < (1ll << 30), "rays_per_cta * S overflows");
-  if (!ds->optin_fwd) {
+  if (split && !ds->optin_split) {
+    if (int rc = smem_optin((const void*)march_split_kernel, FWD_ALLOC)) return rc;
+    ds->optin_split = true;
+  }
+  if (!split && !ds->optin_fwd) {
     if (int rc = smem_optin((const void*)march_wg_kernel<false>, FWD_ALLOC)) return rc;
     if (int rc = smem_optin((const void*)march_wg_kernel<true>, FWD_ALLOC)) return rc;
     ds->optin_fwd = true;
@@ -157,6 +170,12 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
     NB_CUDA(cudaMemcpyToSymbolAsync(g_fwd_phase_slot, &slot, sizeof(int), 0, cudaMemcpyHostToDevice, st));
   }
 #endif
+  if (split) {
+    march_split_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, reinterpret_cast<const float*>(pk + PL.off_wscale));
+    if (tl) cudaEventRecord(tl->b, st);
+    NB_LAUNCH_OK("march_split_kernel");
+    return 0;
+  }
   if (save) march_wg_kernel<true><<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, sv);
   else march_wg_kernel<false><<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, sv);
   if (tl) cudaEventRecord(tl->b, st);
@@ -273,6 +292,62 @@ int nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t packed
   return 0;
 }
 
+size_t nerf_b200_packed_bytes_split(const NerfNetParams* net) {
+  if (!net || check_tc_net(net)) return 0;
+  return make_pack_layout_split(*net).total;
+}
+
+// the split image (precision TC_SPLIT, fused_tc.cuh: make_pack_layout_split): per-layer weight scales, the forward chunks as
+// hi | lo stages of the scaled weights, and the fp16 image's fp32 tables
+int nerf_b200_pack_weights_split(const NerfNetParams* net, void* packed, size_t packed_bytes, void* stream) {
+  if (int rc = check_tc_net(net)) return rc;
+  const PackLayout PL = make_pack_layout_split(*net);
+  NB_CHECK_ARG(packed && packed_bytes >= PL.total, "packed buffer too small (%zu < %zu)", packed_bytes, PL.total);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* dst = static_cast<uint8_t*>(packed);
+  float* scale = reinterpret_cast<float*>(dst + PL.off_wscale);
+  const int IC = net->input_ch, W = net->W;
+  SplitScaleJob sj;
+  memset(&sj, 0, sizeof(sj));
+  sj.n = PL.NL;
+  for (int l = 0; l < PL.NL; ++l) {
+    const bool sk = l < net->D && net->skip >= 0 && l == net->skip + 1;
+    if (l < net->D) { sj.src[l] = net->pts_w[l]; sj.rows[l] = 256; sj.cols[l] = l == 0 ? IC : (sk ? W + IC : W); }
+    else if (l == net->D) { sj.src[l] = net->feature_w; sj.rows[l] = 256; sj.cols[l] = W; }
+    else { sj.src[l] = net->views_w; sj.rows[l] = 128; sj.cols[l] = W; }
+    sj.ld[l] = (l == net->D + 1) ? W + net->input_ch_views : sj.cols[l];
+  }
+  split_scale_kernel<<<PL.NL, 256, 0, st>>>(sj, scale);
+  NB_LAUNCH_OK("split_scale_kernel");
+  PackSplitJob job;
+  memset(&job, 0, sizeof(job));
+  unsigned off = (unsigned)PL.off_chunks;
+  auto add = [&](int layer, const float* src, int ld, int k0, int kvalid, int nrows) {
+    job.layer[job.job.n] = (unsigned char)layer;
+    PackChunk& c = job.job.c[job.job.n++];
+    c.src = src; c.sn = ld; c.sk = 1; c.k0 = k0; c.kvalid = kvalid < 0 ? 0 : (kvalid > 32 ? 32 : kvalid); c.nrows = nrows; c.dst_off = off;
+    off += (unsigned)nrows * 128;                       // two stages of nrows x 64 B
+  };
+  for (int l = 0; l < PL.NL; ++l) {
+    if (l == 0) { add(0, net->pts_w[0], IC, 0, IC, 256); add(0, net->pts_w[0], IC, 32, IC - 32, 256); }
+    else if (l < net->D) {
+      const bool sk = (net->skip >= 0 && l == net->skip + 1);
+      const int ld = sk ? W + IC : W, base = sk ? IC : 0;
+      if (sk) { add(l, net->pts_w[l], ld, 0, IC, 256); add(l, net->pts_w[l], ld, 32, IC - 32, 256); }
+      for (int c = 0; c < 8; ++c) add(l, net->pts_w[l], ld, base + 32 * c, 32, 256);
+    } else if (l == net->D) { for (int c = 0; c < 8; ++c) add(l, net->feature_w, W, 32 * c, 32, 256); }
+    else { for (int c = 0; c < 8; ++c) add(l, net->views_w, W + net->input_ch_views, 32 * c, 32, 128); }
+  }
+  NB_CHECK_ARG(job.job.n == PL.n_chunks && off == PL.off_chunks + PL.chunk_bytes, "internal: split chunk table mismatch");
+  pack_chunks_split_kernel<<<dim3(8, job.job.n), 256, 0, st>>>(job, scale, dst);
+  NB_LAUNCH_OK("pack_chunks_split_kernel");
+  PackTables t;
+  t.net = *net; t.off_bias = PL.off_bias; t.off_heads = PL.off_heads; t.off_vdir = PL.off_vdir;
+  pack_tables_kernel<<<8, 256, 0, st>>>(t, dst);
+  NB_LAUNCH_OK("pack_tables_kernel");
+  return 0;
+}
+
 int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, int S, const NerfNetParams* net,
                           const void* packed, int multires, int multires_views, int precision, float* raw,
                           void* workspace, size_t workspace_bytes, void* stream) {
@@ -289,12 +364,12 @@ int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, in
     NB_LAUNCH_OK("mlp_simt_kernel");
     return 0;
   }
-  NB_CHECK_ARG(precision == NERF_B200_PREC_TC_FP16, "unknown precision %d", precision);
+  NB_CHECK_ARG(is_tc(precision), "unknown precision %d", precision);
   NerfPassOut out;
   memset(&out, 0, sizeof(out));
   out.raw = raw;
   return launch_march(nullptr, 0, nullptr, pts, viewdirs, 3, nullptr, N, S, net, packed, multires, multires_views, 0, 0,
-                      &out, workspace, workspace_bytes, nullptr, nullptr, st);
+                      &out, workspace, workspace_bytes, nullptr, nullptr, st, precision);
 }
 
 int nerf_b200_raw2outputs(const float* raw, const float* z_vals, const float* rays_d, int d_stride, const float* noise,
@@ -492,8 +567,10 @@ static int march_impl(const float* rays, const float* z_vals, const float* noise
     NB_LAUNCH_OK("raw2outputs_kernel");
     return 0;
   }
+  NB_CHECK_ARG(is_tc(cfg->precision), "unknown precision %d", cfg->precision);
   return launch_march(rays, cfg->ray_stride, z_vals, nullptr, rays + 8, cfg->ray_stride, noise, N, S, net, packed,
-                      cfg->multires, cfg->multires_views, cfg->white_bkgd, 1, out, workspace, workspace_bytes, save, vb_pre, st);
+                      cfg->multires, cfg->multires_views, cfg->white_bkgd, 1, out, workspace, workspace_bytes, save, vb_pre, st,
+                      cfg->precision);
 }
 
 int nerf_b200_march(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
@@ -506,6 +583,7 @@ int nerf_b200_march_train(const float* rays, const float* z_vals, const float* n
                           const void* packed, const NerfRenderCfg* cfg, const NerfPassOut* out, void* workspace,
                           size_t workspace_bytes, const NerfTrainSave* save, void* stream) {
   NB_CHECK_ARG(save != nullptr && out && out->raw, "training mode needs the save buffers and out->raw (the compositing adjoint reads raw)");
+  NB_CHECK_ARG(!cfg || cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
   return march_impl(rays, z_vals, noise, N, S, net, packed, cfg, out, workspace, workspace_bytes, save, stream);
 }
 
@@ -549,12 +627,12 @@ static int render_rays_fwd_impl(const float* rays, int64_t N, const NerfRenderCf
   const void* pf = net_fine ? packed_fine : packed_coarse;
   const float* vb_c = nullptr;
   const float* vb_f = nullptr;
-  if (cfg->precision == NERF_B200_PREC_TC_FP16 && net_coarse->use_viewdirs && packed_coarse && (Ni == 0 || (nf->use_viewdirs && pf))) {
+  if (is_tc(cfg->precision) && net_coarse->use_viewdirs && packed_coarse && (Ni == 0 || (nf->use_viewdirs && pf))) {
     if (int rc = check_tc_net(net_coarse)) return rc;
     NB_CHECK_ARG(workspace != nullptr && workspace_bytes >= (size_t)N * 128 * 4 * 2, "workspace too small: need %zu bytes", (size_t)N * 128 * 4 * 2);
     NB_CHECK_ARG(cfg->ray_stride >= 11, "ray_stride %d too small for view directions", cfg->ray_stride);
     NB_CHECK_ARG(3 + 6 * cfg->multires_views == net_coarse->input_ch_views || (cfg->multires_views == 0 && net_coarse->input_ch_views == 3), "multires_views mismatch");
-    const PackLayout PLc = make_pack_layout(*net_coarse);
+    const PackLayout PLc = pack_layout_for(*net_coarse, cfg->precision);
     RaySetupArgs a;
     memset(&a, 0, sizeof(a));
     a.rays = rays; a.ray_stride = cfg->ray_stride; a.N = N; a.Lv = cfg->multires_views; a.ICV = net_coarse->input_ch_views;
@@ -565,7 +643,7 @@ static int render_rays_fwd_impl(const float* rays, int64_t N, const NerfRenderCf
       if (nf == net_coarse || pf == packed_coarse) vb_f = vb_c;
       else {
         NB_CHECK_ARG(nf->input_ch_views == net_coarse->input_ch_views, "coarse and fine networks must encode view directions alike");
-        const PackLayout PLf = make_pack_layout(*nf);
+        const PackLayout PLf = pack_layout_for(*nf, cfg->precision);
         a.vdir_b = reinterpret_cast<const float*>(static_cast<const uint8_t*>(pf) + PLf.off_vdir); a.vb_b = vb + (size_t)N * 128;
         vb_f = a.vb_b;
       }
@@ -624,6 +702,7 @@ int nerf_b200_render_rays_fwd_train(const float* rays, int64_t N, const NerfRend
                                     const float* noise0, const float* noise1, float* z_coarse, const NerfPassOut* coarse,
                                     float* z_fine, float* z_std, const NerfPassOut* fine, void* workspace,
                                     size_t workspace_bytes, const NerfTrainSave* save_coarse, const NerfTrainSave* save_fine, void* stream) {
+  NB_CHECK_ARG(cfg && cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
   NB_CHECK_ARG(cfg && cfg->precision == NERF_B200_PREC_TC_FP16, "training-mode records belong to the tensor-core path");
   NB_CHECK_ARG(save_coarse && coarse && coarse->raw, "training mode needs save_coarse and coarse->raw");
   NB_CHECK_ARG(cfg->N_importance == 0 || (save_fine && fine && fine->raw), "training mode needs save_fine and fine->raw");
@@ -1115,6 +1194,7 @@ NerfOutGrads pass_seeds(const NerfBwdPass* q, const NerfOutGrads* g) { return g 
 
 int check_bwd_pass(const float* rays, const NerfBwdPass* q, const NerfRenderCfg* cfg, const NerfOutGrads* g) {
   NB_CHECK_ARG(rays && q && q->z_vals && q->net && q->packed && cfg && q->raw && q->save && q->grads, "NULL pointer");
+  NB_CHECK_ARG(cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
   NB_CHECK_ARG(!seeds_none(pass_seeds(q, g)), "no output gradient given for a backward pass (g_rgb / every NerfOutGrads member is NULL)");
   if (int rc = check_tc_net(q->net)) return rc;
   NB_CHECK_ARG(q->net->use_viewdirs || q->net->output_ch >= 4, "output_linear needs output_ch >= 4 (got %d)", q->net->output_ch);

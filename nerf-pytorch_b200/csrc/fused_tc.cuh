@@ -50,6 +50,16 @@ constexpr uint32_t FWD_MISC = FWD_BARS + 16 * FWD_NST;          // 228512: compo
 constexpr uint32_t FWD_ALLOC = FWD_MISC + 128;                  // 228640
 static_assert(FWD_ALLOC <= 227 * 1024, "the forward's shared-memory map exceeds the per-block limit");
 
+// The split-operand forward's map (march_split_kernel, precision TC_SPLIT): every operand is a hi and a lo fp16 image.  The lo
+// images of the A operands and encodings sit SPLIT_LO bytes above their hi images (same K-block layout), in the first 80 KB of
+// the forward's ring, and the ring keeps its last three stages.  A stage is one [N = 256 x K = 32] image as today (desc_w)
+// whose columns 0-15 are hi and 16-31 lo of the same 16 weight columns.  Heads, biases, raw rows, barriers and carry are the
+// forward's.
+constexpr int SPLIT_NST = 3;                                    // weight ring stages (16 KB each: K = 16, hi | lo)
+constexpr uint32_t SPLIT_LO = 81920;                            // hi image -> lo image (A operands and encodings)
+constexpr uint32_t SPLIT_WRING = SPLIT_LO + FWD_WRING;          // 163840: 3 x 16 KB weight ring
+static_assert(SPLIT_WRING + SPLIT_NST * TC_STAGE_BYTES == FWD_HEADS && SPLIT_NST <= FWD_NST, "the split map shares the forward's tail");
+
 // heads region (floats): viewdirs: alpha_w[256] rgb_w[3][128] alpha_b rgb_b[3]; else output_w[4][256] output_b[4]
 constexpr int HEADS_FLOATS = 1032;
 
@@ -63,6 +73,7 @@ struct PackLayout {
   // backward (dgrad) stream: transposed weight chunks (bwd_wg.cuh: bwd_stream_chunks); without view directions only the
   // pts-layer steps j >= 2
   size_t off_bwd, bwd_bytes;
+  size_t off_wscale;          // split image only: fp32 power-of-two weight scale per layer [TC_MAXD + 2]
 };
 
 __host__ __device__ inline int tc_layer_chunks(int l, int D, int skip) {
@@ -92,6 +103,23 @@ static inline PackLayout make_pack_layout(const NerfNetParams& n) {
   L.off_bwd = (L.off_bwd + 1023) & ~(size_t)1023;
   L.bwd_bytes = (size_t)(n.use_viewdirs ? 4 + 8 * n.D : 8 * (n.D - 1)) * TC_STAGE_BYTES;
   L.total = L.off_bwd + L.bwd_bytes;
+  L.off_wscale = 0;
+  return L;
+}
+
+// The split packed image (precision TC_SPLIT): each forward chunk becomes two ring stages (K = 16 each, hi | lo columns), the
+// fp32 tables follow as in the fp16 image, then the per-layer weight scales; no backward stream.
+static inline PackLayout make_pack_layout_split(const NerfNetParams& n) {
+  PackLayout L = make_pack_layout(n);
+  const size_t tables = L.off_bwd - L.off_bias;
+  L.chunk_bytes *= 2;
+  L.off_bias = L.off_chunks + L.chunk_bytes;
+  L.off_heads = L.off_bias + (size_t)(TC_MAXD + 1) * 1024;
+  L.off_vdir = L.off_heads + HEADS_FLOATS * 4;
+  L.off_wscale = L.off_bias + tables;
+  L.off_bwd = L.off_wscale + (TC_MAXD + 2) * 4;
+  L.bwd_bytes = 0;
+  L.total = L.off_bwd;
   return L;
 }
 
@@ -121,6 +149,57 @@ __global__ void pack_chunks_kernel(PackJob job, uint8_t* __restrict__ dst) {
   // SWIZZLE_64B K-major: 8-row atoms of 512 B, 16B-chunk index ^= (row%8)>>1
   unsigned off = c.dst_off + (row >> 3) * 512 + (row & 7) * 64 + ((c16 ^ ((row & 7) >> 1)) << 4);
   *reinterpret_cast<uint4*>(dst + off) = o;
+}
+
+// Split image: a power-of-two scale per layer puts the layer's largest |weight| in [2^13, 2^14), so that lo = w - hi of the
+// scaled weights stays a normal fp16 (22 significant bits in hi + lo) for every weight down to 2^-17 of the largest; unscaled,
+// lo of a weight of ~0.06 would be an fp16 subnormal.  The kernel scales the accumulator back exactly.  One block per layer.
+struct SplitScaleJob { const float* src[TC_MAXD + 2]; int rows[TC_MAXD + 2], cols[TC_MAXD + 2], ld[TC_MAXD + 2]; int n; };
+__global__ void __launch_bounds__(256) split_scale_kernel(SplitScaleJob job, float* __restrict__ scale) {
+  __shared__ float red[8];
+  const int l = blockIdx.x;
+  float m = 0.f;
+  for (int i = threadIdx.x; i < job.rows[l] * job.cols[l]; i += 256) m = fmaxf(m, fabsf(job.src[l][(size_t)(i / job.cols[l]) * job.ld[l] + i % job.cols[l]]));
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < 8; ++i) m = fmaxf(m, red[i]);
+    int e = 0;
+    frexpf(m, &e);                                     // m < 2^e
+    const int s = (m > 0.f && isfinite(m)) ? max(-60, min(60, 14 - e)) : 0;
+    scale[l] = ldexpf(1.0f, s);
+  }
+}
+
+// Split stages of forward chunks: chunk ci (PackJob's table, `layer[ci]` its layer) becomes two 16 KB stages at dst_off, stage
+// h holding weight columns k0 + 16 h .. + 15 of the scaled weights as hi (16-byte units 0, 1 of a row) and lo (units 2, 3).
+// One thread per 16-byte unit.
+struct PackSplitJob { PackJob job; unsigned char layer[PACK_MAX_CHUNKS]; };
+__global__ void pack_chunks_split_kernel(PackSplitJob sj, const float* __restrict__ scale, uint8_t* __restrict__ dst) {
+  const int ci = blockIdx.y;
+  if (ci >= sj.job.n) return;
+  const PackChunk c = sj.job.c[ci];
+  const int u = blockIdx.x * blockDim.x + threadIdx.x;  // unit index: (stage * nrows + row) * 4 + c16
+  if (u >= c.nrows * 8) return;
+  const int c16 = u & 3, row = (u >> 2) % c.nrows, h = (u >> 2) / c.nrows;
+  const float sc = scale[sj.layer[ci]];
+  uint32_t o[4];
+#pragma unroll
+  for (int j = 0; j < 8; j += 2) {
+    float v[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int k = 16 * h + 8 * (c16 & 1) + j + e;
+      const float w = (k < c.kvalid) ? c.src[(size_t)row * c.sn + (size_t)(c.k0 + k) * c.sk] * sc : 0.0f;
+      const float hi = __half2float(__float2half_rn(w));
+      v[e] = (c16 >> 1) ? w - hi : hi;
+    }
+    o[j >> 1] = ptx::cvt_f16x2(v[0], v[1]);
+  }
+  // SWIZZLE_64B K-major, as pack_chunks_kernel
+  const unsigned off = c.dst_off + (unsigned)h * (unsigned)c.nrows * 64u + (row >> 3) * 512 + (row & 7) * 64 + ((c16 ^ ((row & 7) >> 1)) << 4);
+  *reinterpret_cast<uint4*>(dst + off) = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
 struct PackTables { NerfNetParams net; size_t off_bias, off_heads, off_vdir; };
@@ -350,6 +429,46 @@ __device__ __forceinline__ void encode_row_store(uint32_t row, int tr_, float px
   for (int k = 0; k < 8; ++k) {
     const uint32_t a = row + (uint32_t)((k ^ (tr_ & 7)) << 4);
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(h[4 * k]), "r"(h[4 * k + 1]), "r"(h[4 * k + 2]), "r"(h[4 * k + 3]) : "memory");
+  }
+}
+
+// The split forward's encoding row: the same 64 channels, each evaluated in fp32 with one sinf / cosf per octave (as
+// mlp_simt_kernel) and stored as its hi and lo fp16 halves into the two images' rows.
+__device__ __forceinline__ void encode_row_store_split(uint32_t row_hi, uint32_t row_lo, int tr_, float px, float py, float pz, int L) {
+  uint32_t hh[32], hl[32];
+  const float q[3] = {px, py, pz};
+  float carry = 0.f;
+  int n = 0;
+  auto emit = [&](float v) {
+    if (n & 1) {
+      const uint32_t hi = ptx::cvt_f16x2(carry, v);
+      const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+      hh[n >> 1] = hi;
+      hl[n >> 1] = ptx::cvt_f16x2(carry - hf.x, v - hf.y);
+    } else carry = v;
+    ++n;
+  };
+  emit(px); emit(py); emit(pz);
+#pragma unroll
+  for (int f = 0; f < 10; ++f) {
+    const bool on = f < L;
+    float s[3], c[3];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const float a = __fmul_rn(q[j], exp2f((float)f));
+      s[j] = on ? sinf(a) : 0.f; c[j] = on ? cosf(a) : 0.f;
+    }
+#pragma unroll
+    for (int j = 0; j < 3; ++j) emit(s[j]);
+#pragma unroll
+    for (int j = 0; j < 3; ++j) emit(c[j]);
+  }
+  emit(0.f);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const uint32_t o = (uint32_t)((k ^ (tr_ & 7)) << 4);
+    ptx::st_shared_v4(row_hi + o, hh[4 * k], hh[4 * k + 1], hh[4 * k + 2], hh[4 * k + 3]);
+    ptx::st_shared_v4(row_lo + o, hl[4 * k], hl[4 * k + 1], hl[4 * k + 2], hl[4 * k + 3]);
   }
 }
 

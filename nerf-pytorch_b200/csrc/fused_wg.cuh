@@ -115,6 +115,43 @@ __device__ __forceinline__ void mma_layer(float (&acc)[R], Ring& rg, uint32_t ri
   mma_layer(acc, rg, ring_base, nch, from_zero, a_of, none);
 }
 
+// The split forward's layer: stage c holds K = 16 columns of chunk c >> 1 (hi | lo), `a_of(c >> 1)` gives the chunk's hi A
+// descriptor and the lo image is SPLIT_LO above it.  Three MMAs per stage into the one accumulator: hi_a hi_b, hi_a lo_b, lo_a hi_b.
+template <int R, typename RG, typename AOf>
+__device__ __forceinline__ void mma_layer_split(float (&acc)[R], RG& rg, uint32_t ring_base, int nst, bool from_zero, AOf a_of, Phases& ph) {
+  ptx::wgmma_fence();
+  int pending = -1;
+  for (int c = 0; c < nst; ++c) {
+    const uint32_t s = rg.stage;
+    ph.wait_full(rg.full + 8 * s, rg.phase);
+    const uint64_t ah = a_of(c >> 1) + (uint64_t)(2 * (c & 1)), al = ah + (SPLIT_LO >> 4);
+    const uint64_t bd = desc_w(ring_base + s * TC_STAGE_BYTES);
+    if constexpr (R == 128) {
+      ptx::wgmma_m64n256k16<0, 0>(acc, ah, bd, (from_zero && c == 0) ? 0u : 1u);
+      ptx::wgmma_m64n256k16<0, 0>(acc, ah, bd + 2, 1u);
+      ptx::wgmma_m64n256k16<0, 0>(acc, al, bd, 1u);
+    } else {
+      ptx::wgmma_m64n128k16<0, 0>(acc, ah, bd, (from_zero && c == 0) ? 0u : 1u);
+      ptx::wgmma_m64n128k16<0, 0>(acc, ah, bd + 2, 1u);
+      ptx::wgmma_m64n128k16<0, 0>(acc, al, bd, 1u);
+    }
+    ptx::wgmma_commit();
+    if (pending >= 0) { ptx::wgmma_wait<1>(); ptx::mbar_arrive(rg.empty + 8 * pending); }
+    pending = (int)s;
+    rg.advance();
+  }
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(acc);
+  if (pending >= 0) ptx::mbar_arrive(rg.empty + 8 * pending);
+}
+
+// {hi, lo} fp16 pairs of (a, b): hi = fp16(x), lo = fp16(x - hi), x - hi exact in fp32
+__device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  hi = ptx::cvt_f16x2(a, b);
+  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  lo = ptx::cvt_f16x2(a - hf.x, b - hf.y);
+}
+
 // OR of a value over the four lanes that share an accumulator row
 __device__ __forceinline__ uint32_t quad_or(uint32_t v) {
   v |= __shfl_xor_sync(0xffffffffu, v, 1);
@@ -125,8 +162,14 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-template <bool EMIT>
-__global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchParams p, const TrainSaveDev sv) {
+// The pass of march_wg_kernel (SPLIT false) and march_split_kernel (SPLIT true, never EMIT).  SPLIT: every MMA operand is a hi
+// and a lo fp16 image (the split map of fused_tc.cuh), each weight chunk streams as two ring stages, the weights are scaled by
+// wscale[l] (a power of two: the accumulator starts at bias * wscale[l] and is scaled back exactly after the MMAs).
+template <bool EMIT, bool SPLIT>
+__device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveDev sv, const float* wscale) {
+  static_assert(!(EMIT && SPLIT), "the split forward has no training mode");
+  constexpr int NST = SPLIT ? SPLIT_NST : FWD_NST;
+  constexpr int CPS = SPLIT ? 2 : 1;                              // ring stages per weight chunk
   uint8_t* smem = tc_smem;
   const uint32_t sb = ptx::smem_u32(smem);
   if ((sb & 1023u) != 0) __trap();
@@ -143,9 +186,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
 
   for (int i = threadIdx.x; i < HEADS_FLOATS; i += TC_THREADS) s_heads[i] = p.heads[i];
   for (int i = threadIdx.x; i < (TC_MAXD + 1) * 256; i += TC_THREADS) s_bias[i] = p.bias[i];
-  RingN<FWD_NST> rg{sb + FWD_BARS, sb + FWD_BARS + 8 * FWD_NST, 0, 0};
+  RingN<NST> rg{sb + FWD_BARS, sb + FWD_BARS + 8 * NST, 0, 0};
   if (threadIdx.x == 0) {
-    for (int i = 0; i < FWD_NST; ++i) { ptx::mbar_init(rg.full + 8 * i, 1); ptx::mbar_init(rg.empty + 8 * i, 256); }
+    for (int i = 0; i < NST; ++i) { ptx::mbar_init(rg.full + 8 * i, 1); ptx::mbar_init(rg.empty + 8 * i, 256); }
     sts32(a_carry + CARRY_T, 1.0f); sts32(a_carry + CARRY_R, 0.f); sts32(a_carry + CARRY_G, 0.f); sts32(a_carry + CARRY_B, 0.f);
     sts32(a_carry + CARRY_D, 0.f); sts32(a_carry + CARRY_A, 0.f); st_release_shared(a_carry + CARRY_TURN, 0u);
     ptx::fence_mbar_init();
@@ -159,12 +202,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
       for (int tile = 0; tile < 2 * nst; ++tile) {
         const uint8_t* src = p.chunks;
         for (int l = 0; l < NL; ++l) {
-          const int nch = tc_layer_chunks(l, D, p.skip);
+          const int nch = tc_layer_chunks(l, D, p.skip) * CPS;
           const uint32_t bytes = tc_layer_chunk_bytes(l, D);
           for (int c = 0; c < nch; ++c) {
             ptx::mbar_wait(rg.empty + 8 * rg.stage, rg.phase ^ 1);
             ptx::mbar_arrive_expect_tx(rg.full + 8 * rg.stage, bytes);
-            ptx::bulk_g2s(sb + FWD_WRING + rg.stage * TC_STAGE_BYTES, src, bytes, rg.full + 8 * rg.stage);
+            ptx::bulk_g2s(sb + (SPLIT ? SPLIT_WRING : FWD_WRING) + rg.stage * TC_STAGE_BYTES, src, bytes, rg.full + 8 * rg.stage);
             src += bytes;
             rg.advance();
           }
@@ -180,7 +223,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
   const int q4 = lane & 3;
   const int r0 = 16 * wq + (lane >> 2), r1 = r0 + 8;              // this thread's two accumulator rows (of the warpgroup's 64)
   const uint32_t act = sb + SM_ACT + (uint32_t)w * 32768u, enc = sb + FWD_ENC + (uint32_t)w * 8192u;
-  const uint32_t ring = sb + FWD_WRING;
+  const uint32_t ring = sb + (SPLIT ? SPLIT_WRING : FWD_WRING);
   const uint64_t l2_first = EMIT ? ptx::l2_policy_evict_first() : 0ull;
   auto wg_sync = [&]() { ptx::named_bar_sync(1 + w, 128); };
   // row-dependent parts of the swizzled addresses of this thread's pairs: column pair (8 j + 2 q4) of row r sits at
@@ -227,7 +270,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
           pz = __fadd_rn(ry[2], __fmul_rn(ry[5], z));
         }
       }
-      encode_row_store(enc + act_row_off(t), t, px, py, pz, p.L);
+      if constexpr (SPLIT) encode_row_store_split(enc + act_row_off(t), enc + SPLIT_LO + act_row_off(t), t, px, py, pz, p.L);
+      else encode_row_store(enc + act_row_off(t), t, px, py, pz, p.L);
     }
     ptx::fence_proxy_async_smem();
     wg_sync();
@@ -246,13 +290,26 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
       if (l <= D) {
         // ---- pts_linears[l] (ReLU) or feature_linear (no activation): 64 x 256 ----
         const float* bias = s_bias + 256 * l;
+        if constexpr (SPLIT) {
+          const float sc = wscale[l], isc = 1.0f / sc;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
-          acc[4 * j] = b.x; acc[4 * j + 1] = b.y; acc[4 * j + 2] = b.x; acc[4 * j + 3] = b.y;
+          for (int j = 0; j < 32; ++j) {
+            const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
+            acc[4 * j] = b.x * sc; acc[4 * j + 1] = b.y * sc; acc[4 * j + 2] = b.x * sc; acc[4 * j + 3] = b.y * sc;
+          }
+          if (l > 0) ph.stop(PH_GAP);
+          mma_layer_split(acc, rg, ring, nch * 2, false, a_of, ph);
+#pragma unroll
+          for (int i = 0; i < 128; ++i) acc[i] *= isc;
+        } else {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
+            acc[4 * j] = b.x; acc[4 * j + 1] = b.y; acc[4 * j + 2] = b.x; acc[4 * j + 3] = b.y;
+          }
+          if (l > 0) ph.stop(PH_GAP);
+          mma_layer(acc, rg, ring, nch, false, a_of, ph);
         }
-        if (l > 0) ph.stop(PH_GAP);
-        mma_layer(acc, rg, ring, nch, false, a_of, ph);
         ph.start();
         if (EMIT && t == 0) ptx::bulk_wait_read0();
         wg_sync();                                                // the whole warpgroup's MMAs and copies are done with the operand
@@ -309,11 +366,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
 #pragma unroll
           for (int j = 0; j < 32; j += 2) {
             uint32_t h[4];
+            if constexpr (SPLIT) {
+              uint32_t lo[4];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int g = j + e;
+                const float x0 = relu ? fmaxf(acc[4 * g], 0.f) : acc[4 * g], x1 = relu ? fmaxf(acc[4 * g + 1], 0.f) : acc[4 * g + 1];
+                const float y0 = relu ? fmaxf(acc[4 * g + 2], 0.f) : acc[4 * g + 2], y1 = relu ? fmaxf(acc[4 * g + 3], 0.f) : acc[4 * g + 3];
+                split_f16x2(x0, x1, h[2 * e], lo[2 * e]);
+                split_f16x2(y0, y1, h[2 * e + 1], lo[2 * e + 1]);
+              }
+              ptx::stmatrix_x4(sm_row + SPLIT_LO + (uint32_t)(j >> 3) * 8192u + ((uint32_t)((j & 7) ^ sm_key) << 4), lo[0], lo[1], lo[2], lo[3]);
+            } else {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int g = j + e;
               h[2 * e] = relu ? ptx::cvt_relu_f16x2(acc[4 * g], acc[4 * g + 1]) : ptx::cvt_f16x2(acc[4 * g], acc[4 * g + 1]);
               h[2 * e + 1] = relu ? ptx::cvt_relu_f16x2(acc[4 * g + 2], acc[4 * g + 3]) : ptx::cvt_f16x2(acc[4 * g + 2], acc[4 * g + 3]);
+            }
             }
             ptx::stmatrix_x4(sm_row + (uint32_t)(j >> 3) * 8192u + ((uint32_t)((j & 7) ^ sm_key) << 4), h[0], h[1], h[2], h[3]);
           }
@@ -327,8 +397,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
       } else {
         // ---- views_linears[0] (N = 128) + per-ray view bias, ReLU, rgb_linear ----
         float* accv = acc;                                        // the first 64 accumulators
-        ph.stop(PH_GAP);
-        mma_layer(*reinterpret_cast<float(*)[64]>(accv), rg, ring, nch, true, a_of, ph);
+        if constexpr (SPLIT) {
+          const float isc = 1.0f / wscale[l];
+          ph.stop(PH_GAP);
+          mma_layer_split(*reinterpret_cast<float(*)[64]>(accv), rg, ring, nch * 2, true, a_of, ph);
+#pragma unroll
+          for (int i = 0; i < 64; ++i) acc[i] *= isc;
+        } else {
+          ph.stop(PH_GAP);
+          mma_layer(*reinterpret_cast<float(*)[64]>(accv), rg, ring, nch, true, a_of, ph);
+        }
         ph.start();
         wg_sync();
         const float* vb0 = p.vb + nray[0] * 128;
@@ -405,6 +483,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
   }
   if (EMIT && t == 0) ptx::bulk_wait_all();
   ph.flush(w, t);
+}
+
+template <bool EMIT>
+__global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchParams p, const TrainSaveDev sv) {
+  march_pass<EMIT, false>(p, sv, nullptr);
+}
+
+// precision TC_SPLIT: fp32-class results from three fp16 MMAs per K-step (inference only; wscale: the split image's scales)
+__global__ void __launch_bounds__(TC_THREADS, 1) march_split_kernel(const MarchParams p, const float* __restrict__ wscale) {
+  march_pass<false, true>(p, TrainSaveDev{}, wscale);
 }
 
 }  // namespace nb
