@@ -102,6 +102,29 @@ int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, in
                           int multires_views, int precision, float* raw,
                           void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- mesh extraction: density on a grid, marching cubes ---------------------------------------- */
+/* sigma [nx,ny,nz] (C order, k fastest) = raw[..., 3] of nerf_b200_run_network on the points       */
+/* (xs[i], ys[j], zs[k]) with zero view directions, bit for bit, in every precision: the            */
+/* pre-ReLU density, no noise.  The tensor-core precisions run the fused pass's pts layers and       */
+/* sigma head only (no workspace); FP32 runs the exact path slab by slab in the workspace.           */
+/* The net is checked as nerf_b200_run_network checks it, with the same messages.                   */
+size_t nerf_b200_density_grid_workspace_bytes(int nx, int ny, int nz, const NerfNetParams* net, int precision);
+int nerf_b200_density_grid(const float* xs, int nx, const float* ys, int ny, const float* zs, int nz,
+                           const NerfNetParams* net, const void* packed, int multires, int precision,
+                           float* sigma, void* workspace, size_t workspace_bytes, void* stream);
+/* Marching cubes on sigma [nx,ny,nz] at `iso` (inside: sigma > iso; NaN is outside), nx,ny,nz >= 2:  */
+/* _count writes (V, F) to the device int64 counts[2] and leaves the scans in the workspace; _emit    */
+/* (same sigma, grid, iso and workspace) writes verts [V,3] (world coordinates from xs/ys/zs) and     */
+/* faces [F,3] (vertex ids, normals toward decreasing density).  _emit reads (V, F) back from the     */
+/* workspace to check the capacities, which synchronises the stream.  No atomics: deterministic.      */
+size_t nerf_b200_marching_cubes_workspace_bytes(int nx, int ny, int nz);
+int nerf_b200_marching_cubes_count(const float* sigma, int nx, int ny, int nz, float iso, int64_t* counts,
+                                   void* workspace, size_t workspace_bytes, void* stream);
+int nerf_b200_marching_cubes_emit(const float* sigma, const float* xs, const float* ys, const float* zs,
+                                  int nx, int ny, int nz, float iso, float* verts, int64_t max_verts,
+                                  int32_t* faces, int64_t max_faces, void* workspace, size_t workspace_bytes,
+                                  void* stream);
+
 /* ---- raw2outputs (run_nerf.py:262-305) and its adjoint (SURVEY App. E) ------------------------ */
 /* raw [N,S,4], z_vals [N,S], rays_d row pointer with stride `d_stride` floats, noise [N,S]|NULL.  */
 int nerf_b200_raw2outputs(const float* raw, const float* z_vals, const float* rays_d, int d_stride,

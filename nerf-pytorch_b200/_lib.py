@@ -78,6 +78,13 @@ SIGNATURES = {
     "nerf_b200_pack_weights_split": (C.c_int, [C.POINTER(NerfNetParams), c_fp, C.c_size_t, c_fp]),
     "nerf_b200_run_network": (C.c_int, [c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp, C.c_int,
                                         C.c_int, C.c_int, c_fp, c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_density_grid_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.POINTER(NerfNetParams), C.c_int]),
+    "nerf_b200_density_grid": (C.c_int, [c_fp, C.c_int, c_fp, C.c_int, c_fp, C.c_int, C.POINTER(NerfNetParams), c_fp, C.c_int,
+                                         C.c_int, c_fp, c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_marching_cubes_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "nerf_b200_marching_cubes_count": (C.c_int, [c_fp, C.c_int, C.c_int, C.c_int, C.c_float, c_fp, c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_marching_cubes_emit": (C.c_int, [c_fp, c_fp, c_fp, c_fp, C.c_int, C.c_int, C.c_int, C.c_float, c_fp, C.c_int64,
+                                                c_fp, C.c_int64, c_fp, C.c_size_t, c_fp]),
     "nerf_b200_raw2outputs": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, c_fp, C.c_int64, C.c_int, C.c_int,
                                         C.POINTER(NerfPassOut), c_fp]),
     "nerf_b200_raw2outputs_bwd": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, c_fp, C.c_int64, C.c_int, C.c_int, c_fp, c_fp, c_fp]),

@@ -29,7 +29,8 @@ from ._lib import (NerfCamera, NerfNetGrads, NerfNetParams, NerfPassOut, NerfRen
 __all__ = ["NeRF", "Embedder", "get_embedder", "sample_pdf", "raw2outputs", "run_network", "batchify",
            "batchify_rays", "render_rays", "render", "create_nerf",
            "img2mse", "mse2psnr", "to8b", "set_precision", "get_precision", "set_backward", "get_backward",
-           "launch_count", "DEBUG", "GraphedRender", "render_to8b", "DeviceRayBatcher"]
+           "launch_count", "DEBUG", "GraphedRender", "render_to8b", "DeviceRayBatcher", "density_grid", "marching_cubes",
+           "extract_mesh", "save_ply"]
 
 DEBUG = False
 _PRECISION = {"mode": PREC_TC_FP16}
@@ -1174,3 +1175,91 @@ class GraphedRender:
         out.copy_(self.packed_out, non_blocking=True)
         torch.cuda.current_stream(self.rays.device).synchronize()
         return out
+
+
+# ------------------------------------------------------------------------------------------------
+# mesh extraction: the density over a grid and marching cubes on it
+# ------------------------------------------------------------------------------------------------
+
+def _axis(a, what, dev=None):
+    a = _f32c(torch.as_tensor(a, device=dev) if not torch.is_tensor(a) else a, what).reshape(-1)
+    if dev is not None and a.device != dev:
+        raise RuntimeError(f"nerf_b200: {what} is on {a.device}, expected {dev}")
+    return a
+
+
+@torch.no_grad()
+def density_grid(network_fn, network_query_fn, xs, ys, zs):
+    """sigma [nx, ny, nz] (float32, on xs' device) of `network_fn` at the points (xs[i], ys[j], zs[k]), in the current
+    set_precision: bit for bit run_network(torch.meshgrid(xs, ys, zs, indexing='ij'), zero viewdirs)[..., 3], the pre-ReLU
+    density without noise, but without materialising the points or evaluating the view layers.  `multires` is read from
+    `network_query_fn` as render_rays reads it."""
+    if not isinstance(network_fn, NeRF):
+        raise RuntimeError("nerf_b200.density_grid: network must be a nerf_b200.NeRF")
+    xs = _axis(xs, "xs")
+    ys, zs = _axis(ys, "ys", xs.device), _axis(zs, "zs", xs.device)
+    mr = getattr(network_query_fn, "multires", None)
+    if mr is None:
+        mr = (network_fn.input_ch - 3) // 6
+    nx, ny, nz = xs.numel(), ys.numel(), zs.numel()
+    lib = _lib.load()
+    n = network_fn.net_params()
+    prec = _PRECISION["mode"]
+    packed = _packed_for(network_fn, prec)
+    sigma = torch.empty((nx, ny, nz), device=xs.device, dtype=torch.float32)
+    ws_bytes = lib.nerf_b200_density_grid_workspace_bytes(nx, ny, nz, C.byref(n), prec)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=xs.device)
+    with _on(xs):
+        check(lib.nerf_b200_density_grid(_ptr(xs), nx, _ptr(ys), ny, _ptr(zs), nz, C.byref(n), _ptr(packed), int(mr), prec,
+                                         _ptr(sigma), _ptr(ws), ws_bytes, _stream(xs)), "density_grid")
+    return sigma
+
+
+@torch.no_grad()
+def marching_cubes(sigma, xs, ys, zs, iso):
+    """Marching cubes of sigma [nx, ny, nz] at `iso` on the grid xs, ys, zs -> (verts [V, 3] float32, faces [F, 3] int64), on the
+    device.  Inside is sigma > iso (NaN is outside); one vertex per grid edge that crosses the level, shared by its cells; face
+    normals point toward decreasing density.  Deterministic; synchronises once to size the outputs."""
+    sigma = _f32c(sigma, "sigma")
+    if sigma.dim() != 3:
+        raise RuntimeError(f"nerf_b200.marching_cubes: sigma must be [nx, ny, nz] (got shape {tuple(sigma.shape)})")
+    dev = sigma.device
+    xs, ys, zs = _axis(xs, "xs", dev), _axis(ys, "ys", dev), _axis(zs, "zs", dev)
+    nx, ny, nz = sigma.shape
+    if (xs.numel(), ys.numel(), zs.numel()) != (nx, ny, nz):
+        raise RuntimeError(f"nerf_b200.marching_cubes: axes of {xs.numel()}, {ys.numel()}, {zs.numel()} points for sigma {tuple(sigma.shape)}")
+    lib = _lib.load()
+    ws_bytes = lib.nerf_b200_marching_cubes_workspace_bytes(nx, ny, nz)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    st = _stream(sigma)
+    with _on(sigma):
+        check(lib.nerf_b200_marching_cubes_count(_ptr(sigma), nx, ny, nz, float(iso), _ptr(counts), _ptr(ws), ws_bytes, st),
+              "marching_cubes_count")
+        V, F = (int(v) for v in counts.tolist())
+        verts = torch.empty((V, 3), device=dev, dtype=torch.float32)
+        faces = torch.empty((F, 3), device=dev, dtype=torch.int32)
+        check(lib.nerf_b200_marching_cubes_emit(_ptr(sigma), _ptr(xs), _ptr(ys), _ptr(zs), nx, ny, nz, float(iso), _ptr(verts), V,
+                                                _ptr(faces), F, _ptr(ws), ws_bytes, st), "marching_cubes_emit")
+    return verts, faces.long()
+
+
+def extract_mesh(network_fn, network_query_fn, xs, ys, zs, iso):
+    """The mesh of `network_fn`'s density at level `iso` on the grid xs, ys, zs: density_grid, then marching_cubes.  Usually
+    network_fn = render_kwargs_test['network_fine']."""
+    return marching_cubes(density_grid(network_fn, network_query_fn, xs, ys, zs), xs, ys, zs, iso)
+
+
+def save_ply(path, verts, faces):
+    """Write a triangle mesh (verts [V, 3], faces [F, 3]; tensors or arrays) as binary little-endian PLY."""
+    v = np.ascontiguousarray(verts.detach().cpu().numpy() if torch.is_tensor(verts) else verts, dtype="<f4").reshape(-1, 3)
+    f = np.asarray(faces.detach().cpu().numpy() if torch.is_tensor(faces) else faces).reshape(-1, 3)
+    rec = np.empty(len(f), dtype=[("n", "u1"), ("idx", "<i4", (3,))])
+    rec["n"] = 3
+    rec["idx"] = f
+    header = (f"ply\nformat binary_little_endian 1.0\nelement vertex {len(v)}\nproperty float x\nproperty float y\n"
+              f"property float z\nelement face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(v.tobytes())
+        fh.write(rec.tobytes())

@@ -8,6 +8,7 @@
 #include "fused_wg.cuh"
 #include "bwd_wg.cuh"
 #include "train_step.cuh"
+#include "mesh.cuh"
 #include <stdlib.h>
 
 namespace nb {
@@ -370,6 +371,153 @@ int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, in
   out.raw = raw;
   return launch_march(nullptr, 0, nullptr, pts, viewdirs, 3, nullptr, N, S, net, packed, multires, multires_views, 0, 0,
                       &out, workspace, workspace_bytes, nullptr, nullptr, st, precision);
+}
+
+// ---- mesh extraction ----------------------------------------------------------------------------------------------------
+// precision FP32 evaluates the grid in slabs of DENSITY_SLAB points: the points, then mlp_simt_kernel into raw rows, then their
+// sigma column.  Workspace: 256 B (the zero view direction every row reads, dir_stride 0) | pts [slab, 3] | raw [slab, 4].
+static const long long DENSITY_SLAB = 1ll << 20;
+static size_t density_pts_floats(long long slab) { return ((size_t)slab * 3 + 3) & ~(size_t)3; }
+
+size_t nerf_b200_density_grid_workspace_bytes(int nx, int ny, int nz, const NerfNetParams* net, int precision) {
+  if (nx < 1 || ny < 1 || nz < 1) return 0;
+  if (precision == NERF_B200_PREC_FP32) {
+    if (check_exact_net(net)) return 0;
+    const long long P = (long long)nx * ny * nz, slab = P < DENSITY_SLAB ? P : DENSITY_SLAB;
+    return 256 + density_pts_floats(slab) * 4 + (size_t)slab * 16;
+  }
+  if (!is_tc(precision) || check_tc_net(net)) return 0;
+  return 256;                                          // the tensor-core pass needs none
+}
+
+int nerf_b200_density_grid(const float* xs, int nx, const float* ys, int ny, const float* zs, int nz,
+                           const NerfNetParams* net, const void* packed, int multires, int precision,
+                           float* sigma, void* workspace, size_t workspace_bytes, void* stream) {
+  NB_CHECK_ARG(xs && ys && zs && sigma && net, "NULL pointer");
+  NB_CHECK_ARG(nx >= 1 && ny >= 1 && nz >= 1, "empty grid (nx=%d ny=%d nz=%d)", nx, ny, nz);
+  NB_CHECK_ARG(precision == NERF_B200_PREC_FP32 || is_tc(precision), "unknown precision %d", precision);
+  if (precision == NERF_B200_PREC_FP32) { if (int rc = check_exact_net(net)) return rc; }
+  else if (int rc = check_tc_net(net)) return rc;
+  NB_CHECK_ARG(3 + 6 * multires == net->input_ch || (multires == 0 && net->input_ch == 3), "multires %d does not match input_ch %d",
+               multires, net->input_ch);
+  const long long N = (long long)nx * ny, P = N * nz;
+  NB_CHECK_ARG(P < (1ll << 40), "grid too large");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (precision == NERF_B200_PREC_FP32) {
+    const size_t need = nerf_b200_density_grid_workspace_bytes(nx, ny, nz, net, precision);
+    NB_CHECK_ARG(workspace && workspace_bytes >= need, "workspace too small: need %zu bytes", need);
+    uint8_t* ws = static_cast<uint8_t*>(workspace);
+    const float* zero_dir = reinterpret_cast<const float*>(ws);
+    float* pts = reinterpret_cast<float*>(ws + 256);
+    const long long slab = P < DENSITY_SLAB ? P : DENSITY_SLAB;
+    float* raw = pts + density_pts_floats(slab);
+    NB_CUDA(cudaMemsetAsync(ws, 0, 256, st));
+    const size_t sm = simt_smem_bytes(*net);
+    if (int rc = smem_optin((const void*)mlp_simt_kernel, sm)) return rc;
+    for (long long m0 = 0; m0 < P; m0 += slab) {
+      const long long M = P - m0 < slab ? P - m0 : slab;
+      grid_pts_kernel<<<cdiv(M, 256), 256, 0, st>>>(xs, ys, zs, ny, nz, m0, M, pts);
+      NB_LAUNCH_OK("grid_pts_kernel");
+      mlp_simt_kernel<<<cdiv(M, SIMT_ROWS), SIMT_THREADS, sm, st>>>(pts, zero_dir, 0, M, 1, *net, multires, 0, raw, SimtSave{});
+      NB_LAUNCH_OK("mlp_simt_kernel");
+      raw_sigma_kernel<<<cdiv(M, 256), 256, 0, st>>>(raw, M, sigma + m0);
+      NB_LAUNCH_OK("raw_sigma_kernel");
+    }
+    return 0;
+  }
+  const bool split = precision == NERF_B200_PREC_TC_SPLIT;
+  NB_CHECK_ARG(packed != nullptr, split ? "packed weights are NULL (call nerf_b200_pack_weights_split)" : "packed weights are NULL (call nerf_b200_pack_weights)");
+  DeviceState* ds = device_state();
+  const TilePlan plan = make_tile_plan(N, nz, ds->sms);
+  NB_CHECK_ARG((long long)plan.rays_per_cta * nz < (1ll << 30), "rays_per_cta * S overflows");
+  const PackLayout PL = pack_layout_for(*net, precision);
+  const uint8_t* pk = static_cast<const uint8_t*>(packed);
+  MarchParams p;
+  memset(&p, 0, sizeof(p));
+  p.N = N; p.S = nz; p.rays_per_cta = plan.rays_per_cta;
+  p.chunks = pk + PL.off_chunks;
+  p.bias = reinterpret_cast<const float*>(pk + PL.off_bias);
+  p.heads = reinterpret_cast<const float*>(pk + PL.off_heads);
+  p.D = net->D; p.skip = net->skip; p.use_viewdirs = net->use_viewdirs; p.L = multires; p.IC = net->input_ch;
+  const DensityGrid g{xs, ys, zs, ny, sigma};
+  if (split) {
+    if (int rc = smem_optin((const void*)density_split_kernel, FWD_ALLOC)) return rc;
+    density_split_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, g, reinterpret_cast<const float*>(pk + PL.off_wscale));
+    NB_LAUNCH_OK("density_split_kernel");
+  } else {
+    if (int rc = smem_optin((const void*)density_wg_kernel, FWD_ALLOC)) return rc;
+    density_wg_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, g);
+    NB_LAUNCH_OK("density_wg_kernel");
+  }
+  return 0;
+}
+
+// workspace of marching cubes: McHeader (256 B) | per-point (vertex, face) counts, then offsets [P] | tile sums [P / 4096]
+static long long mc_tiles(long long P) { return (P + MC_SCAN_TILE - 1) / MC_SCAN_TILE; }
+static size_t mc_need(int nx, int ny, int nz) {
+  const long long P = (long long)nx * ny * nz;
+  return MC_HEADER_BYTES + (size_t)P * sizeof(int2) + (size_t)mc_tiles(P) * sizeof(int2);
+}
+// ids and offsets are 32-bit: at most 3 vertices per point and 5 faces per cell
+static int check_mc_grid(int nx, int ny, int nz) {
+  NB_CHECK_ARG(nx >= 2 && ny >= 2 && nz >= 2, "marching cubes needs nx, ny, nz >= 2 (got %d, %d, %d)", nx, ny, nz);
+  const long long P = (long long)nx * ny * nz, Cl = (long long)(nx - 1) * (ny - 1) * (nz - 1);
+  NB_CHECK_ARG(3 * P < (1ll << 31) && 5 * Cl < (1ll << 31), "grid of %lld points too large for 32-bit vertex ids", P);
+  return 0;
+}
+
+size_t nerf_b200_marching_cubes_workspace_bytes(int nx, int ny, int nz) {
+  if (check_mc_grid(nx, ny, nz)) return 0;
+  return mc_need(nx, ny, nz);
+}
+
+int nerf_b200_marching_cubes_count(const float* sigma, int nx, int ny, int nz, float iso, int64_t* counts,
+                                   void* workspace, size_t workspace_bytes, void* stream) {
+  if (int rc = check_mc_grid(nx, ny, nz)) return rc;
+  NB_CHECK_ARG(sigma && counts && workspace, "NULL pointer");
+  const size_t need = mc_need(nx, ny, nz);
+  NB_CHECK_ARG(workspace_bytes >= need, "workspace too small: need %zu bytes", need);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const long long P = (long long)nx * ny * nz, nt = mc_tiles(P);
+  int2* cnt = reinterpret_cast<int2*>(ws + MC_HEADER_BYTES);
+  int2* tsum = cnt + P;
+  mc_count_kernel<<<cdiv(P, 256), 256, 0, st>>>(sigma, nx, ny, nz, iso, cnt);
+  NB_LAUNCH_OK("mc_count_kernel");
+  mc_scan_tiles_kernel<<<(int)nt, MC_SCAN_THREADS, 0, st>>>(cnt, P, tsum);
+  NB_LAUNCH_OK("mc_scan_tiles_kernel");
+  McHeader h;
+  memset(&h, 0, sizeof(h));
+  h.nx = nx; h.ny = ny; h.nz = nz; h.iso = iso;
+  mc_scan_sums_kernel<<<1, MC_SCAN_THREADS, 0, st>>>(tsum, (int)nt, reinterpret_cast<long long*>(counts), reinterpret_cast<McHeader*>(ws), h);
+  NB_LAUNCH_OK("mc_scan_sums_kernel");
+  mc_scan_add_kernel<<<cdiv(P, 256), 256, 0, st>>>(cnt, P, tsum);
+  NB_LAUNCH_OK("mc_scan_add_kernel");
+  return 0;
+}
+
+int nerf_b200_marching_cubes_emit(const float* sigma, const float* xs, const float* ys, const float* zs,
+                                  int nx, int ny, int nz, float iso, float* verts, int64_t max_verts,
+                                  int32_t* faces, int64_t max_faces, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  if (int rc = check_mc_grid(nx, ny, nz)) return rc;
+  NB_CHECK_ARG(sigma && xs && ys && zs && workspace, "NULL pointer");
+  NB_CHECK_ARG((verts || max_verts == 0) && (faces || max_faces == 0) && max_verts >= 0 && max_faces >= 0, "NULL output with a capacity");
+  const size_t need = mc_need(nx, ny, nz);
+  NB_CHECK_ARG(workspace_bytes >= need, "workspace too small: need %zu bytes", need);
+  cudaStream_t st = (cudaStream_t)stream;
+  McHeader h;
+  NB_CUDA(cudaMemcpyAsync(&h, workspace, sizeof(h), cudaMemcpyDeviceToHost, st));
+  NB_CUDA(cudaStreamSynchronize(st));
+  NB_CHECK_ARG(h.nx == nx && h.ny == ny && h.nz == nz && memcmp(&h.iso, &iso, sizeof(float)) == 0,
+               "the workspace holds the counts of another grid or iso (call nerf_b200_marching_cubes_count first)");
+  NB_CHECK_ARG(max_verts >= h.V && max_faces >= h.F, "outputs too small: %lld vertices and %lld faces need room (got %lld, %lld)",
+               h.V, h.F, (long long)max_verts, (long long)max_faces);
+  const long long P = (long long)nx * ny * nz;
+  mc_emit_kernel<<<cdiv(P, 256), 256, 0, st>>>(sigma, xs, ys, zs, nx, ny, nz, iso,
+                                                reinterpret_cast<const int2*>(static_cast<uint8_t*>(workspace) + MC_HEADER_BYTES), verts, faces);
+  NB_LAUNCH_OK("mc_emit_kernel");
+  return 0;
 }
 
 int nerf_b200_raw2outputs(const float* raw, const float* z_vals, const float* rays_d, int d_stride, const float* noise,

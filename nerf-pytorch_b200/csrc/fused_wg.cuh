@@ -162,12 +162,21 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+// The density grid of density_wg_kernel / density_split_kernel: column n = i * ny + j of the pass is the "ray" of the nz points
+// (xs[i], ys[j], zs[k]), k = 0 .. nz - 1 (p.S = nz), and row m = n * nz + k of the pass is sigma's C-order index.
+struct DensityGrid { const float* xs; const float* ys; const float* zs; int ny; float* sigma; };
+
 // The pass of march_wg_kernel (SPLIT false) and march_split_kernel (SPLIT true, never EMIT).  SPLIT: every MMA operand is a hi
 // and a lo fp16 image (the split map of fused_tc.cuh), each weight chunk streams as two ring stages, the weights are scaled by
 // wscale[l] (a power of two: the accumulator starts at bias * wscale[l] and is scaled back exactly after the MMAs).
-template <bool EMIT, bool SPLIT>
-__device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveDev sv, const float* wscale) {
+// DENSITY (never EMIT): the points come from the axes of `grid`, only the pts layers stream and run, and the sigma head
+// (alpha_linear, or row 3 of output_linear without view directions) goes straight out as one fp32 per row: no view layers,
+// view bias, raw rows or compositing.  The head is the same code in the same order as the other modes, so sigma is bit for bit
+// raw[..., 3] of the pts mode on the same points.
+template <bool EMIT, bool SPLIT, bool DENSITY = false>
+__device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveDev sv, const float* wscale, const DensityGrid grid = {}) {
   static_assert(!(EMIT && SPLIT), "the split forward has no training mode");
+  static_assert(!(EMIT && DENSITY), "the density pass has no training mode");
   constexpr int NST = SPLIT ? SPLIT_NST : FWD_NST;
   constexpr int CPS = SPLIT ? 2 : 1;                              // ring stages per weight chunk
   uint8_t* smem = tc_smem;
@@ -176,7 +185,7 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
   float* s_heads = reinterpret_cast<float*>(smem + FWD_HEADS);
   float* s_bias = reinterpret_cast<float*>(smem + FWD_BIAS);
   const uint32_t a_heads = sb + FWD_HEADS, a_carry = sb + FWD_MISC;
-  const int D = p.D, NL = p.D + (p.use_viewdirs ? 2 : 0);
+  const int D = p.D, NL = DENSITY ? p.D : p.D + (p.use_viewdirs ? 2 : 0);
 
   // this CTA's rays / rows; the number of super-tiles is the tile plan's (train_common.cuh: plan_cta_nst)
   const long long ray0 = (long long)blockIdx.x * p.rays_per_cta;
@@ -261,7 +270,10 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
       float px = 0.f, py = 0.f, pz = 0.f;
       if (lr < nrows) {
         const long long m = row_begin + lr;
-        if (p.pts) { px = p.pts[m * 3]; py = p.pts[m * 3 + 1]; pz = p.pts[m * 3 + 2]; }
+        if constexpr (DENSITY) {
+          const long long n = m / p.S;
+          px = grid.xs[n / grid.ny]; py = grid.ys[n % grid.ny]; pz = grid.zs[m - n * p.S];
+        } else if (p.pts) { px = p.pts[m * 3]; py = p.pts[m * 3 + 1]; pz = p.pts[m * 3 + 2]; }
         else {
           const float* ry = p.rays + (ray0 + lr / p.S) * p.ray_stride;
           const float z = p.z_vals[m];
@@ -347,9 +359,9 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
               const float2 wa = *reinterpret_cast<const float2*>(s_heads + c);
               hp[0][3] = fmaf(a1, wa.y, fmaf(a0, wa.x, hp[0][3]));
               hp[1][3] = fmaf(b1, wa.y, fmaf(b0, wa.x, hp[1][3]));
-            } else {                                              // output_linear (:117)
+            } else {                                              // output_linear (:117); DENSITY: its sigma row only
 #pragma unroll
-              for (int k = 0; k < 4; ++k) {
+              for (int k = DENSITY ? 3 : 0; k < 4; ++k) {
                 const float2 wk = *reinterpret_cast<const float2*>(s_heads + 256 * k + c);
                 hp[0][k] = fmaf(a1, wk.y, fmaf(a0, wk.x, hp[0][k]));
                 hp[1][k] = fmaf(b1, wk.y, fmaf(b0, wk.x, hp[1][k]));
@@ -358,8 +370,8 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
           }
         }
         // without view directions only the fp32 head above reads h_{D-1}: inference skips the fp16 image, training mode still
-        // records it (output_linear's weight gradient reads it, dA_seed_output_kernel in bwd_wg.cuh)
-        if (EMIT || !(last_pts && !p.use_viewdirs)) {
+        // records it (output_linear's weight gradient reads it, dA_seed_output_kernel in bwd_wg.cuh); the density pass ends there
+        if (EMIT || !(last_pts && (DENSITY || !p.use_viewdirs))) {
           const bool relu = l < D;
           // column groups j, j + 1 of the warp's 16 rows as four 8 x 8 matrices (the accumulator fragment is stmatrix's):
           // matrix m = (group j + (m >> 1), rows + 8 (m & 1)); this lane addresses row (lane & 7) of matrix lane >> 3
@@ -451,6 +463,16 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
       }
     }
 
+    if constexpr (DENSITY) {
+      // ---- the sigma head's row sum over the quad (as raw[h][3] below) -> sigma ----
+      const float s0 = quad_sum(hp[0][3]), s1 = quad_sum(hp[1][3]);
+      if (q4 == 0) {
+        const float b = p.use_viewdirs ? s_heads[640] : s_heads[1027];
+        if (lrb + r0 < nrows) grid.sigma[row_begin + lrb + r0] = s0 + b;
+        if (lrb + r1 < nrows) grid.sigma[row_begin + lrb + r1] = s1 + b;
+      }
+      continue;
+    }
     // ---- heads: full row sums over the quad -> raw rows of the tile -> compositing ----
     ph.start();
     float raw[2][4];
@@ -493,6 +515,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
 // precision TC_SPLIT: fp32-class results from three fp16 MMAs per K-step (inference only; wscale: the split image's scales)
 __global__ void __launch_bounds__(TC_THREADS, 1) march_split_kernel(const MarchParams p, const float* __restrict__ wscale) {
   march_pass<false, true>(p, TrainSaveDev{}, wscale);
+}
+
+// The density grid (nerf_b200_density_grid): sigma on the points of `g`, precision TC_FP16 on the fp16 image, TC_SPLIT (wscale
+// the split image's scales) on the split image.  The forward's shared-memory map; the raw rows, carry and the ring stages of
+// the view layers go unused.
+static_assert(FWD_ALLOC <= 227 * 1024, "the density pass's shared-memory map exceeds the per-block limit");
+__global__ void __launch_bounds__(TC_THREADS, 1) density_wg_kernel(const MarchParams p, const DensityGrid g) {
+  march_pass<false, false, true>(p, TrainSaveDev{}, nullptr, g);
+}
+__global__ void __launch_bounds__(TC_THREADS, 1) density_split_kernel(const MarchParams p, const DensityGrid g, const float* __restrict__ wscale) {
+  march_pass<false, true, true>(p, TrainSaveDev{}, wscale, g);
 }
 
 }  // namespace nb
