@@ -499,8 +499,21 @@ def _train_save(lib, N, S, net_params, dev):
     check(lib.nerf_b200_train_record_bytes(N, S, C.byref(net_params), C.byref(ab), C.byref(mb)), "train_record_bytes")
     act = torch.empty(ab.value, dtype=torch.uint8, device=dev)
     mask = torch.empty(mb.value, dtype=torch.uint8, device=dev)
-    sv = NerfTrainSave(_ptr(act), ab.value, _ptr(mask), mb.value)
-    return sv, act, mask
+    return _records_save(act, mask), act, mask
+
+
+def _records_save(act, mask):
+    """NerfTrainSave over the records (uint8 tensors) of one training-mode pass."""
+    return NerfTrainSave(_ptr(act), act.numel(), _ptr(mask), mask.numel())
+
+
+def _pass_structs(net, gbuf, rec, train_tc):
+    """NerfNetParams, NerfNetGrads and, for the tensor-core backward, NerfTrainSave of one backward pass (rec: raw, act, mask)."""
+    return net.net_params(), net.grad_struct(gbuf), (_records_save(rec[1], rec[2]) if train_tc else None)
+
+
+def _workspace(nbytes, dev):
+    return torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
 
 
 # render() -> batchify_rays -> render_rays -> _RenderRays.forward: when the whole image is ONE chunk, render() does not launch
@@ -638,18 +651,17 @@ class _RenderRays(torch.autograd.Function):
             s_coarse = dict(rgb_map=g[3], disp_map=g[4], acc_map=g[5])
         else:
             s_fine, s_coarse = {}, dict(rgb_map=g[0], disp_map=g[1], acc_map=g[2], raw=g[3])
-        extra = any(v is not None for s in (s_fine, s_coarse) for k, v in s.items() if k != "rgb_map")
-        if not extra:
-            # rgb / rgb0 only: the entry points (and the zero gradient of an unused rgb output) of the rgb-only backward
-            g_fine = None
-            if fine:
-                g_fine = s_fine["rgb_map"] if s_fine["rgb_map"] is not None else torch.zeros((N, 3), device=ray_batch.device)
-                g_coarse = s_coarse["rgb_map"] if s_coarse["rgb_map"] is not None else torch.zeros((N, 3), device=ray_batch.device)
-            else:
-                g_coarse = s_coarse["rgb_map"]
-            return _RenderRays._backward_rgb(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg, g_fine, g_coarse)
-        return _RenderRays._backward_outs(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg,
-                                          s_fine if fine else None, s_coarse)
+        rgb_only = not any(v is not None for s in (s_fine, s_coarse) for k, v in s.items() if k != "rgb_map")
+
+        def seed(s):
+            if not rgb_only:
+                return _out_grads(**s) if any(v is not None for v in s.values()) else None
+            g_rgb = s["rgb_map"]
+            if g_rgb is None and fine:                  # both passes run: an unused rgb output seeds zeros
+                g_rgb = torch.zeros((N, 3), device=ray_batch.device)
+            return None if g_rgb is None else g_rgb.contiguous().float()
+        return _RenderRays._backward(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg,
+                                     seed(s_fine) if fine else None, seed(s_coarse), rgb_only)
 
     @staticmethod
     def _passes(ctx, z_c, z_f, noise0, noise1, rec, seed_f, seed_c):
@@ -670,94 +682,50 @@ class _RenderRays(torch.autograd.Function):
         return passes, tuple(out)
 
     @staticmethod
-    def _backward_outs(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg, s_fine, s_coarse):
-        """Backward from the gradients of any of the outputs (NerfOutGrads per pass): the _outs entry points.  A pass runs
-        when any of its seeds is present."""
+    def _backward(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg, seed_f, seed_c, rgb_only):
+        """The backward of the passes with a seed (None: the pass does not run).  rgb_only: each seed is dL/drgb_map and the
+        rgb-only entry points run (nerf_b200_render_rays_bwd_tc / march_bwd_tc / march_bwd); otherwise each seed is a
+        (NerfOutGrads, tensors) pair from _out_grads and their _outs variants run."""
         N = ray_batch.shape[0]
-        og_f = _out_grads(**s_fine) if s_fine is not None and any(v is not None for v in s_fine.values()) else None
-        og_c = _out_grads(**s_coarse) if any(v is not None for v in s_coarse.values()) else None
-        passes, out = _RenderRays._passes(ctx, z_c, z_f, noise0, noise1, rec, og_f, og_c)
+        sfx = "" if rgb_only else "_outs"
+
+        def seed_arg(seed):
+            return _ptr(seed) if rgb_only else C.byref(seed[0])
+        passes, out = _RenderRays._passes(ctx, z_c, z_f, noise0, noise1, rec, seed_f, seed_c)
         with _on(ray_batch):
-            if ctx.train_tc and og_f is not None and og_c is not None:
+            if ctx.train_tc and seed_f is not None and seed_c is not None:
+                # both passes in one call: one after the other on the stream (capi.cu: render_rays_bwd_tc_impl)
                 keep, bp = [], []
-                for (og, _), z, noise, net, gbuf, rc in passes:
-                    raw, act, mask = rc
-                    n, gs = net.net_params(), net.grad_struct(gbuf)
-                    sv = NerfTrainSave(_ptr(act), act.numel(), _ptr(mask), mask.numel())
+                for seed, z, noise, net, gbuf, rc in passes:
+                    n, gs, sv = _pass_structs(net, gbuf, rc, True)
                     keep += [n, gs, sv]
                     bp.append(_lib.NerfBwdPass(_ptr(z), _ptr(noise if noise.numel() else None), z.shape[1], C.pointer(n), _ptr(net.packed()),
-                                               _ptr(raw), C.pointer(sv), _ptr(None), C.pointer(gs)))
+                                               _ptr(rc[0]), C.pointer(sv), _ptr(seed if rgb_only else None), C.pointer(gs)))
                 ws_bytes = lib.nerf_b200_render_rays_bwd_tc_workspace_bytes(N, bp[0].S, bp[0].net, bp[1].S, bp[1].net)
-                ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=ray_batch.device)
-                check(lib.nerf_b200_render_rays_bwd_tc_outs(_ptr(ray_batch), N, C.byref(cfg), C.byref(bp[0]), C.byref(bp[1]),
-                                                            C.byref(og_c[0]), C.byref(og_f[0]), _ptr(ws), ws_bytes, _stream(ray_batch)),
-                      "render_rays_bwd_tc_outs")
+                ws = _workspace(ws_bytes, ray_batch.device)
+                seeds = () if rgb_only else (C.byref(seed_c[0]), C.byref(seed_f[0]))
+                check(getattr(lib, "nerf_b200_render_rays_bwd_tc" + sfx)(_ptr(ray_batch), N, C.byref(cfg), C.byref(bp[0]), C.byref(bp[1]),
+                                                                         *seeds, _ptr(ws), ws_bytes, _stream(ray_batch)),
+                      "render_rays_bwd_tc" + sfx)
                 return out
-            for og, z, noise, net, gbuf, rc in passes:
-                if og is None:
+            for seed, z, noise, net, gbuf, rc in passes:
+                if seed is None:
                     continue
                 S = z.shape[1]
-                n = net.net_params()
-                gs = net.grad_struct(gbuf)
+                n, gs, sv = _pass_structs(net, gbuf, rc, ctx.train_tc)
                 nz = _ptr(noise if noise.numel() else None)
                 if ctx.train_tc:
-                    raw, act, mask = rc
-                    sv = NerfTrainSave(_ptr(act), act.numel(), _ptr(mask), mask.numel())
                     ws_bytes = lib.nerf_b200_march_bwd_tc_workspace_bytes(N, S, C.byref(n))
-                    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=z.device)
-                    check(lib.nerf_b200_march_bwd_tc_outs(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(net.packed()), C.byref(cfg),
-                                                          _ptr(raw), C.byref(sv), C.byref(og[0]), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)),
-                          "march_bwd_tc_outs")
+                    ws = _workspace(ws_bytes, z.device)
+                    check(getattr(lib, "nerf_b200_march_bwd_tc" + sfx)(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(net.packed()),
+                                                                       C.byref(cfg), _ptr(rc[0]), C.byref(sv), seed_arg(seed), C.byref(gs),
+                                                                       _ptr(ws), ws_bytes, _stream(z)), "march_bwd_tc" + sfx)
                 else:
                     ws_bytes = lib.nerf_b200_march_bwd_workspace_bytes(N, S, C.byref(n))
-                    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=z.device)
-                    check(lib.nerf_b200_march_bwd_outs(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(None), C.byref(cfg),
-                                                       C.byref(og[0]), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)), "march_bwd_outs")
-        return out
-
-    @staticmethod
-    def _backward_rgb(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg, g_fine, g_coarse):
-        """Backward from dL/drgb_map (and dL/drgb0) alone: nerf_b200_render_rays_bwd_tc / march_bwd_tc / march_bwd."""
-        N = ray_batch.shape[0]
-        fine = ctx.cfgd["N_importance"] > 0
-        passes, out = _RenderRays._passes(ctx, z_c, z_f, noise0, noise1, rec, g_fine, g_coarse)
-        with _on(ray_batch):
-            if ctx.train_tc and fine and g_fine is not None and g_coarse is not None:
-                # both passes in one call: the chain of one pass runs next to the weight gradient of the other (capi.cu)
-                keep, bp = [], []
-                for g_rgb, z, noise, net, gbuf, rc in passes:
-                    raw, act, mask = rc
-                    n, gs, g_rgb = net.net_params(), net.grad_struct(gbuf), g_rgb.contiguous().float()
-                    sv = NerfTrainSave(_ptr(act), act.numel(), _ptr(mask), mask.numel())
-                    keep += [n, gs, g_rgb, sv]
-                    bp.append(_lib.NerfBwdPass(_ptr(z), _ptr(noise if noise.numel() else None), z.shape[1], C.pointer(n), _ptr(net.packed()),
-                                               _ptr(raw), C.pointer(sv), _ptr(g_rgb), C.pointer(gs)))
-                ws_bytes = lib.nerf_b200_render_rays_bwd_tc_workspace_bytes(N, bp[0].S, bp[0].net, bp[1].S, bp[1].net)
-                ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=ray_batch.device)
-                check(lib.nerf_b200_render_rays_bwd_tc(_ptr(ray_batch), N, C.byref(cfg), C.byref(bp[0]), C.byref(bp[1]), _ptr(ws), ws_bytes,
-                                                       _stream(ray_batch)), "render_rays_bwd_tc")
-                passes = []
-            for g_rgb, z, noise, net, gbuf, rc in passes:
-                if g_rgb is None:
-                    continue
-                S = z.shape[1]
-                n = net.net_params()
-                gs = net.grad_struct(gbuf)
-                g_rgb = g_rgb.contiguous().float()
-                nz = _ptr(noise if noise.numel() else None)
-                if ctx.train_tc:
-                    raw, act, mask = rc
-                    sv = NerfTrainSave(_ptr(act), act.numel(), _ptr(mask), mask.numel())
-                    ws_bytes = lib.nerf_b200_march_bwd_tc_workspace_bytes(N, S, C.byref(n))
-                    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=z.device)
-                    check(lib.nerf_b200_march_bwd_tc(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(net.packed()), C.byref(cfg),
-                                                     _ptr(raw), C.byref(sv), _ptr(g_rgb), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)),
-                          "march_bwd_tc")
-                else:
-                    ws_bytes = lib.nerf_b200_march_bwd_workspace_bytes(N, S, C.byref(n))
-                    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=z.device)
-                    check(lib.nerf_b200_march_bwd(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(None), C.byref(cfg),
-                                                  _ptr(g_rgb), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)), "march_bwd")
+                    ws = _workspace(ws_bytes, z.device)
+                    check(getattr(lib, "nerf_b200_march_bwd" + sfx)(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(None), C.byref(cfg),
+                                                                    seed_arg(seed), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)),
+                          "march_bwd" + sfx)
         return out
 
 

@@ -31,6 +31,18 @@ static bool g_timing = false;
 static TimedLaunch g_timed[4096];
 static int g_ntimed = 0;
 
+// the device-time bracket of one launch: NULL when timing is off (or the table is full)
+static TimedLaunch* timing_begin(int kind, double flops, cudaStream_t st) {
+  if (!g_timing || g_ntimed >= 4096) return nullptr;
+  TimedLaunch* tl = &g_timed[g_ntimed++];
+  cudaEventCreate(&tl->a); cudaEventCreate(&tl->b);
+  tl->flops = flops;
+  tl->kind = kind;
+  cudaEventRecord(tl->a, st);
+  return tl;
+}
+static void timing_end(TimedLaunch* tl, cudaStream_t st) { if (tl) cudaEventRecord(tl->b, st); }
+
 static double net_macs_per_row(const NerfNetParams& n) {
   // MACs of the reference's Linear layers per sample row (SURVEY Appendix B)
   double m = (double)n.input_ch * n.W;
@@ -68,9 +80,9 @@ static int smem_optin(const void* fn, size_t bytes) {
   return 0;
 }
 
-// per-device facts (SM count; which kernels already have their > 48 KB shared-memory opt-in): the library may be used
-// on several devices of one process, and cudaFuncSetAttribute is per device
-struct DeviceState { int sms; bool optin_fwd, optin_bwd, optin_split; };
+// per-device facts (SM count; which fixed-size kernels already have their > 48 KB shared-memory opt-in): the library may be
+// used on several devices of one process, and cudaFuncSetAttribute is per device
+struct DeviceState { int sms, n_optin; const void* optin[16]; };
 static DeviceState* device_state() {
   static DeviceState st[64];
   static bool init[64] = {false};
@@ -81,7 +93,7 @@ static DeviceState* device_state() {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     st[dev].sms = n > 0 ? n : 132;
-    st[dev].optin_fwd = st[dev].optin_bwd = st[dev].optin_split = false;
+    st[dev].n_optin = 0;
     cudaGetLastError();
     init[dev] = true;
   }
@@ -89,11 +101,59 @@ static DeviceState* device_state() {
 }
 static int num_sms() { return device_state()->sms; }
 
+// the opt-in of a kernel whose shared memory is the same on every launch: once per device.  (Kernels whose shared memory
+// follows the arguments opt in on every call.)
+static int smem_optin_once(const void* fn, size_t bytes) {
+  DeviceState* ds = device_state();
+  for (int i = 0; i < ds->n_optin; ++i) if (ds->optin[i] == fn) return 0;
+  if (int rc = smem_optin(fn, bytes)) return rc;
+  if (ds->n_optin < 16) ds->optin[ds->n_optin++] = fn;
+  return 0;
+}
+
+// n floats rounded up to 16 bytes: mlp_simt_kernel stores raw as float4, and raw2outputs_bwd_kernel loads it so, so the exact
+// path's scratch buffers start on 16-byte boundaries whatever their row counts
+static long long round4(long long n) { return (n + 3) & ~3ll; }
+
+// the exact path's MLP (mlp_simt_kernel) over M rows; its shared memory follows the net, so it opts in on every call
+static int launch_mlp_simt(const float* pts, const float* dirs, int dir_stride, long long M, int S, const NerfNetParams& net,
+                           int L, int Lv, float* raw, const SimtSave& sv, cudaStream_t st) {
+  const size_t sm = simt_smem_bytes(net);
+  if (int rc = smem_optin((const void*)mlp_simt_kernel, sm)) return rc;
+  mlp_simt_kernel<<<cdiv(M, SIMT_ROWS), SIMT_THREADS, sm, st>>>(pts, dirs, dir_stride, M, S, net, L, Lv, raw, sv);
+  NB_LAUNCH_OK("mlp_simt_kernel");
+  return 0;
+}
+
 static bool is_tc(int precision) { return precision == NERF_B200_PREC_TC_FP16 || precision == NERF_B200_PREC_TC_SPLIT; }
 static PackLayout pack_layout_for(const NerfNetParams& net, int precision) {
   return precision == NERF_B200_PREC_TC_SPLIT ? make_pack_layout_split(net) : make_pack_layout(net);
 }
 #define NB_SPLIT_TRAIN_MSG "precision TC_SPLIT has no training-mode records: it trains through the exact backward (nerf_b200_march_bwd)"
+
+// The network half of a fused tensor-core pass over N rays of S samples (march, run_network, density_grid): validates it,
+// fills MarchParams' network fields from the packed image of `precision` and plans the persistent grid (whole rays per CTA,
+// balanced over the SMs).
+static int tc_pass_setup(const NerfNetParams* net, const void* packed, int precision, int L, long long N, int S,
+                         MarchParams& p, PackLayout& PL, TilePlan& plan) {
+  if (int rc = check_tc_net(net)) return rc;
+  NB_CHECK_ARG(packed != nullptr, precision == NERF_B200_PREC_TC_SPLIT ? "packed weights are NULL (call nerf_b200_pack_weights_split)"
+                                                                      : "packed weights are NULL (call nerf_b200_pack_weights)");
+  NB_CHECK_ARG(N > 0 && S > 0, "empty ray batch must be handled by the caller (N=%lld S=%d)", N, S);
+  NB_CHECK_ARG((long long)N * S < (1ll << 40), "batch too large");
+  NB_CHECK_ARG(3 + 6 * L == net->input_ch || (L == 0 && net->input_ch == 3), "multires %d does not match input_ch %d", L, net->input_ch);
+  plan = make_tile_plan(N, S, num_sms());
+  NB_CHECK_ARG((long long)plan.rays_per_cta * S < (1ll << 30), "rays_per_cta * S overflows");
+  PL = pack_layout_for(*net, precision);
+  const uint8_t* pk = static_cast<const uint8_t*>(packed);
+  memset(&p, 0, sizeof(p));
+  p.N = N; p.S = S; p.rays_per_cta = plan.rays_per_cta;
+  p.chunks = pk + PL.off_chunks;
+  p.bias = reinterpret_cast<const float*>(pk + PL.off_bias);
+  p.heads = reinterpret_cast<const float*>(pk + PL.off_heads);
+  p.D = net->D; p.skip = net->skip; p.use_viewdirs = net->use_viewdirs; p.L = L; p.IC = net->input_ch;
+  return 0;
+}
 
 // shared launcher of the fused tensor-core pass; `save` != NULL selects the training-mode kernel (EMIT); precision TC_SPLIT runs
 // march_split_kernel on the split packed image (nerf_b200_pack_weights_split)
@@ -102,24 +162,24 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
                         const NerfNetParams* net, const void* packed, int L, int Lv, int white_bkgd, int do_composite,
                         const NerfPassOut* out, void* workspace, size_t workspace_bytes, const NerfTrainSave* save, const float* vb_pre,
                         cudaStream_t st, int precision = NERF_B200_PREC_TC_FP16) {
-  if (int rc = check_tc_net(net)) return rc;
-  const bool split = precision == NERF_B200_PREC_TC_SPLIT;
-  NB_CHECK_ARG(!(split && save), NB_SPLIT_TRAIN_MSG);
-  NB_CHECK_ARG(packed != nullptr, split ? "packed weights are NULL (call nerf_b200_pack_weights_split)" : "packed weights are NULL (call nerf_b200_pack_weights)");
-  NB_CHECK_ARG(N > 0 && S > 0, "empty ray batch must be handled by the caller (N=%lld S=%d)", N, S);
-  NB_CHECK_ARG((long long)N * S < (1ll << 40), "batch too large");
-  NB_CHECK_ARG(3 + 6 * L == net->input_ch || (L == 0 && net->input_ch == 3), "multires %d does not match input_ch %d", L, net->input_ch);
-  const PackLayout PL = pack_layout_for(*net, precision);
-  const uint8_t* pk = static_cast<const uint8_t*>(packed);
   MarchParams p;
-  memset(&p, 0, sizeof(p));
+  PackLayout PL;
+  TilePlan plan;
+  if (int rc = tc_pass_setup(net, packed, precision, L, N, S, p, PL, plan)) return rc;
+  const uint8_t* pk = static_cast<const uint8_t*>(packed);
   p.rays = rays; p.ray_stride = ray_stride; p.z_vals = z_vals; p.pts = pts; p.noise = noise;
-  p.N = N; p.S = S;
-  p.bias = reinterpret_cast<const float*>(pk + PL.off_bias);
-  p.heads = reinterpret_cast<const float*>(pk + PL.off_heads);
-  p.D = net->D; p.skip = net->skip; p.use_viewdirs = net->use_viewdirs; p.L = L; p.IC = net->input_ch;
   p.white_bkgd = white_bkgd; p.do_composite = do_composite;
   if (out) p.out = *out;
+  TrainSaveDev sv;
+  memset(&sv, 0, sizeof(sv));
+  if (save) {
+    NB_CHECK_ARG(save->act && save->mask, "training-mode save buffers are NULL");
+    NB_CHECK_ARG(save->act_bytes >= (size_t)plan.n_tiles * rec_act_bytes(net->D) && save->mask_bytes >= (size_t)plan.n_tiles * rec_mask_bytes(net->D),
+                 "training-mode save buffers too small (see nerf_b200_train_record_bytes)");
+    NB_CHECK_ARG((reinterpret_cast<uintptr_t>(save->act) & 15) == 0 && (reinterpret_cast<uintptr_t>(save->mask) & 15) == 0, "save buffers must be 16-byte aligned");
+    sv.act = static_cast<uint8_t*>(save->act); sv.mask = static_cast<uint8_t*>(save->mask);
+    sv.nst_plan = plan.nst; sv.rec_act = rec_act_bytes(net->D); sv.rec_mask = rec_mask_bytes(net->D);
+  }
   if (net->use_viewdirs && vb_pre != nullptr) {
     p.vb = vb_pre;                                     // the per-ray view-bias table was prepared by ray_setup_kernel
   } else if (net->use_viewdirs) {
@@ -132,39 +192,10 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
     NB_LAUNCH_OK("view_bias_kernel");
     p.vb = vb;
   }
-  // persistent grid: whole rays per CTA, balanced over the SMs (the tile plan)
-  DeviceState* ds = device_state();
-  const TilePlan plan = make_tile_plan(N, S, ds->sms);
-  p.rays_per_cta = plan.rays_per_cta;
-  NB_CHECK_ARG((long long)p.rays_per_cta * S < (1ll << 30), "rays_per_cta * S overflows");
-  if (split && !ds->optin_split) {
-    if (int rc = smem_optin((const void*)march_split_kernel, FWD_ALLOC)) return rc;
-    ds->optin_split = true;
-  }
-  if (!split && !ds->optin_fwd) {
-    if (int rc = smem_optin((const void*)march_wg_kernel<false>, FWD_ALLOC)) return rc;
-    if (int rc = smem_optin((const void*)march_wg_kernel<true>, FWD_ALLOC)) return rc;
-    ds->optin_fwd = true;
-  }
-  TrainSaveDev sv;
-  memset(&sv, 0, sizeof(sv));
-  if (save) {
-    NB_CHECK_ARG(save->act && save->mask, "training-mode save buffers are NULL");
-    NB_CHECK_ARG(save->act_bytes >= (size_t)plan.n_tiles * rec_act_bytes(net->D) && save->mask_bytes >= (size_t)plan.n_tiles * rec_mask_bytes(net->D),
-                 "training-mode save buffers too small (see nerf_b200_train_record_bytes)");
-    NB_CHECK_ARG((reinterpret_cast<uintptr_t>(save->act) & 15) == 0 && (reinterpret_cast<uintptr_t>(save->mask) & 15) == 0, "save buffers must be 16-byte aligned");
-    sv.act = static_cast<uint8_t*>(save->act); sv.mask = static_cast<uint8_t*>(save->mask);
-    sv.nst_plan = plan.nst; sv.rec_act = rec_act_bytes(net->D); sv.rec_mask = rec_mask_bytes(net->D);
-  }
-  TimedLaunch* tl = nullptr;
-  if (g_timing && g_ntimed < 4096) {
-    tl = &g_timed[g_ntimed++];
-    cudaEventCreate(&tl->a); cudaEventCreate(&tl->b);
-    tl->flops = 2.0 * net_macs_per_row(*net) * (double)(N * (long long)S);
-    tl->kind = 0;
-    cudaEventRecord(tl->a, st);
-  }
-  p.chunks = pk + PL.off_chunks;
+  const bool split = precision == NERF_B200_PREC_TC_SPLIT;
+  const void* kernel = split ? (const void*)march_split_kernel : !save ? (const void*)march_wg_kernel<false> : (const void*)march_wg_kernel<true>;
+  if (int rc = smem_optin_once(kernel, FWD_ALLOC)) return rc;
+  TimedLaunch* tl = timing_begin(0, 2.0 * net_macs_per_row(*net) * (double)(N * (long long)S), st);
 #ifdef NERF_B200_PHASE_PROBE
   {
     const int slot = (int)(g_phase_launches++ % PH_SLOTS);
@@ -173,14 +204,56 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
 #endif
   if (split) {
     march_split_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, reinterpret_cast<const float*>(pk + PL.off_wscale));
-    if (tl) cudaEventRecord(tl->b, st);
+    timing_end(tl, st);
     NB_LAUNCH_OK("march_split_kernel");
     return 0;
   }
   if (save) march_wg_kernel<true><<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, sv);
   else march_wg_kernel<false><<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, sv);
-  if (tl) cudaEventRecord(tl->b, st);
+  timing_end(tl, st);
   NB_LAUNCH_OK("march_wg_kernel");
+  return 0;
+}
+
+// Forward layer l of the packed image: weight [rows][ld], whose first `in` columns are the encoded input (layer 0 and the layer
+// after the skip: cat([input_pts, h])) and the next `h` the previous activation.
+struct FwdLayer { const float* w; int ld, rows, in, h; };
+static FwdLayer fwd_layer(const NerfNetParams& n, int l) {
+  const int IC = n.input_ch, W = n.W;
+  if (l == 0) return {n.pts_w[0], IC, 256, IC, 0};
+  if (l < n.D) {
+    const bool sk = n.skip >= 0 && l == n.skip + 1;
+    return {n.pts_w[l], sk ? W + IC : W, 256, sk ? IC : 0, W};
+  }
+  if (l == n.D) return {n.feature_w, W, 256, 0, W};
+  return {n.views_w, W + n.input_ch_views, 128, 0, W};                  // the view columns go to the per-ray view bias
+}
+
+// The forward's chunks in stream order (K = 32 each: two over the input columns, eight over h), `row_bytes` per row of a chunk
+// from PL.off_chunks; layer[i] (if given) receives chunk i's layer.  False when the table disagrees with the layout.
+static bool fwd_chunks(const NerfNetParams& n, const PackLayout& PL, unsigned row_bytes, PackJob& job, unsigned char* layer) {
+  job.n = 0;
+  unsigned off = (unsigned)PL.off_chunks;
+  for (int l = 0; l < PL.NL; ++l) {
+    const FwdLayer L = fwd_layer(n, l);
+    auto add = [&](int k0, int kvalid) {
+      if (layer) layer[job.n] = (unsigned char)l;
+      PackChunk& c = job.c[job.n++];
+      c.src = L.w; c.sn = L.ld; c.sk = 1; c.k0 = k0; c.kvalid = kvalid < 0 ? 0 : (kvalid > 32 ? 32 : kvalid); c.nrows = L.rows; c.dst_off = off;
+      off += (unsigned)L.rows * row_bytes;
+    };
+    if (L.in) { add(0, L.in); add(32, L.in - 32); }
+    for (int k0 = L.in; k0 < L.in + L.h; k0 += 32) add(k0, 32);
+  }
+  return job.n == PL.n_chunks && off == PL.off_chunks + PL.chunk_bytes;
+}
+
+// the fp32 tables (biases, heads, view-layer columns) of either image
+static int pack_tables(const NerfNetParams& net, const PackLayout& PL, uint8_t* dst, cudaStream_t st) {
+  PackTables t;
+  t.net = net; t.off_bias = PL.off_bias; t.off_heads = PL.off_heads; t.off_vdir = PL.off_vdir;
+  pack_tables_kernel<<<8, 256, 0, st>>>(t, dst);
+  NB_LAUNCH_OK("pack_tables_kernel");
   return 0;
 }
 
@@ -237,26 +310,9 @@ int nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t packed
   const PackLayout PL = make_pack_layout(*net);
   NB_CHECK_ARG(packed && packed_bytes >= PL.total, "packed buffer too small (%zu < %zu)", packed_bytes, PL.total);
   cudaStream_t st = (cudaStream_t)stream;
-  PackJob job;
-  job.n = 0;
-  unsigned off = (unsigned)PL.off_chunks;
   const int IC = net->input_ch, W = net->W;
-  auto add = [&](const float* src, int ld, int k0, int kvalid, int nrows) {
-    PackChunk& c = job.c[job.n++];
-    c.src = src; c.sn = ld; c.sk = 1; c.k0 = k0; c.kvalid = kvalid < 0 ? 0 : (kvalid > 32 ? 32 : kvalid); c.nrows = nrows; c.dst_off = off;
-    off += (unsigned)nrows * 64;
-  };
-  for (int l = 0; l < PL.NL; ++l) {
-    if (l == 0) { add(net->pts_w[0], IC, 0, IC, 256); add(net->pts_w[0], IC, 32, IC - 32, 256); }
-    else if (l < net->D) {
-      const bool sk = (net->skip >= 0 && l == net->skip + 1);
-      const int ld = sk ? W + IC : W, base = sk ? IC : 0;
-      if (sk) { add(net->pts_w[l], ld, 0, IC, 256); add(net->pts_w[l], ld, 32, IC - 32, 256); }    // cat([input_pts, h])
-      for (int c = 0; c < 8; ++c) add(net->pts_w[l], ld, base + 32 * c, 32, 256);
-    } else if (l == net->D) { for (int c = 0; c < 8; ++c) add(net->feature_w, W, 32 * c, 32, 256); }
-    else { for (int c = 0; c < 8; ++c) add(net->views_w, W + net->input_ch_views, 32 * c, 32, 128); }
-  }
-  NB_CHECK_ARG(job.n == PL.n_chunks && off == PL.off_chunks + PL.chunk_bytes, "internal: chunk table mismatch");
+  PackJob job;
+  NB_CHECK_ARG(fwd_chunks(*net, PL, 64, job, nullptr), "internal: chunk table mismatch");
   dim3 grid(4, job.n);
   pack_chunks_kernel<<<grid, 256, 0, st>>>(job, static_cast<uint8_t*>(packed));
   NB_LAUNCH_OK("pack_chunks_kernel");
@@ -286,11 +342,7 @@ int nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t packed
     pack_chunks_kernel<<<g2, 256, 0, st>>>(bj2, static_cast<uint8_t*>(packed));
     NB_LAUNCH_OK("pack_chunks_kernel (backward stream)");
   }
-  PackTables t;
-  t.net = *net; t.off_bias = PL.off_bias; t.off_heads = PL.off_heads; t.off_vdir = PL.off_vdir;
-  pack_tables_kernel<<<8, 256, 0, st>>>(t, static_cast<uint8_t*>(packed));
-  NB_LAUNCH_OK("pack_tables_kernel");
-  return 0;
+  return pack_tables(*net, PL, static_cast<uint8_t*>(packed), st);
 }
 
 size_t nerf_b200_packed_bytes_split(const NerfNetParams* net) {
@@ -307,46 +359,21 @@ int nerf_b200_pack_weights_split(const NerfNetParams* net, void* packed, size_t 
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* dst = static_cast<uint8_t*>(packed);
   float* scale = reinterpret_cast<float*>(dst + PL.off_wscale);
-  const int IC = net->input_ch, W = net->W;
+  PackSplitJob job;
+  memset(&job, 0, sizeof(job));
+  NB_CHECK_ARG(fwd_chunks(*net, PL, 128, job.job, job.layer), "internal: split chunk table mismatch");   // hi | lo stages
   SplitScaleJob sj;
   memset(&sj, 0, sizeof(sj));
   sj.n = PL.NL;
   for (int l = 0; l < PL.NL; ++l) {
-    const bool sk = l < net->D && net->skip >= 0 && l == net->skip + 1;
-    if (l < net->D) { sj.src[l] = net->pts_w[l]; sj.rows[l] = 256; sj.cols[l] = l == 0 ? IC : (sk ? W + IC : W); }
-    else if (l == net->D) { sj.src[l] = net->feature_w; sj.rows[l] = 256; sj.cols[l] = W; }
-    else { sj.src[l] = net->views_w; sj.rows[l] = 128; sj.cols[l] = W; }
-    sj.ld[l] = (l == net->D + 1) ? W + net->input_ch_views : sj.cols[l];
+    const FwdLayer L = fwd_layer(*net, l);
+    sj.src[l] = L.w; sj.rows[l] = L.rows; sj.cols[l] = L.in + L.h; sj.ld[l] = L.ld;
   }
   split_scale_kernel<<<PL.NL, 256, 0, st>>>(sj, scale);
   NB_LAUNCH_OK("split_scale_kernel");
-  PackSplitJob job;
-  memset(&job, 0, sizeof(job));
-  unsigned off = (unsigned)PL.off_chunks;
-  auto add = [&](int layer, const float* src, int ld, int k0, int kvalid, int nrows) {
-    job.layer[job.job.n] = (unsigned char)layer;
-    PackChunk& c = job.job.c[job.job.n++];
-    c.src = src; c.sn = ld; c.sk = 1; c.k0 = k0; c.kvalid = kvalid < 0 ? 0 : (kvalid > 32 ? 32 : kvalid); c.nrows = nrows; c.dst_off = off;
-    off += (unsigned)nrows * 128;                       // two stages of nrows x 64 B
-  };
-  for (int l = 0; l < PL.NL; ++l) {
-    if (l == 0) { add(0, net->pts_w[0], IC, 0, IC, 256); add(0, net->pts_w[0], IC, 32, IC - 32, 256); }
-    else if (l < net->D) {
-      const bool sk = (net->skip >= 0 && l == net->skip + 1);
-      const int ld = sk ? W + IC : W, base = sk ? IC : 0;
-      if (sk) { add(l, net->pts_w[l], ld, 0, IC, 256); add(l, net->pts_w[l], ld, 32, IC - 32, 256); }
-      for (int c = 0; c < 8; ++c) add(l, net->pts_w[l], ld, base + 32 * c, 32, 256);
-    } else if (l == net->D) { for (int c = 0; c < 8; ++c) add(l, net->feature_w, W, 32 * c, 32, 256); }
-    else { for (int c = 0; c < 8; ++c) add(l, net->views_w, W + net->input_ch_views, 32 * c, 32, 128); }
-  }
-  NB_CHECK_ARG(job.job.n == PL.n_chunks && off == PL.off_chunks + PL.chunk_bytes, "internal: split chunk table mismatch");
   pack_chunks_split_kernel<<<dim3(8, job.job.n), 256, 0, st>>>(job, scale, dst);
   NB_LAUNCH_OK("pack_chunks_split_kernel");
-  PackTables t;
-  t.net = *net; t.off_bias = PL.off_bias; t.off_heads = PL.off_heads; t.off_vdir = PL.off_vdir;
-  pack_tables_kernel<<<8, 256, 0, st>>>(t, dst);
-  NB_LAUNCH_OK("pack_tables_kernel");
-  return 0;
+  return pack_tables(*net, PL, dst, st);
 }
 
 int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, int S, const NerfNetParams* net,
@@ -358,12 +385,7 @@ int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, in
   if (precision == NERF_B200_PREC_FP32) {
     if (int rc = check_exact_net(net)) return rc;
     NB_CHECK_ARG(!net->use_viewdirs || viewdirs, "viewdirs required");
-    const long long M = N * (long long)S;
-    const size_t sm = simt_smem_bytes(*net);
-    if (int rc = smem_optin((const void*)mlp_simt_kernel, sm)) return rc;
-    mlp_simt_kernel<<<cdiv(M, SIMT_ROWS), SIMT_THREADS, sm, st>>>(pts, viewdirs, 3, M, S, *net, multires, multires_views, raw, SimtSave{});
-    NB_LAUNCH_OK("mlp_simt_kernel");
-    return 0;
+    return launch_mlp_simt(pts, viewdirs, 3, N * (long long)S, S, *net, multires, multires_views, raw, SimtSave{}, st);
   }
   NB_CHECK_ARG(is_tc(precision), "unknown precision %d", precision);
   NerfPassOut out;
@@ -377,14 +399,13 @@ int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, in
 // precision FP32 evaluates the grid in slabs of DENSITY_SLAB points: the points, then mlp_simt_kernel into raw rows, then their
 // sigma column.  Workspace: 256 B (the zero view direction every row reads, dir_stride 0) | pts [slab, 3] | raw [slab, 4].
 static const long long DENSITY_SLAB = 1ll << 20;
-static size_t density_pts_floats(long long slab) { return ((size_t)slab * 3 + 3) & ~(size_t)3; }
 
 size_t nerf_b200_density_grid_workspace_bytes(int nx, int ny, int nz, const NerfNetParams* net, int precision) {
   if (nx < 1 || ny < 1 || nz < 1) return 0;
   if (precision == NERF_B200_PREC_FP32) {
     if (check_exact_net(net)) return 0;
     const long long P = (long long)nx * ny * nz, slab = P < DENSITY_SLAB ? P : DENSITY_SLAB;
-    return 256 + density_pts_floats(slab) * 4 + (size_t)slab * 16;
+    return 256 + (size_t)round4(slab * 3) * 4 + (size_t)slab * 16;
   }
   if (!is_tc(precision) || check_tc_net(net)) return 0;
   return 256;                                          // the tensor-core pass needs none
@@ -410,42 +431,29 @@ int nerf_b200_density_grid(const float* xs, int nx, const float* ys, int ny, con
     const float* zero_dir = reinterpret_cast<const float*>(ws);
     float* pts = reinterpret_cast<float*>(ws + 256);
     const long long slab = P < DENSITY_SLAB ? P : DENSITY_SLAB;
-    float* raw = pts + density_pts_floats(slab);
+    float* raw = pts + round4(slab * 3);
     NB_CUDA(cudaMemsetAsync(ws, 0, 256, st));
-    const size_t sm = simt_smem_bytes(*net);
-    if (int rc = smem_optin((const void*)mlp_simt_kernel, sm)) return rc;
     for (long long m0 = 0; m0 < P; m0 += slab) {
       const long long M = P - m0 < slab ? P - m0 : slab;
       grid_pts_kernel<<<cdiv(M, 256), 256, 0, st>>>(xs, ys, zs, ny, nz, m0, M, pts);
       NB_LAUNCH_OK("grid_pts_kernel");
-      mlp_simt_kernel<<<cdiv(M, SIMT_ROWS), SIMT_THREADS, sm, st>>>(pts, zero_dir, 0, M, 1, *net, multires, 0, raw, SimtSave{});
-      NB_LAUNCH_OK("mlp_simt_kernel");
+      if (int rc = launch_mlp_simt(pts, zero_dir, 0, M, 1, *net, multires, 0, raw, SimtSave{}, st)) return rc;
       raw_sigma_kernel<<<cdiv(M, 256), 256, 0, st>>>(raw, M, sigma + m0);
       NB_LAUNCH_OK("raw_sigma_kernel");
     }
     return 0;
   }
-  const bool split = precision == NERF_B200_PREC_TC_SPLIT;
-  NB_CHECK_ARG(packed != nullptr, split ? "packed weights are NULL (call nerf_b200_pack_weights_split)" : "packed weights are NULL (call nerf_b200_pack_weights)");
-  DeviceState* ds = device_state();
-  const TilePlan plan = make_tile_plan(N, nz, ds->sms);
-  NB_CHECK_ARG((long long)plan.rays_per_cta * nz < (1ll << 30), "rays_per_cta * S overflows");
-  const PackLayout PL = pack_layout_for(*net, precision);
-  const uint8_t* pk = static_cast<const uint8_t*>(packed);
   MarchParams p;
-  memset(&p, 0, sizeof(p));
-  p.N = N; p.S = nz; p.rays_per_cta = plan.rays_per_cta;
-  p.chunks = pk + PL.off_chunks;
-  p.bias = reinterpret_cast<const float*>(pk + PL.off_bias);
-  p.heads = reinterpret_cast<const float*>(pk + PL.off_heads);
-  p.D = net->D; p.skip = net->skip; p.use_viewdirs = net->use_viewdirs; p.L = multires; p.IC = net->input_ch;
+  PackLayout PL;
+  TilePlan plan;
+  if (int rc = tc_pass_setup(net, packed, precision, multires, N, nz, p, PL, plan)) return rc;
   const DensityGrid g{xs, ys, zs, ny, sigma};
-  if (split) {
-    if (int rc = smem_optin((const void*)density_split_kernel, FWD_ALLOC)) return rc;
-    density_split_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, g, reinterpret_cast<const float*>(pk + PL.off_wscale));
+  if (precision == NERF_B200_PREC_TC_SPLIT) {
+    if (int rc = smem_optin_once((const void*)density_split_kernel, FWD_ALLOC)) return rc;
+    density_split_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, g, reinterpret_cast<const float*>(static_cast<const uint8_t*>(packed) + PL.off_wscale));
     NB_LAUNCH_OK("density_split_kernel");
   } else {
-    if (int rc = smem_optin((const void*)density_wg_kernel, FWD_ALLOC)) return rc;
+    if (int rc = smem_optin_once((const void*)density_wg_kernel, FWD_ALLOC)) return rc;
     density_wg_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, g);
     NB_LAUNCH_OK("density_wg_kernel");
   }
@@ -699,18 +707,14 @@ static int march_impl(const float* rays, const float* z_vals, const float* noise
     NB_CHECK_ARG(save == nullptr, "training-mode records belong to the tensor-core path");
     if (int rc = check_exact_net(net)) return rc;
     const long long M = N * (long long)S;
-    // mlp_simt_kernel stores raw as float4: its scratch starts on a 16-byte boundary whatever M is
-    const size_t pts_floats = ((size_t)M * 3 + 3) & ~(size_t)3;
+    const size_t pts_floats = round4(M * 3);
     const size_t need = pts_floats * 4 + (out->raw ? 0 : (size_t)M * 16);
     NB_CHECK_ARG(workspace && workspace_bytes >= need, "exact-mode workspace too small: need %zu bytes", need);
     float* pts = static_cast<float*>(workspace);
     float* raw = out->raw ? out->raw : pts + pts_floats;
     pts_kernel<<<cdiv(M, 256), 256, 0, st>>>(rays, cfg->ray_stride, z_vals, M, S, pts);
     NB_LAUNCH_OK("pts_kernel");
-    const size_t sm = simt_smem_bytes(*net);
-    if (int rc = smem_optin((const void*)mlp_simt_kernel, sm)) return rc;
-    mlp_simt_kernel<<<cdiv(M, SIMT_ROWS), SIMT_THREADS, sm, st>>>(pts, rays + 8, cfg->ray_stride, M, S, *net, cfg->multires, cfg->multires_views, raw, SimtSave{});
-    NB_LAUNCH_OK("mlp_simt_kernel");
+    if (int rc = launch_mlp_simt(pts, rays + 8, cfg->ray_stride, M, S, *net, cfg->multires, cfg->multires_views, raw, SimtSave{}, st)) return rc;
     raw2outputs_kernel<<<cdiv(N * 32, 256), 256, 0, st>>>(raw, z_vals, rays + 3, cfg->ray_stride, noise, N, S, cfg->white_bkgd, *out);
     NB_LAUNCH_OK("raw2outputs_kernel");
     return 0;
@@ -926,31 +930,26 @@ static int march_bwd_impl(const float* rays, const float* z_vals, const float* n
     const float* ry = rays + n0 * rs;
     const float* zz = z_vals + n0 * S;
     const float* nz = noise ? noise + n0 * S : nullptr;
-    // every one of the BWD_BUFFERS buffers starts on a 16-byte boundary: mlp_simt_kernel stores raw as float4 and
-    // raw2outputs_bwd_kernel loads it so, and neither M * (3 + IC + ICV) nor M * W / 2 need be a multiple of 4 (odd M, W = 4k
-    // with k odd).  The rounding takes at most BWD_BUFFERS * 12 of the workspace's 1024 spare bytes.
+    // every one of the BWD_BUFFERS buffers starts on a 16-byte boundary (round4): neither M * (3 + IC + ICV) nor M * W / 2 need
+    // be a multiple of 4 (odd M, W = 4k with k odd).  The rounding takes at most BWD_BUFFERS * 12 of the workspace's 1024 spare bytes.
     float* p = static_cast<float*>(workspace);
-    auto q4 = [](long long n) { return (n + 3) & ~3ll; };
-    float* pts = p;        p += q4(M * 3);
+    float* pts = p;        p += round4(M * 3);
     SimtSave sv;
-    sv.enc = p;            p += q4(M * IC);
-    sv.encv = p;           p += q4(M * ICV);
-    sv.h = p;              p += q4((long long)D * M * W);
-    sv.feat = p;           p += q4(M * W);
-    sv.hv = p;             p += q4(M * W2);
-    float* raw = p;        p += q4(M * 4);
-    float* d_raw = p;      p += q4(M * 4);
-    float* dh0 = p;        p += q4(M * W);
-    float* dh1 = p;        p += q4(M * W);
-    float* d_hv = p;       p += q4(M * W2);
+    sv.enc = p;            p += round4(M * IC);
+    sv.encv = p;           p += round4(M * ICV);
+    sv.h = p;              p += round4((long long)D * M * W);
+    sv.feat = p;           p += round4(M * W);
+    sv.hv = p;             p += round4(M * W2);
+    float* raw = p;        p += round4(M * 4);
+    float* d_raw = p;      p += round4(M * 4);
+    float* dh0 = p;        p += round4(M * W);
+    float* dh1 = p;        p += round4(M * W);
+    float* d_hv = p;       p += round4(M * W2);
     if (!net->use_viewdirs) { sv.encv = nullptr; sv.feat = nullptr; sv.hv = nullptr; }
     // 1. recompute the pass in fp32 with saved activations
     pts_kernel<<<cdiv(M, 256), 256, 0, st>>>(ry, rs, zz, M, S, pts);
     NB_LAUNCH_OK("pts_kernel");
-    const size_t sm = simt_smem_bytes(*net);
-    NB_TRY(smem_optin((const void*)mlp_simt_kernel, sm));
-    mlp_simt_kernel<<<cdiv(M, SIMT_ROWS), SIMT_THREADS, sm, st>>>(pts, net->use_viewdirs ? ry + 8 : nullptr, rs, M, S, *net, cfg->multires, cfg->multires_views, raw, sv);
-    NB_LAUNCH_OK("mlp_simt_kernel");
+    NB_TRY(launch_mlp_simt(pts, net->use_viewdirs ? ry + 8 : nullptr, rs, M, S, *net, cfg->multires, cfg->multires_views, raw, sv, st));
     // 2. compositing adjoint -> dL/draw
     NB_TRY(raw2outputs_bwd_impl(raw, zz, ry + 3, rs, nz, nn, S, cfg->white_bkgd, seeds_at(g, n0, S), nullptr, d_raw, st));
     const float* h_last = sv.h + (size_t)(D - 1) * M * W;
@@ -1164,6 +1163,25 @@ struct BwdTcPass {
   unsigned int* amax; float *d_raw, *encv, *dsum, *gv, *dbv, *partial; uint8_t* grec; const uint8_t *act, *mask;
   int seed_grid; long long seed_off, views_rays;      // seed kernels: blocks, partial rows from `seed_off`; rays per views block
 
+  // the refusals of a pass, before anything is launched
+  int check() const {
+    NB_CHECK_ARG(rays && z && net && packed && cfg && raw && save && grads, "NULL pointer");
+    NB_CHECK_ARG(cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
+    NB_CHECK_ARG(!seeds_none(seeds), "no output gradient given for a backward pass (g_rgb / every NerfOutGrads member is NULL)");
+    if (int rc = check_tc_net(net)) return rc;
+    NB_CHECK_ARG(net->use_viewdirs || net->output_ch >= 4, "output_linear needs output_ch >= 4 (got %d)", net->output_ch);
+    NB_CHECK_ARG(S > 0, "S must be positive");
+    return 0;
+  }
+
+  int run(void* workspace, size_t workspace_bytes, cudaStream_t st) {
+    NB_TRY(init(workspace, workspace_bytes));
+    NB_TRY(prologue(st));
+    NB_TRY(dgrad(st));
+    NB_TRY(wgrad(st));
+    return heads(st);
+  }
+
   int init(void* workspace, size_t workspace_bytes) {
     ds = device_state();
     plan = make_tile_plan(N, S, ds->sms);
@@ -1196,11 +1214,8 @@ struct BwdTcPass {
     const long long views_floats = net->use_viewdirs ? (long long)sms * (net->input_ch_views + 1) * 128 : 0;
     NB_CHECK_ARG(J.part_floats <= upper && seed_off + seed_floats <= cap && upper + views_floats <= cap,
                  "internal: backward partials exceed the partial region");
-    if (!ds->optin_bwd) {
-      NB_TRY(smem_optin((const void*)dgrad_wg_kernel, SM_ALLOC));
-      NB_TRY(smem_optin((const void*)wgrad_wg_kernel, WG2_TOTAL));
-      ds->optin_bwd = true;
-    }
+    NB_TRY(smem_optin_once((const void*)dgrad_wg_kernel, SM_ALLOC));
+    NB_TRY(smem_optin_once((const void*)wgrad_wg_kernel, WG2_TOTAL));
     return 0;
   }
 
@@ -1244,7 +1259,6 @@ struct BwdTcPass {
 
   // 3. dgrad chain, one CTA per forward CTA (the forward's tile order)
   int dgrad(cudaStream_t st) {
-    const int vc0 = 0, vc1 = plan.grid;
     const int D = net->D;
     const uint8_t* pk = static_cast<const uint8_t*>(packed);
     DgradParams dp;
@@ -1254,21 +1268,13 @@ struct BwdTcPass {
     dp.chunks = pk + PL.off_bwd;
     dp.N = N; dp.S = S; dp.rays_per_cta = plan.rays_per_cta; dp.nst_plan = plan.nst; dp.D = D;
     dp.rec_mask = rec_mask_bytes(D); dp.rec_grad = rec_grad_bytes(D);
-    dp.vc0 = vc0; dp.vc1 = vc1;
+    dp.vc0 = 0; dp.vc1 = plan.grid;                   // every CTA of the plan
     dp.first_step = bwd_first_step(net->use_viewdirs);
-    const int grid = plan.grid;
-    TimedLaunch* tl = nullptr;
-    if (g_timing && g_ntimed < 4096) {
-      tl = &g_timed[g_ntimed++];
-      cudaEventCreate(&tl->a); cudaEventCreate(&tl->b);
-      // MACs per row of the steps the kernel runs: K = W/2 (step 0) + D steps of W x W, or without view directions D - 1 steps
-      const double macs = views ? (double)(net->W / 2) * net->W + (double)D * net->W * net->W : (double)(D - 1) * net->W * net->W;
-      tl->flops = 2.0 * macs * (double)(N * (long long)S) * (double)(vc1 - vc0) / (double)plan.grid;
-      tl->kind = 1;
-      cudaEventRecord(tl->a, st);
-    }
-    dgrad_wg_kernel<<<grid, TC_THREADS, SM_ALLOC, st>>>(dp);
-    if (tl) cudaEventRecord(tl->b, st);
+    // MACs per row of the steps the kernel runs: K = W/2 (step 0) + D steps of W x W, or without view directions D - 1 steps
+    const double macs = views ? (double)(net->W / 2) * net->W + (double)D * net->W * net->W : (double)(D - 1) * net->W * net->W;
+    TimedLaunch* tl = timing_begin(1, 2.0 * macs * (double)(N * (long long)S), st);
+    dgrad_wg_kernel<<<plan.grid, TC_THREADS, SM_ALLOC, st>>>(dp);
+    timing_end(tl, st);
     NB_LAUNCH_OK("dgrad_wg_kernel");
     return 0;
   }
@@ -1276,28 +1282,20 @@ struct BwdTcPass {
   // 4. weight gradients (layer-major) + bias gradients on all SMs, then the reduction of the per-CTA partials (and of the seed
   // kernels' partial rows) in CTA order (adds into the gradient tensors)
   int wgrad(cudaStream_t st) {
-    const int vc0 = 0, vc1 = plan.grid;
     const int D = net->D;
     const bool views = net->use_viewdirs != 0;
     WgradParams wp;
     memset(&wp, 0, sizeof(wp));
     wp.act = act; wp.grad = grec; wp.rec_act = rec_act_bytes(D); wp.rec_grad = rec_grad_bytes(D);
     wp.N = N; wp.S = S; wp.rays_per_cta = plan.rays_per_cta; wp.nst_plan = plan.nst; wp.n_tiles = plan.n_tiles;
-    wp.t0 = (long long)vc0 * plan.nst * 2; wp.t1 = (long long)vc1 * plan.nst * 2;
+    wp.t0 = 0; wp.t1 = (long long)plan.grid * plan.nst * 2;   // every tile of the plan
     wp.partial = partial; wp.d_raw = d_raw; wp.njobs = J.n;
     for (int i = 0; i < J.n; ++i) wp.jobs[i] = J.w[i];
-    TimedLaunch* tl = nullptr;
-    if (g_timing && g_ntimed < 4096) {
-      tl = &g_timed[g_ntimed++];
-      cudaEventCreate(&tl->a); cudaEventCreate(&tl->b);
-      // every Linear but the heads (alpha / rgb_linear and the view columns, or output_linear: other kernels form those)
-      const double heads = views ? (double)net->W + 3.0 * (net->W / 2) + (double)net->input_ch_views * (net->W / 2) : (double)net->W * net->output_ch;
-      tl->flops = 2.0 * (net_macs_per_row(*net) - heads) * (double)(N * (long long)S) * (double)(vc1 - vc0) / (double)plan.grid;
-      tl->kind = 2;
-      cudaEventRecord(tl->a, st);
-    }
+    // every Linear but the heads (alpha / rgb_linear and the view columns, or output_linear: other kernels form those)
+    const double heads = views ? (double)net->W + 3.0 * (net->W / 2) + (double)net->input_ch_views * (net->W / 2) : (double)net->W * net->output_ch;
+    TimedLaunch* tl = timing_begin(2, 2.0 * (net_macs_per_row(*net) - heads) * (double)(N * (long long)S), st);
     wgrad_wg_kernel<<<J.total_ctas, WG2_THREADS, WG2_TOTAL, st>>>(wp);
-    if (tl) cudaEventRecord(tl->b, st);
+    timing_end(tl, st);
     NB_LAUNCH_OK("wgrad_wg_kernel");
     ReduceParams rp;
     memset(&rp, 0, sizeof(rp));
@@ -1337,42 +1335,27 @@ struct BwdTcPass {
   }
 };
 
-// q's seeds: `g` when given, else {rgb_map = q->g_rgb}
-NerfOutGrads pass_seeds(const NerfBwdPass* q, const NerfOutGrads* g) { return g ? *g : rgb_seed(q->g_rgb); }
-
-int check_bwd_pass(const float* rays, const NerfBwdPass* q, const NerfRenderCfg* cfg, const NerfOutGrads* g) {
-  NB_CHECK_ARG(rays && q && q->z_vals && q->net && q->packed && cfg && q->raw && q->save && q->grads, "NULL pointer");
-  NB_CHECK_ARG(cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
-  NB_CHECK_ARG(!seeds_none(pass_seeds(q, g)), "no output gradient given for a backward pass (g_rgb / every NerfOutGrads member is NULL)");
-  if (int rc = check_tc_net(q->net)) return rc;
-  NB_CHECK_ARG(q->net->use_viewdirs || q->net->output_ch >= 4, "output_linear needs output_ch >= 4 (got %d)", q->net->output_ch);
-  NB_CHECK_ARG(q->net->W == 256, "the tensor-core backward supports netwidth == 256");
-  NB_CHECK_ARG(q->S > 0, "S must be positive");
-  return 0;
-}
+// pass q of a render_rays backward (a zero pass, which check() refuses, when q is NULL); its seeds are `g` when given, else
+// {rgb_map = q->g_rgb}
 BwdTcPass bind_pass(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* q, const NerfOutGrads* g) {
   BwdTcPass b;
   memset(&b, 0, sizeof(b));
+  if (!q) return b;
   b.rays = rays; b.z = q->z_vals; b.noise = q->noise; b.N = N; b.S = q->S; b.net = q->net; b.packed = q->packed; b.cfg = cfg;
-  b.raw = q->raw; b.save = q->save; b.seeds = pass_seeds(q, g); b.grads = q->grads;
+  b.raw = q->raw; b.save = q->save; b.seeds = g ? *g : rgb_seed(q->g_rgb); b.grads = q->grads;
   return b;
 }
 
 int march_bwd_tc_impl(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
                       const void* packed, const NerfRenderCfg* cfg, const float* raw, const NerfTrainSave* save,
                       const NerfOutGrads& g, const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
-  NerfBwdPass q;
-  q.z_vals = z_vals; q.noise = noise; q.S = S; q.net = net; q.packed = packed; q.raw = raw; q.save = save; q.g_rgb = g.rgb_map; q.grads = grads;
-  if (int rc = check_bwd_pass(rays, &q, cfg, &g)) return rc;
+  BwdTcPass b;
+  memset(&b, 0, sizeof(b));
+  b.rays = rays; b.z = z_vals; b.noise = noise; b.N = N; b.S = S; b.net = net; b.packed = packed; b.cfg = cfg;
+  b.raw = raw; b.save = save; b.seeds = g; b.grads = grads;
+  NB_TRY(b.check());
   if (N == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  BwdTcPass b = bind_pass(rays, N, cfg, &q, &g);
-  NB_TRY(b.init(workspace, workspace_bytes));
-  NB_TRY(b.prologue(st));
-  NB_TRY(b.dgrad(st));
-  NB_TRY(b.wgrad(st));
-  NB_TRY(b.heads(st));
-  return 0;
+  return b.run(workspace, workspace_bytes, (cudaStream_t)stream);
 }
 }  // namespace
 
@@ -1405,22 +1388,17 @@ size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, con
 static int render_rays_bwd_tc_impl(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse, const NerfBwdPass* fine,
                                    const NerfOutGrads* coarse_g, const NerfOutGrads* fine_g, void* workspace, size_t workspace_bytes,
                                    void* stream) {
-  if (int rc = check_bwd_pass(rays, coarse, cfg, coarse_g)) return rc;
-  if (fine) if (int rc = check_bwd_pass(rays, fine, cfg, fine_g)) return rc;
+  BwdTcPass c = bind_pass(rays, N, cfg, coarse, coarse_g), f = bind_pass(rays, N, cfg, fine, fine_g);
+  NB_TRY(c.check());
+  if (fine) NB_TRY(f.check());
   NB_CHECK_ARG(!fine || (fine->net->use_viewdirs != 0) == (coarse->net->use_viewdirs != 0),
                "coarse and fine networks must agree on use_viewdirs (they share one ray batch)");
   if (N == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  BwdTcPass c = bind_pass(rays, N, cfg, coarse, coarse_g);
   const size_t cb = bwd_pass_bytes(N, coarse->S, coarse->net);
   NB_CHECK_ARG(workspace && workspace_bytes >= cb, "render_rays_bwd_tc workspace too small");
-  NB_TRY(c.init(workspace, cb));
-  NB_TRY(c.prologue(st)); NB_TRY(c.dgrad(st)); NB_TRY(c.wgrad(st)); NB_TRY(c.heads(st));
-  if (!fine) return 0;
-  BwdTcPass f = bind_pass(rays, N, cfg, fine, fine_g);
-  NB_TRY(f.init(static_cast<uint8_t*>(workspace) + cb, workspace_bytes - cb));
-  NB_TRY(f.prologue(st)); NB_TRY(f.dgrad(st)); NB_TRY(f.wgrad(st)); NB_TRY(f.heads(st));
-  return 0;
+  NB_TRY(c.run(workspace, cb, st));
+  return fine ? f.run(static_cast<uint8_t*>(workspace) + cb, workspace_bytes - cb, st) : 0;
 }
 
 int nerf_b200_render_rays_bwd_tc(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse, const NerfBwdPass* fine,

@@ -28,7 +28,7 @@ import torch
 
 from . import _lib
 from . import api
-from ._lib import NerfPassOut, NerfTrainSave, check
+from ._lib import NerfPassOut, check
 
 # The key of the reference's checkpoint dict under which a continuation's extra state goes: {"train_step":
 # FusedTrainStep.state_dict(), "batcher": DeviceRayBatcher.state_dict()}.  The reference's create_nerf reads only its own four
@@ -203,12 +203,12 @@ class FusedTrainStep:
         if cap is not None and all(b[k] is cap[k] for k in b):
             return cap
         o = self.out
-        b["sv_c"] = NerfTrainSave(api._ptr(b["act_c"]), b["act_c"].numel(), api._ptr(b["mask_c"]), b["mask_c"].numel())
+        b["sv_c"] = api._records_save(b["act_c"], b["mask_c"])
         b["bp_c"] = _lib.NerfBwdPass(api._ptr(self.z_c), api._ptr(self.noise0), self.Sc, C.pointer(self._np_c), api._ptr(self._pk_c),
                                      api._ptr(o["raw0"]), C.pointer(b["sv_c"]), api._ptr(o["g_rgb0"]), C.pointer(self._gs[0]))
         b["sv_f"] = b["bp_f"] = None
         if fine:
-            b["sv_f"] = NerfTrainSave(api._ptr(b["act_f"]), b["act_f"].numel(), api._ptr(b["mask_f"]), b["mask_f"].numel())
+            b["sv_f"] = api._records_save(b["act_f"], b["mask_f"])
             b["bp_f"] = _lib.NerfBwdPass(api._ptr(self.z_f), api._ptr(self.noise1), Sf, C.pointer(self._np_f), api._ptr(self._pk_f),
                                          api._ptr(o["raw"]), C.pointer(b["sv_f"]), api._ptr(o["g_rgb"]), C.pointer(self._gs[-1]))
         return b
