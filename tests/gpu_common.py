@@ -89,9 +89,9 @@ def _seed_args(seeds):
     return True, seeds
 
 
-def march_bwd_tc(net, rays, z, raw, act, mask, seeds, L=10, Lv=4, white=True):
+def march_bwd_tc(net, rays, z, raw, act, mask, seeds, L=10, Lv=4, white=True, on_device=False):
     """nerf_b200_march_bwd_tc (seeds: dL/drgb_map [N, 3]) or nerf_b200_march_bwd_tc_outs (seeds: dict output name -> gradient)
-    -> (grads dict name -> np, workspace bytes np from its 1 KB-aligned base)"""
+    -> (grads dict name -> np, workspace bytes np from its 1 KB-aligned base; on_device: a uint8 tensor on the device)"""
     lib = _lib.load()
     N, S = z.shape
     n = net.net_params()
@@ -111,7 +111,7 @@ def march_bwd_tc(net, rays, z, raw, act, mask, seeds, L=10, Lv=4, white=True):
     else:
         _lib.check(lib.nerf_b200_march_bwd_tc_outs(*args, C.byref(s), *tail), "march_bwd_tc_outs")
     torch.cuda.synchronize()
-    return {k: v.cpu().numpy() for k, v in grads.items()}, ws.cpu().numpy()[base:]
+    return {k: v.cpu().numpy() for k, v in grads.items()}, (ws[base:] if on_device else ws.cpu().numpy()[base:])
 
 
 def run_network_exact(net, pts, viewdirs, S, L=10, Lv=4):

@@ -52,12 +52,15 @@ def restate_layout(N, S, D, input_ch_views, sms):
 class Plan:
     """tile plan of one pass: nerf_b200_march_bwd_tc_layout"""
 
-    def __init__(self, lib, N, S, net_params):
-        out = (C.c_int64 * 12)()
-        rc = lib.nerf_b200_march_bwd_tc_layout(N, S, C.byref(net_params), out)
-        assert rc == 0, lib.nerf_b200_last_error()
+    def __init__(self, lib, N, S, net_params, layout=None):
+        """the library's layout, or (lib None) the 12 values given, e.g. restate_layout's"""
+        if layout is None:
+            out = (C.c_int64 * 12)()
+            rc = lib.nerf_b200_march_bwd_tc_layout(N, S, C.byref(net_params), out)
+            assert rc == 0, lib.nerf_b200_last_error()
+            layout = out
         (self.off_draw, self.off_grad, self.rec_act, self.rec_mask, self.rec_grad, self.grid, self.rays_per_cta, self.nst,
-         self.n_tiles, self.off_amax, self.off_dsum, self.off_partial) = [int(v) for v in out]
+         self.n_tiles, self.off_amax, self.off_dsum, self.off_partial) = [int(v) for v in layout]
         self.N, self.S = N, S
 
     def rows_of_tile(self, t):
@@ -90,6 +93,43 @@ def gather_image(buf_u8, plan, rec_bytes, off, Ccols):
         ok = rows >= 0
         out[rows[ok]] = tile[ok]
     return out
+
+
+def plan_row_keep(plan):
+    """bool [len(valid_tiles) * 128]: which rows of the valid tiles, in tile order, are rows of the batch.  The valid tiles of a
+    CTA hold its rows in order and the CTAs follow each other, so the kept rows come out in global row order."""
+    return np.concatenate([plan.rows_of_tile(t) >= 0 for t in plan.valid_tiles()])
+
+
+def _valid_records(buf, plan, rec_bytes, off, nbytes):
+    """uint8 [n_valid, nbytes]: bytes [off, off + nbytes) of every valid tile's record, from a torch uint8 buffer (any device)"""
+    import torch
+    recs = buf[:plan.n_tiles * rec_bytes].view(plan.n_tiles, rec_bytes)
+    valid = torch.as_tensor(plan.valid_tiles(), device=buf.device)
+    return recs[valid, off:off + nbytes]
+
+
+def gather_image_t(buf, plan, rec_bytes, off, Ccols):
+    """gather_image on a torch uint8 buffer, on its device: [M, Ccols] float16 in global row order"""
+    import torch
+    x = _valid_records(buf, plan, rec_bytes, off, 128 * Ccols * 2).contiguous().view(torch.float16)
+    x = x.view(-1, 2, Ccols // 64, 8, 8, 8, 8)                  # [tile][half][K-block][row >> 3][row & 7][16-byte chunk][col & 7]
+    r7 = torch.arange(8, device=buf.device)
+    x = x[:, :, :, :, r7[:, None], r7[:, None] ^ r7[None, :], :]   # logical chunk c of row r sits at (c ^ (r & 7))
+    x = x.permute(0, 1, 3, 4, 2, 5, 6).reshape(-1, Ccols)
+    return x[torch.as_tensor(plan_row_keep(plan), device=buf.device)]
+
+
+def gather_mask_t(buf, plan, layer, D, hv=False):
+    """gather_mask on a torch uint8 buffer, on its device: [M, 256 | 128] bool, True where the pre-activation was positive"""
+    import torch
+    nw = 2 if hv else 4
+    w = _valid_records(buf, plan, plan.rec_mask, D * 4096 if hv else layer * 4096, 2 * 128 * nw * 4).contiguous()
+    w = w.view(torch.int32).view(-1, 2, 128, nw)               # [tile][column half][row][word]
+    sh = 31 - torch.arange(32, device=buf.device, dtype=torch.int32)
+    bits = (w[..., None] >> sh) & 1                            # column (32 b + j) of a word at bit (31 - j)
+    bits = bits.permute(0, 2, 1, 3, 4).reshape(-1, 2 * nw * 32)
+    return bits[torch.as_tensor(plan_row_keep(plan), device=buf.device)] == 0
 
 
 def gather_mask(buf_u8, plan, layer, D, hv=False):

@@ -175,27 +175,34 @@ def _tc_pass(G, net, rays, z, g_rgb, fill):
     return [grads[k] for k in sorted(grads)], ws.cpu().numpy()[base:]
 
 
-def _pass_inputs(G, N, S):
+def _pass_inputs(G, N, S, views=True):
     sb = G.synth.ray_batch("lego", N, seed=2)
-    rays = torch.from_numpy(G.O.pack_rays(400, 400, sb["K"], sb["rays"][0], sb["rays"][1], False, 2., 6., True).astype(np.float32)).to(G.DEV)
+    rays = torch.from_numpy(G.O.pack_rays(400, 400, sb["K"], sb["rays"][0], sb["rays"][1], False, 2., 6., views).astype(np.float32)).to(G.DEV)
     t = torch.linspace(0., 1., S, device=G.DEV)
     z = (rays[:, 6:7] * (1 - t) + rays[:, 7:8] * t).contiguous()
     g = torch.randn((N, 3), device=G.DEV, generator=torch.Generator(G.DEV).manual_seed(S))
     return rays, z, g
 
 
-@pytest.mark.parametrize("N,S", [(4096, 192), (37, 70), (700, 1), (150, 300), (40, 1024)])
-def test_buffer_contents_do_not_matter_and_dsum_is_exact(G, N, S):
-    """0x00- and 0xFF-filled workspace and records give the same gradient bits.  The per-ray sums of d_hv (dsum) equal float64
-    sums of the decoded d_hv images to within fp32 summation error."""
+BUFFER_CASES = [(4096, 192, True), (37, 70, True), (700, 1, True), (150, 300, True), (40, 1024, True), (4096, 192, False)]
+
+
+@pytest.mark.parametrize("N,S,views", BUFFER_CASES, ids=[f"{n}-{s}" + ("" if v else "-noviews") for n, s, v in BUFFER_CASES])
+def test_buffer_contents_do_not_matter_and_dsum_is_exact(G, N, S, views):
+    """0x00- and 0xFF-filled workspace and records give the same gradient bits, with view directions (d_hv seed) and without
+    (dA_seed_output_kernel).  The per-ray sums of d_hv (dsum) equal float64 sums of the decoded d_hv images to within fp32
+    summation error."""
     import tc_records as R
     from nerf_pytorch_b200 import _lib
-    net = G.make_net(G.synth.nerf_state(0))
-    rays, z, g = _pass_inputs(G, N, S)
+    from oracle import noviews
+    net = G.make_net(G.synth.nerf_state(0)) if views else G.make_net(noviews.nerf_state_noviews(0, True), use_viewdirs=False)
+    rays, z, g = _pass_inputs(G, N, S, views)
     ga, ws = _tc_pass(G, net, rays, z, g, 0x00)
     gb, _ = _tc_pass(G, net, rays, z, g, 0xFF)
     assert all(torch.isfinite(x).all() for x in ga)
-    assert_same_bits(ga, gb, f"N={N} S={S} poisoned buffers")
+    assert_same_bits(ga, gb, f"N={N} S={S} views={views} poisoned buffers")
+    if not views:
+        return
     plan = R.Plan(_lib.load(), N, S, net.net_params())
     amax = float(ws[plan.off_amax:plan.off_amax + 4].view(np.float32)[0])
     scale = 2.0 ** np.floor(np.log2(np.float32(2048.0) / np.float32(amax)))
