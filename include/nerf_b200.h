@@ -65,8 +65,11 @@ typedef struct NerfRenderCfg {
 #define NERF_B200_PREC_TC_FP16 0   /* wgmma f16, fp16 operands, fp32 accumulate (fast path)        */
 #define NERF_B200_PREC_FP32    1   /* CUDA-core fp32 FMA chain (exact mode, validation)             */
 #define NERF_B200_PREC_TC_SPLIT 2  /* wgmma f16, each operand split into hi + lo fp16 halves, three  */
-                                   /* MMAs per K-step, fp32 accumulate: fp32-class inference; packed */
-                                   /* by nerf_b200_pack_weights_split; no training-mode records      */
+                                   /* MMAs per K-step, fp32 accumulate: fp32-class inference, packed */
+                                   /* by nerf_b200_pack_weights_split; training through the _split   */
+                                   /* entry points (split records, split backward) on the image of   */
+                                   /* nerf_b200_pack_weights_split_train; the other training entries */
+                                   /* refuse it                                                       */
 
 /* Outputs of one network pass over N rays x S samples.  NULL pointers are skipped. */
 typedef struct NerfPassOut {
@@ -92,6 +95,10 @@ int    nerf_b200_pack_weights(const NerfNetParams* net, void* packed, size_t pac
 /* the scaled weights, the same fp32 tables; no backward stream                                      */
 size_t nerf_b200_packed_bytes_split(const NerfNetParams* net);
 int    nerf_b200_pack_weights_split(const NerfNetParams* net, void* packed, size_t packed_bytes, void* stream);
+/* the split training image: the split image above byte for byte, then the backward's transposed chunks as hi | lo stages of */
+/* the weights under their layer's scale (what nerf_b200_march_bwd_split streams)                                           */
+size_t nerf_b200_packed_bytes_split_train(const NerfNetParams* net);
+int    nerf_b200_pack_weights_split_train(const NerfNetParams* net, void* packed, size_t packed_bytes, void* stream);
 
 /* ---- run_network + batchify + NeRF.forward (run_nerf.py:27-51, run_nerf_helpers.py:96-119) --- */
 /* pts [N*S,3], viewdirs [N,3] (NULL when the net has no view input) -> raw [N*S,4].               */
@@ -259,6 +266,24 @@ int nerf_b200_render_rays_fwd_train(const float* rays, int64_t N, const NerfRend
                                     float* z_fine, float* z_std, const NerfPassOut* fine,
                                     void* workspace, size_t workspace_bytes,
                                     const NerfTrainSave* save_coarse, const NerfTrainSave* save_fine, void* stream);
+/* precision TC_SPLIT in training mode: the same outputs, bit for bit, as the inference call, and SPLIT records -- per tile the
+ * activation record of its hi fp16 images followed by one of their lo halves (lo = fp16(x - hi)); the mask record as above.
+ * `packed` may be the split image or the split training image (the backward needs the latter). */
+int nerf_b200_train_record_bytes_split(int64_t N, int S, const NerfNetParams* net, size_t* act_bytes, size_t* mask_bytes);
+int nerf_b200_march_train_split(const float* rays, const float* z_vals, const float* noise, int64_t N, int S,
+                                const NerfNetParams* net, const void* packed, const NerfRenderCfg* cfg,
+                                const NerfPassOut* out, void* workspace, size_t workspace_bytes,
+                                const NerfTrainSave* save, void* stream);
+int nerf_b200_render_rays_fwd_train_split(const float* rays, int64_t N, const NerfRenderCfg* cfg,
+                                          const NerfNetParams* net_coarse, const void* packed_coarse,
+                                          const NerfNetParams* net_fine, const void* packed_fine,
+                                          const float* t_vals, const float* u_det,
+                                          const float* t_rand, const float* u_rand,
+                                          const float* noise0, const float* noise1,
+                                          float* z_coarse, const NerfPassOut* coarse,
+                                          float* z_fine, float* z_std, const NerfPassOut* fine,
+                                          void* workspace, size_t workspace_bytes,
+                                          const NerfTrainSave* save_coarse, const NerfTrainSave* save_fine, void* stream);
 
 /* ---- backward of one network pass: what loss.backward() (run_nerf.py:775) does through
  *      run_nerf.py:381-386 / :397-403.  dL/dtheta is ACCUMULATED (+=) into fp32 grads laid out like the
@@ -324,6 +349,23 @@ int nerf_b200_render_rays_bwd_tc_outs(const float* rays, int64_t N, const NerfRe
                                       void* workspace, size_t workspace_bytes, void* stream);
 size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, const NerfNetParams* net_coarse, int S_fine,
                                                     const NerfNetParams* net_fine);
+/* split backward (precision TC_SPLIT): the tensor-core backward above on split operands.  Activation gradients are hi + lo
+ * fp16 images under the same power-of-two loss scale, every MMA is hi*hi + hi*lo + lo*hi into an fp32 accumulator, the
+ * dgrad chain streams the split training image's backward chunks and undoes their scale before the ReLU mask, and head /
+ * bias sums read hi + lo in fp32.  It consumes the split records of nerf_b200_march_train_split / render_rays_fwd_train_split
+ * and `packed` = the split training image.  Seeds as the _outs calls (rgb_map alone for an rgb loss). */
+int nerf_b200_march_bwd_split(const float* rays, const float* z_vals, const float* noise, int64_t N, int S,
+                              const NerfNetParams* net, const void* packed, const NerfRenderCfg* cfg,
+                              const float* raw, const NerfTrainSave* save, const NerfOutGrads* g,
+                              const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream);
+size_t nerf_b200_march_bwd_split_workspace_bytes(int64_t N, int S, const NerfNetParams* net);
+/* as nerf_b200_march_bwd_tc_layout; out[2] / out[4] are the per-tile strides of the hi + lo record pairs */
+int nerf_b200_march_bwd_split_layout(int64_t N, int S, const NerfNetParams* net, int64_t* out);
+int nerf_b200_render_rays_bwd_split(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse,
+                                    const NerfBwdPass* fine, const NerfOutGrads* coarse_g, const NerfOutGrads* fine_g,
+                                    void* workspace, size_t workspace_bytes, void* stream);
+size_t nerf_b200_render_rays_bwd_split_workspace_bytes(int64_t N, int S_coarse, const NerfNetParams* net_coarse, int S_fine,
+                                                       const NerfNetParams* net_fine);
 /* exact mode (csrc/bwd_simt.cuh): fp32 recompute with saved activations + fp32 CUDA-core GEMMs; any network
  * the exact forward supports (with or without view directions). */
 int nerf_b200_march_bwd(const float* rays, const float* z_vals, const float* noise, int64_t N, int S,

@@ -76,6 +76,8 @@ SIGNATURES = {
     "nerf_b200_pack_weights": (C.c_int, [C.POINTER(NerfNetParams), c_fp, C.c_size_t, c_fp]),
     "nerf_b200_packed_bytes_split": (C.c_size_t, [C.POINTER(NerfNetParams)]),
     "nerf_b200_pack_weights_split": (C.c_int, [C.POINTER(NerfNetParams), c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_packed_bytes_split_train": (C.c_size_t, [C.POINTER(NerfNetParams)]),
+    "nerf_b200_pack_weights_split_train": (C.c_int, [C.POINTER(NerfNetParams), c_fp, C.c_size_t, c_fp]),
     "nerf_b200_run_network": (C.c_int, [c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp, C.c_int,
                                         C.c_int, C.c_int, c_fp, c_fp, C.c_size_t, c_fp]),
     "nerf_b200_density_grid_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.POINTER(NerfNetParams), C.c_int]),
@@ -133,6 +135,25 @@ SIGNATURES = {
                                                     C.POINTER(NerfBwdPass), C.POINTER(NerfOutGrads), C.POINTER(NerfOutGrads),
                                                     c_fp, C.c_size_t, c_fp]),
     "nerf_b200_render_rays_bwd_tc_workspace_bytes":(C.c_size_t, [C.c_int64, C.c_int, C.POINTER(NerfNetParams), C.c_int, C.POINTER(NerfNetParams)]),
+    "nerf_b200_train_record_bytes_split": (C.c_int, [C.c_int64, C.c_int, C.POINTER(NerfNetParams), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    "nerf_b200_march_train_split": (C.c_int, [c_fp, c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp,
+                                              C.POINTER(NerfRenderCfg), C.POINTER(NerfPassOut), c_fp, C.c_size_t,
+                                              C.POINTER(NerfTrainSave), c_fp]),
+    "nerf_b200_render_rays_fwd_train_split": (C.c_int, [c_fp, C.c_int64, C.POINTER(NerfRenderCfg),
+                                                        C.POINTER(NerfNetParams), c_fp, C.POINTER(NerfNetParams), c_fp,
+                                                        c_fp, c_fp, c_fp, c_fp, c_fp, c_fp,
+                                                        c_fp, C.POINTER(NerfPassOut), c_fp, c_fp, C.POINTER(NerfPassOut),
+                                                        c_fp, C.c_size_t, C.POINTER(NerfTrainSave), C.POINTER(NerfTrainSave), c_fp]),
+    "nerf_b200_march_bwd_split": (C.c_int, [c_fp, c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp,
+                                            C.POINTER(NerfRenderCfg), c_fp, C.POINTER(NerfTrainSave), C.POINTER(NerfOutGrads),
+                                            C.POINTER(NerfNetGrads), c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_march_bwd_split_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.POINTER(NerfNetParams)]),
+    "nerf_b200_march_bwd_split_layout": (C.c_int, [C.c_int64, C.c_int, C.POINTER(NerfNetParams), C.POINTER(C.c_int64)]),
+    "nerf_b200_render_rays_bwd_split": (C.c_int, [c_fp, C.c_int64, C.POINTER(NerfRenderCfg), C.POINTER(NerfBwdPass),
+                                                  C.POINTER(NerfBwdPass), C.POINTER(NerfOutGrads), C.POINTER(NerfOutGrads),
+                                                  c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_render_rays_bwd_split_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.POINTER(NerfNetParams), C.c_int,
+                                                                     C.POINTER(NerfNetParams)]),
     "nerf_b200_march_bwd": (C.c_int, [c_fp, c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp,
                                       C.POINTER(NerfRenderCfg), c_fp, C.POINTER(NerfNetGrads), c_fp, C.c_size_t, c_fp]),
     "nerf_b200_march_bwd_outs": (C.c_int, [c_fp, c_fp, c_fp, C.c_int64, C.c_int, C.POINTER(NerfNetParams), c_fp,

@@ -56,9 +56,11 @@ def get_precision() -> str:
 
 def set_backward(mode: str):
     """'tc' (default in tc_fp16 precision: wgmma backward from the forward's saved tile records, with or without view
-    directions) or 'exact' (fp32 CUDA-core recompute backward; always used in fp32 and tc_split precision: tc_split's forward
-    is the split tensor-core pass, its backward recomputes the pass in fp32 on CUDA cores)."""
-    if mode not in ("tc", "exact"):
+    directions), 'exact' (fp32 CUDA-core recompute backward; always used in fp32 precision, and in tc_split precision unless
+    'tc_split' is selected: the split tensor-core forward, then the pass recomputed in fp32 on CUDA cores) or 'tc_split'
+    (precision tc_split only: the split training forward leaves hi + lo tile records and the backward runs on tensor cores
+    with every operand split into hi + lo fp16 halves; a call that needs gradients in another precision raises)."""
+    if mode not in ("tc", "exact", "tc_split"):
         raise ValueError(mode)
     _PRECISION["backward"] = mode
 
@@ -277,6 +279,11 @@ class NeRF(nn.Module):
         packed() and re-packed on the same conditions."""
         return self._packed_image("_pack_split", "_split")
 
+    def packed_split_train(self):
+        """The split training image of set_backward('tc_split'): packed_split()'s bytes followed by the backward's transposed
+        chunks as hi | lo halves, cached apart from the other images and re-packed on the same conditions."""
+        return self._packed_image("_pack_split_train", "_split_train")
+
     def _packed_image(self, attr, kind):
         dev = self._check_device()
         key = (getattr(self, "_pack_epoch", 0),) + tuple((q.data_ptr(), q._version) for _, _, _, q in self._named_params())
@@ -493,10 +500,12 @@ def _cfg_struct(cfgd, ray_stride):
     return cfg
 
 
-def _train_save(lib, N, S, net_params, dev):
-    """Allocate the per-tile records of one training-mode pass (csrc/train_common.cuh) -> (NerfTrainSave, tensors)."""
+def _train_save(lib, N, S, net_params, dev, split=False):
+    """Allocate the per-tile records of one training-mode pass (csrc/train_common.cuh; split: hi + lo records) ->
+    (NerfTrainSave, tensors)."""
     ab, mb = C.c_size_t(0), C.c_size_t(0)
-    check(lib.nerf_b200_train_record_bytes(N, S, C.byref(net_params), C.byref(ab), C.byref(mb)), "train_record_bytes")
+    sfx = "_split" if split else ""
+    check(getattr(lib, "nerf_b200_train_record_bytes" + sfx)(N, S, C.byref(net_params), C.byref(ab), C.byref(mb)), "train_record_bytes" + sfx)
     act = torch.empty(ab.value, dtype=torch.uint8, device=dev)
     mask = torch.empty(mb.value, dtype=torch.uint8, device=dev)
     return _records_save(act, mask), act, mask
@@ -583,6 +592,14 @@ class _RenderRays(torch.autograd.Function):
         # (the tensor-core backward needs both nets alike with or without view directions: they share the ray batch)
         train_tc = bool(tc and cfgd["want_grad"] and get_backward() == "tc" and
                         (net_f is None or bool(net_f.use_viewdirs) == bool(net_c.use_viewdirs)))
+        # set_backward('tc_split') under tc_split: the split training forward and the split backward (render_rays refused the
+        # mode under the other precisions before any launch)
+        train_split = bool(cfg.precision == PREC_TC_SPLIT and cfgd["want_grad"] and get_backward() == "tc_split")
+        if train_split and net_f is not None and bool(net_f.use_viewdirs) != bool(net_c.use_viewdirs):
+            raise RuntimeError("set_backward('tc_split') needs the coarse and fine networks to agree on use_viewdirs")
+        if train_split:
+            pk_c = net_c.packed_split_train()
+            pk_f = net_f.packed_split_train() if net_f is not None else None
         raw_c = torch.empty((N, Sc, 4), **f32) if ((retraw and not fine) or not tc or train_tc) else None
         out_c = NerfPassOut(_ptr(o["rgb0"]), _ptr(o["disp0"]), _ptr(o["acc0"]), C.c_void_p(0), _ptr(o["w0"]), _ptr(raw_c))
         z_f = z_std = raw_f = None
@@ -602,24 +619,25 @@ class _RenderRays(torch.autograd.Function):
         # render() may have left the construction of this very batch to the prologue launch (_DEFERRED_PACK): take it over here
         gen = _take_deferred_pack(ray_batch)
         with _on(ray_batch):
-            if gen is not None and train_tc:                 # the training-mode entry builds nothing: one extra launch now
+            if gen is not None and (train_tc or train_split):  # the training-mode entry builds nothing: one extra launch now
                 _launch_pack(lib, gen, ray_batch)
                 gen = None
-            if train_tc:
-                sv_c, act_c, mask_c = _train_save(lib, N, Sc, pc, dev)
+            if train_tc or train_split:
+                sv_c, act_c, mask_c = _train_save(lib, N, Sc, pc, dev, train_split)
                 saved_rec = (raw_c, act_c, mask_c)
                 sv_f = None
                 if fine:
-                    sv_f, act_f, mask_f = _train_save(lib, N, Sf, pf if pf is not None else pc, dev)
+                    sv_f, act_f, mask_f = _train_save(lib, N, Sf, pf if pf is not None else pc, dev, train_split)
                     saved_rec += (raw_f, act_f, mask_f)
-                check(lib.nerf_b200_render_rays_fwd_train(*common, C.byref(sv_c), C.byref(sv_f) if sv_f is not None else None,
-                                                          _stream(ray_batch)), "render_rays_fwd_train")
+                sfx = "_split" if train_split else ""
+                check(getattr(lib, "nerf_b200_render_rays_fwd_train" + sfx)(*common, C.byref(sv_c), C.byref(sv_f) if sv_f is not None else None,
+                                                                            _stream(ray_batch)), "render_rays_fwd_train" + sfx)
             elif gen is not None:
                 check(lib.nerf_b200_render_fwd(C.byref(gen[0]), *common, _stream(ray_batch)), "render_fwd")
             else:
                 check(lib.nerf_b200_render_rays_fwd(*common, _stream(ray_batch)), "render_rays_fwd")
         if ctx is not None:
-            ctx.cfgd, ctx.nets, ctx.train_tc = cfgd, (net_c, net_f), train_tc
+            ctx.cfgd, ctx.nets, ctx.train_tc, ctx.train_split = cfgd, (net_c, net_f), train_tc, train_split
             ctx.save_for_backward(ray_batch, z_c, z_f if fine else torch.empty(0, device=dev),
                                   noise0 if noise0 is not None else torch.empty(0, device=dev),
                                   noise1 if noise1 is not None else torch.empty(0, device=dev), *saved_rec)
@@ -652,6 +670,9 @@ class _RenderRays(torch.autograd.Function):
         else:
             s_fine, s_coarse = {}, dict(rgb_map=g[0], disp_map=g[1], acc_map=g[2], raw=g[3])
         rgb_only = not any(v is not None for s in (s_fine, s_coarse) for k, v in s.items() if k != "rgb_map")
+
+        if ctx.train_split:                             # the split backward takes NerfOutGrads only; a pass without one is skipped
+            rgb_only = False
 
         def seed(s):
             if not rgb_only:
@@ -692,6 +713,8 @@ class _RenderRays(torch.autograd.Function):
         def seed_arg(seed):
             return _ptr(seed) if rgb_only else C.byref(seed[0])
         passes, out = _RenderRays._passes(ctx, z_c, z_f, noise0, noise1, rec, seed_f, seed_c)
+        if ctx.train_split:
+            return _RenderRays._backward_split(lib, ray_batch, cfg, passes, out)
         with _on(ray_batch):
             if ctx.train_tc and seed_f is not None and seed_c is not None:
                 # both passes in one call: one after the other on the stream (capi.cu: render_rays_bwd_tc_impl)
@@ -727,6 +750,43 @@ class _RenderRays(torch.autograd.Function):
                                                                     seed_arg(seed), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)),
                           "march_bwd" + sfx)
         return out
+
+
+    @staticmethod
+    def _backward_split(lib, ray_batch, cfg, passes, out):
+        """The split backward (set_backward('tc_split')): both passes in one nerf_b200_render_rays_bwd_split call when both have
+        a seed, else each pass that has one through nerf_b200_march_bwd_split."""
+        N = ray_batch.shape[0]
+        keep, bp, seeds = [], [], []
+        for seed, z, noise, net, gbuf, rc in passes:
+            if seed is None:
+                continue
+            n, gs, sv = _pass_structs(net, gbuf, rc, True)
+            keep += [n, gs, sv, seed]
+            seeds.append(seed)
+            bp.append(_lib.NerfBwdPass(_ptr(z), _ptr(noise if noise.numel() else None), z.shape[1], C.pointer(n),
+                                       _ptr(net.packed_split_train()), _ptr(rc[0]), C.pointer(sv), _ptr(None), C.pointer(gs)))
+        with _on(ray_batch):
+            if len(bp) == 2:
+                ws_bytes = lib.nerf_b200_render_rays_bwd_split_workspace_bytes(N, bp[0].S, bp[0].net, bp[1].S, bp[1].net)
+                ws = _workspace(ws_bytes, ray_batch.device)
+                check(lib.nerf_b200_render_rays_bwd_split(_ptr(ray_batch), N, C.byref(cfg), C.byref(bp[0]), C.byref(bp[1]),
+                                                          C.byref(seeds[0][0]), C.byref(seeds[1][0]), _ptr(ws), ws_bytes,
+                                                          _stream(ray_batch)), "render_rays_bwd_split")
+            for q, seed in zip(bp if len(bp) == 1 else [], seeds):
+                ws_bytes = lib.nerf_b200_march_bwd_split_workspace_bytes(N, q.S, q.net)
+                ws = _workspace(ws_bytes, ray_batch.device)
+                check(lib.nerf_b200_march_bwd_split(_ptr(ray_batch), q.z_vals, q.noise, N, q.S, q.net, q.packed, C.byref(cfg), q.raw,
+                                                    q.save, C.byref(seed[0]), q.grads, _ptr(ws), ws_bytes, _stream(ray_batch)),
+                      "march_bwd_split")
+        return out
+
+
+def _check_split_backward(want_grad):
+    """set_backward('tc_split') trains only in precision tc_split: refuse a call that needs gradients in any other."""
+    if want_grad and get_backward() == "tc_split" and get_precision() != "tc_split":
+        raise RuntimeError(f"set_backward('tc_split') needs precision tc_split (precision is {get_precision()}): "
+                           "call set_precision('tc_split') or set_backward('tc')")
 
 
 def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False, lindisp=False, perturb=0.,
@@ -774,6 +834,7 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
     net_f = network_fine if N_importance > 0 else None          # the reference ignores network_fine without fine samples
     params = [q for _, _, _, q in network_fn._named_params()] + ([q for _, _, _, q in net_f._named_params()] if net_f is not None else [])
     cfgd["want_grad"] = bool(torch.is_grad_enabled() and any(p.requires_grad for p in params))
+    _check_split_backward(cfgd["want_grad"])
     if cfgd["want_grad"]:
         outs = _RenderRays.apply(ray_batch, cfgd, network_fn, net_f, t_rand, u_rand, noise0, noise1, *params)
     else:                                                        # inference: no autograd node to build (saves ~50 us of host time per call)
@@ -837,6 +898,8 @@ def render(H, W, K, chunk=1024 * 32, rays=None, c2w=None, ndc=True, near=0., far
     every mode, `c2w_staticcam` (rays from one camera, view directions from another, :104-107) included; per-ray
     near/far arrays are written into their two columns afterwards."""
     lib = _lib.load()
+    grad_nets = [n for n in (kwargs.get("network_fn"), kwargs.get("network_fine")) if isinstance(n, nn.Module)]
+    _check_split_backward(torch.is_grad_enabled() and any(p.requires_grad for n in grad_nets for p in n.parameters()))
     if get_precision() == "fp32":                  # refuse a net the exact path cannot run before the batch is built
         nets = [kwargs.get("network_fn")] + ([kwargs.get("network_fine")] if kwargs.get("N_importance", 0) > 0 else [])
         for net in nets:

@@ -76,6 +76,13 @@ __global__ void encv_kernel(const float* __restrict__ dirs, int stride, long lon
   out[i] = v;
 }
 
+// {hi, lo} of a split activation gradient: hi = satfinite(x), lo = satfinite(x - hi) (x - hi exact in fp32 unless hi saturated)
+__device__ __forceinline__ void split_sat_f16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  hi = ptx::cvt_sat_f16x2(a, b);
+  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  lo = ptx::cvt_sat_f16x2(a - hf.x, b - hf.y);
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // rgb_linear's backward (run_nerf_helpers.py:114), both halves in one sweep over the rows:
 //   seed of the dgrad chain: d_hv[row][c] = scale * (hv[row][c] > 0) * sum_j d_rgb[row][j] W_rgb[j][c]   (c < 128), written as the
@@ -92,8 +99,10 @@ struct SeedParams {
   float* part;
 };
 
-__global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams p) {
-  __shared__ float s_acc[8][12 * 32 + 3];
+// SPLIT (dhv_seed_heads_split_kernel): hv is read as hi + lo (the lo record rec_split_lo above), d_hv is written as
+// hi = satfinite(x) and lo = satfinite(x - hi) (the lo gradient record rec_grad_split_lo above); the sums take hv = hi + lo.
+template <bool SPLIT>
+__device__ __forceinline__ void dhv_seed_heads_body(const SeedParams& p, float (&s_acc)[8][12 * 32 + 3]) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = lane * 4, ch = lane >> 4, wsel = (lane >> 3) & 1, bit0 = c & 31;
   const float scale = loss_scale_from_absmax(__uint_as_float(*p.amax));
@@ -119,14 +128,16 @@ __global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams
     const int rbase = warp * 16;
     float4 dmine = make_float4(0.f, 0.f, 0.f, 0.f);
     if (lane < 16 && rbase + lane < nv) dmine = reinterpret_cast<const float4*>(p.d_raw)[row_begin + lr0 + rbase + lane];
-    uint2 hw[16];
+    uint2 hw[16], lw[SPLIT ? 16 : 1];
     uint32_t mw[16];
 #pragma unroll
     for (int k = 0; k < 16; ++k) {
       const int r = rbase + k;
       hw[k] = make_uint2(0u, 0u); mw[k] = 0u;
+      if constexpr (SPLIT) lw[k] = make_uint2(0u, 0u);
       if (r < nv) {
         hw[k] = *reinterpret_cast<const uint2*>(hv + img_off(r, c, 128));
+        if constexpr (SPLIT) lw[k] = *reinterpret_cast<const uint2*>(hv + rec_split_lo(p.D) + img_off(r, c, 128));
         mw[k] = *reinterpret_cast<const uint32_t*>(mrec + (uint32_t)r * 8u);
       }
     }
@@ -134,10 +145,14 @@ __global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams
     for (int k = 0; k < 16; ++k) {
       const int r = rbase + k;
       const float dx = __shfl_sync(0xffffffffu, dmine.x, k), dy = __shfl_sync(0xffffffffu, dmine.y, k), dz = __shfl_sync(0xffffffffu, dmine.z, k);
-      uint2 out = make_uint2(0u, 0u);
+      uint2 out = make_uint2(0u, 0u), out_lo = make_uint2(0u, 0u);
       if (r < nv) {
         const __half2 h01 = *reinterpret_cast<const __half2*>(&hw[k].x), h23 = *reinterpret_cast<const __half2*>(&hw[k].y);
-        const float h[4] = {__low2float(h01), __high2float(h01), __low2float(h23), __high2float(h23)};
+        float h[4] = {__low2float(h01), __high2float(h01), __low2float(h23), __high2float(h23)};
+        if constexpr (SPLIT) {
+          const __half2 l01 = *reinterpret_cast<const __half2*>(&lw[k].x), l23 = *reinterpret_cast<const __half2*>(&lw[k].y);
+          h[0] += __low2float(l01); h[1] += __high2float(l01); h[2] += __low2float(l23); h[3] += __high2float(l23);
+        }
         float x[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -145,9 +160,15 @@ __global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams
           x[i] = mask_apply(mw[k], bit0 + i, fmaf(dx, wr[i], fmaf(dy, wg[i], dz * wb[i])));
         }
         b0 += dx; b1 += dy; b2 += dz;
+        if constexpr (SPLIT) {
+          split_sat_f16x2(x[0], x[1], out.x, out_lo.x);
+          split_sat_f16x2(x[2], x[3], out.y, out_lo.y);
+        } else {
         out = make_uint2(ptx::cvt_sat_f16x2(x[0], x[1]), ptx::cvt_sat_f16x2(x[2], x[3]));
+        }
       }
       *reinterpret_cast<uint2*>(g + img_off(r, c, 128)) = out;
+      if constexpr (SPLIT) *reinterpret_cast<uint2*>(g + rec_grad_split_lo(p.D) + img_off(r, c, 128)) = out_lo;
     }
   }
 #pragma unroll
@@ -162,6 +183,16 @@ __global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams
     if (i < 384) { const int j = i / 128, k = (i / 32) & 3, ln = i & 31; o = j * 128 + ln * 4 + k; }
     p.part[(size_t)blockIdx.x * SEED_HEADS_PART + o] = v;
   }
+}
+
+__global__ void __launch_bounds__(256, 3) dhv_seed_heads_kernel(const SeedParams p) {
+  __shared__ float s_acc[8][12 * 32 + 3];
+  dhv_seed_heads_body<false>(p, s_acc);
+}
+// precision TC_SPLIT: the split records (rec_act / rec_grad = the strides of the hi + lo records)
+__global__ void __launch_bounds__(256, 1) dhv_seed_heads_split_kernel(const SeedParams p) {
+  __shared__ float s_acc[8][12 * 32 + 3];
+  dhv_seed_heads_body<true>(p, s_acc);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -183,8 +214,9 @@ struct SeedOutParams {
 };
 constexpr int SEED_OUT_BATCH = 4;         // rows of a warp whose loads are in flight together
 
-__global__ void __launch_bounds__(256, 2) dA_seed_output_kernel(const SeedOutParams p) {
-  __shared__ float s_acc[8][32 * 32 + 4];
+// SPLIT (dA_seed_output_split_kernel): h_{D-1} read as hi + lo, dA_{D-1} written as hi and lo images (as dhv_seed_heads_body)
+template <bool SPLIT>
+__device__ __forceinline__ void dA_seed_output_body(const SeedOutParams& p, float (&s_acc)[8][32 * 32 + 4]) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = lane * 8, word = (lane >> 4) * 4 + ((lane >> 2) & 3), bit0 = 8 * (lane & 3);
   const float scale = loss_scale_from_absmax(__uint_as_float(*p.amax));
@@ -209,14 +241,16 @@ __global__ void __launch_bounds__(256, 2) dA_seed_output_kernel(const SeedOutPar
     float4 dmine = make_float4(0.f, 0.f, 0.f, 0.f);
     if (lane < 16 && rbase + lane < nv) dmine = reinterpret_cast<const float4*>(p.d_raw)[row_begin + lr0 + rbase + lane];
     for (int r8 = 0; r8 < 16; r8 += SEED_OUT_BATCH) {
-      uint4 hw[SEED_OUT_BATCH];
+      uint4 hw[SEED_OUT_BATCH], lw[SPLIT ? SEED_OUT_BATCH : 1];
       uint32_t mw[SEED_OUT_BATCH];
 #pragma unroll
       for (int k = 0; k < SEED_OUT_BATCH; ++k) {
         const int r = rbase + r8 + k;
         hw[k] = make_uint4(0u, 0u, 0u, 0u); mw[k] = 0u;
+        if constexpr (SPLIT) lw[k] = make_uint4(0u, 0u, 0u, 0u);
         if (r < nv) {
           hw[k] = *reinterpret_cast<const uint4*>(h + img_off(r, c, 256));
+          if constexpr (SPLIT) lw[k] = *reinterpret_cast<const uint4*>(h + rec_split_lo(p.D) + img_off(r, c, 256));
           mw[k] = *reinterpret_cast<const uint32_t*>(mrec + (uint32_t)r * 16u);
         }
       }
@@ -225,14 +259,19 @@ __global__ void __launch_bounds__(256, 2) dA_seed_output_kernel(const SeedOutPar
         const int r = rbase + r8 + k;
         const float d[4] = {__shfl_sync(0xffffffffu, dmine.x, r8 + k), __shfl_sync(0xffffffffu, dmine.y, r8 + k),
                             __shfl_sync(0xffffffffu, dmine.z, r8 + k), __shfl_sync(0xffffffffu, dmine.w, r8 + k)};
-        uint4 out = make_uint4(0u, 0u, 0u, 0u);
+        uint4 out = make_uint4(0u, 0u, 0u, 0u), out_lo = make_uint4(0u, 0u, 0u, 0u);
         if (r < nv) {
           const uint32_t hu[4] = {hw[k].x, hw[k].y, hw[k].z, hw[k].w};
           float x[8];
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             const __half2 hh = *reinterpret_cast<const __half2*>(&hu[q]);
-            const float hv2[2] = {__low2float(hh), __high2float(hh)};
+            float hv2[2] = {__low2float(hh), __high2float(hh)};
+            if constexpr (SPLIT) {
+              const uint32_t lu[4] = {lw[k].x, lw[k].y, lw[k].z, lw[k].w};
+              const __half2 ll = *reinterpret_cast<const __half2*>(&lu[q]);
+              hv2[0] += __low2float(ll); hv2[1] += __high2float(ll);
+            }
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int i = 2 * q + e;
@@ -243,9 +282,15 @@ __global__ void __launch_bounds__(256, 2) dA_seed_output_kernel(const SeedOutPar
           }
 #pragma unroll
           for (int kk = 0; kk < 4; ++kk) b[kk] += d[kk];
+          if constexpr (SPLIT) {
+            split_sat_f16x2(x[0], x[1], out.x, out_lo.x); split_sat_f16x2(x[2], x[3], out.y, out_lo.y);
+            split_sat_f16x2(x[4], x[5], out.z, out_lo.z); split_sat_f16x2(x[6], x[7], out.w, out_lo.w);
+          } else {
           out = make_uint4(ptx::cvt_sat_f16x2(x[0], x[1]), ptx::cvt_sat_f16x2(x[2], x[3]), ptx::cvt_sat_f16x2(x[4], x[5]), ptx::cvt_sat_f16x2(x[6], x[7]));
+          }
         }
         *reinterpret_cast<uint4*>(g + img_off(r, c, 256)) = out;
+        if constexpr (SPLIT) *reinterpret_cast<uint4*>(g + rec_grad_split_lo(p.D) + img_off(r, c, 256)) = out_lo;
       }
     }
   }
@@ -263,6 +308,16 @@ __global__ void __launch_bounds__(256, 2) dA_seed_output_kernel(const SeedOutPar
     if (i < 1024) { const int k = i >> 8, e = (i >> 5) & 7, ln = i & 31; o = k * 256 + ln * 8 + e; }
     p.part[(size_t)blockIdx.x * SEED_OUT_PART + o] = v;
   }
+}
+
+__global__ void __launch_bounds__(256, 2) dA_seed_output_kernel(const SeedOutParams p) {
+  __shared__ float s_acc[8][32 * 32 + 4];
+  dA_seed_output_body<false>(p, s_acc);
+}
+// precision TC_SPLIT: the split records (rec_act / rec_grad = the strides of the hi + lo records)
+__global__ void __launch_bounds__(256, 1) dA_seed_output_split_kernel(const SeedOutParams p) {
+  __shared__ float s_acc[8][32 * 32 + 4];
+  dA_seed_output_body<true>(p, s_acc);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -284,18 +339,35 @@ struct DgradParams {
   int first_step;                           // 0: d_hv seed (view directions), 2: dA_{D-1} seed (output_linear head)
 };
 
-__global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradParams p) {
+// The split chain (dgrad_split_kernel, precision TC_SPLIT): every operand is a hi and a lo fp16 image.  Its map: the hi A operands
+// at 0, alpha_linear.weight and the barriers in the 16 KB above them, the lo A operands SPLIT_LO above the hi ones (the split
+// forward's offset), then a ring of DS_NST stages of [N = 256 x K = 16] hi | lo columns (the split packed image's backward stream).
+// The seed goes straight into the A operands (hi and lo), as the fp16 chain's dA_{D-1} seed does.
+constexpr int DS_NST = 5;
+constexpr uint32_t DS_ALPHA = 65536;                             // alpha_linear.weight, 1 KB
+constexpr uint32_t DS_BARS = DS_ALPHA + 1024;                    // full, empty [DS_NST], seed [2]
+constexpr uint32_t DS_WRING = SPLIT_LO + 65536;                  // 147456
+constexpr uint32_t DS_ALLOC = DS_WRING + DS_NST * TC_STAGE_BYTES;   // 229376
+static_assert(DS_BARS + 16 * DS_NST + 16 <= SPLIT_LO && DS_ALLOC <= 227 * 1024, "the split chain's shared-memory map");
+
+// layer of the forward whose (transposed) weights step j multiplies by: the view layer, feature_linear, pts_linears[D + 1 - j]
+__host__ __device__ __forceinline__ int bwd_step_layer(int j, int D) { return j == 0 ? D + 1 : D + 1 - j; }
+
+template <bool SPLIT>
+__device__ __forceinline__ void dgrad_chain(const DgradParams& p, const float* wscale) {
+  constexpr int NST = SPLIT ? DS_NST : TC_NST;
   uint8_t* smem = tc_smem;
   const uint32_t sb = ptx::smem_u32(smem);
   if ((sb & 1023u) != 0) __trap();
-  float* s_alpha = reinterpret_cast<float*>(smem + SM_HEADS);
+  float* s_alpha = reinterpret_cast<float*>(smem + (SPLIT ? DS_ALPHA : SM_HEADS));
   const int D = p.D, NS = D + 1, j0 = p.first_step;
-  Ring rg{sb + SM_BARS, sb + SM_BARS + 8 * TC_NST, 0, 0};
-  const uint32_t bar_seed = sb + SM_BARS + 16 * TC_NST;          // [2]: one per MMA warpgroup
+  const uint32_t bars = sb + (SPLIT ? DS_BARS : SM_BARS);
+  RingN<NST> rg{bars, bars + 8 * NST, 0, 0};
+  const uint32_t bar_seed = bars + 16 * NST;                     // [2]: one per MMA warpgroup
   if (j0 == 0)
     for (int i = threadIdx.x; i < 256; i += TC_THREADS) s_alpha[i] = p.alpha_w[i];
   if (threadIdx.x == 0) {
-    for (int i = 0; i < TC_NST; ++i) { ptx::mbar_init(rg.full + 8 * i, 1); ptx::mbar_init(rg.empty + 8 * i, 256); }
+    for (int i = 0; i < NST; ++i) { ptx::mbar_init(rg.full + 8 * i, 1); ptx::mbar_init(rg.empty + 8 * i, 256); }
     ptx::mbar_init(bar_seed, 1); ptx::mbar_init(bar_seed + 8, 1);
     ptx::fence_mbar_init();
   }
@@ -309,10 +381,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
         for (int tile = 0, nt = 2 * plan_cta_nst(p.N, p.S, p.rays_per_cta, vc); tile < nt; ++tile) {
           const uint8_t* src = p.chunks;
           for (int j = j0; j < NS; ++j)
-            for (int u = 0; u < bwd_step_units(j); ++u) {
+            for (int u = 0; u < bwd_step_units(j) * (SPLIT ? 2 : 1); ++u) {
               ptx::mbar_wait(rg.empty + 8 * rg.stage, rg.phase ^ 1);
               ptx::mbar_arrive_expect_tx(rg.full + 8 * rg.stage, TC_STAGE_BYTES);
-              ptx::bulk_g2s(sb + SM_WRING + rg.stage * TC_STAGE_BYTES, src, TC_STAGE_BYTES, rg.full + 8 * rg.stage);
+              ptx::bulk_g2s(sb + (SPLIT ? DS_WRING : SM_WRING) + rg.stage * TC_STAGE_BYTES, src, TC_STAGE_BYTES, rg.full + 8 * rg.stage);
               src += TC_STAGE_BYTES;
               rg.advance();
             }
@@ -326,8 +398,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
   const int w = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
   const int q4 = lane & 3;
   const int r0 = 16 * wq + (lane >> 2), r1 = r0 + 8;
-  const uint32_t act = sb + SM_ACT + (uint32_t)w * 32768u, seed = sb + SM_ENC + (uint32_t)w * 16384u;
-  const uint32_t ring = sb + SM_WRING;
+  const uint32_t act = sb + SM_ACT + (uint32_t)w * 32768u, seed = SPLIT ? act : sb + SM_ENC + (uint32_t)w * 16384u;
+  const uint32_t ring = sb + (SPLIT ? DS_WRING : SM_WRING);
+  const uint32_t glo = SPLIT ? rec_grad_split_lo(D) : 0u;       // the lo gradient record above the hi one
   const float scale = loss_scale_from_absmax(__uint_as_float(*p.amax));
   const uint64_t l2_first = ptx::l2_policy_evict_first();
   auto wg_sync = [&]() { ptx::named_bar_sync(1 + w, 128); };
@@ -335,6 +408,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
   auto pair_addr = [&](uint32_t ro, int r, int j) { return act + ro + (uint32_t)(j >> 3) * 8192u + (uint32_t)(((j & 7) ^ (r & 7)) << 4); };
   uint32_t sph = 0;
   float acc[128];
+  Phases none;
   for (int vc = p.vc0 + (int)blockIdx.x; vc < p.vc1; vc += (int)gridDim.x) {
     const int nrows = plan_cta_rows(p.N, p.S, p.rays_per_cta, vc);
     const int nt = 2 * plan_cta_nst(p.N, p.S, p.rays_per_cta, vc);
@@ -346,9 +420,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
       uint8_t* const grec = p.grad + (size_t)tid * p.rec_grad;
       const int lrb = st * TC_ST + X * TC_TILE + 64 * w;
       // the warpgroup's 64 rows of the seed (the MMAs of the previous tile's step 0 have read the buffer); a dA_{D-1} seed goes
-      // to the A operand, once the previous tile's last record copy has read it
+      // to the A operand, once the previous tile's last record copy has read it.  SPLIT: both seeds go to the A operands (hi, lo).
       if (t == 0) {
-        if (j0 == 0) {
+        if constexpr (SPLIT) {
+          const uint32_t sbytes = j0 == 0 ? 16384u : 32768u;
+          const uint8_t* src = grec + (j0 == 0 ? (uint32_t)w * 16384u : rec_grad_step(1) + (uint32_t)w * 32768u);
+          ptx::bulk_wait_read0();
+          ptx::mbar_arrive_expect_tx(bar_seed + 8 * w, 2 * sbytes);
+          ptx::bulk_g2s(act, src, sbytes, bar_seed + 8 * w);
+          ptx::bulk_g2s(act + SPLIT_LO, src + glo, sbytes, bar_seed + 8 * w);
+        } else if (j0 == 0) {
           ptx::mbar_arrive_expect_tx(bar_seed + 8 * w, 16384u);
           ptx::bulk_g2s(seed, grec + (uint32_t)w * 16384u, 16384u, bar_seed + 8 * w);
         } else {
@@ -377,13 +458,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
             mk[h][ch] = (j >= 1) ? *reinterpret_cast<const uint4*>(mrec + (uint32_t)(D - j) * 4096u + (uint32_t)ch * 2048u + (uint32_t)(64 * w + (h ? r1 : r0)) * 16u)
                                  : make_uint4(0u, 0u, 0u, 0u);
         const uint32_t abase = (j == 0) ? seed : act;
-        mma_layer(acc, rg, ring, bwd_step_units(j), true, [&](int c) { return desc_act(abase + (uint32_t)(c >> 1) * 8192u + (uint32_t)(c & 1) * 64u); });
+        auto a_of = [&](int c) { return desc_act(abase + (uint32_t)(c >> 1) * 8192u + (uint32_t)(c & 1) * 64u); };
+        float isc = 1.0f;
+        if constexpr (SPLIT) {
+          mma_layer_split(acc, rg, ring, 2 * bwd_step_units(j), true, a_of, none);
+          isc = 1.0f / wscale[bwd_step_layer(j, D)];
+        } else {
+          mma_layer(acc, rg, ring, bwd_step_units(j), true, a_of);
+        }
         if (t == 0) ptx::bulk_wait_read0();                     // the previous step's record copy has read the operand
         wg_sync();
 #pragma unroll
         for (int jj = 0; jj < 32; ++jj) {
           const int c = 8 * jj + 2 * q4;
           float x[2][2] = {{acc[4 * jj], acc[4 * jj + 1]}, {acc[4 * jj + 2], acc[4 * jj + 3]}};
+          if constexpr (SPLIT) {                                // undo the weights' power-of-two scale (exact)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) { x[h][0] *= isc; x[h][1] *= isc; }
+          }
           if (j == 1) {                                         // + d_sigma * alpha_linear.weight (run_nerf_helpers.py:106)
             const float2 a = *reinterpret_cast<const float2*>(s_alpha + c);
 #pragma unroll
@@ -399,19 +491,39 @@ __global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradPara
               x[h][1] = mask_apply(m, (c & 31) + 1, x[h][1]);
             }
           }
+          if constexpr (SPLIT) {
+            uint32_t h0, l0, h1, l1;
+            split_sat_f16x2(x[0][0], x[0][1], h0, l0);
+            split_sat_f16x2(x[1][0], x[1][1], h1, l1);
+            ptx::st_shared_b32(pair_addr(ro0, r0, jj), h0);
+            ptx::st_shared_b32(pair_addr(ro1, r1, jj), h1);
+            ptx::st_shared_b32(pair_addr(ro0, r0, jj) + SPLIT_LO, l0);
+            ptx::st_shared_b32(pair_addr(ro1, r1, jj) + SPLIT_LO, l1);
+          } else {
           ptx::st_shared_b32(pair_addr(ro0, r0, jj), ptx::cvt_sat_f16x2(x[0][0], x[0][1]));
           ptx::st_shared_b32(pair_addr(ro1, r1, jj), ptx::cvt_sat_f16x2(x[1][0], x[1][1]));
+          }
         }
         ptx::fence_proxy_async_smem();
         wg_sync();
         if (t == 0) {
           ptx::bulk_s2g_hint(grec + rec_grad_step(j) + (uint32_t)w * 32768u, act, 32768u, l2_first);
+          if constexpr (SPLIT) ptx::bulk_s2g_hint(grec + glo + rec_grad_step(j) + (uint32_t)w * 32768u, act + SPLIT_LO, 32768u, l2_first);
           ptx::bulk_commit();
         }
       }
     }
   }
   if (t == 0) ptx::bulk_wait_all();
+}
+
+__global__ void __launch_bounds__(TC_THREADS, 1) dgrad_wg_kernel(const DgradParams p) {
+  dgrad_chain<false>(p, nullptr);
+}
+// precision TC_SPLIT: the chain on split operands (three MMAs per K = 16 step), p.chunks = the split training image's backward
+// stream, wscale = its per-layer weight scales, p.rec_grad = the stride of the hi + lo gradient records
+__global__ void __launch_bounds__(TC_THREADS, 1) dgrad_split_kernel(const DgradParams p, const float* __restrict__ wscale) {
+  dgrad_chain<true>(p, wscale);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -607,9 +719,10 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams p)
 // ray's rows through the tile plan in the d_hv seed images (offset 0 of each gradient record).  A ray's rows may span tiles and
 // super-tiles but never CTAs (whole rays per CTA).
 constexpr int DSUM_BATCH = 8;             // rows of a warp whose loads are in flight together
-__global__ void __launch_bounds__(256) dhv_ray_sum_kernel(const uint8_t* __restrict__ grad, uint32_t rec_grad, long long N, int S,
-                                                        int rays_per_cta, int nst_plan, const unsigned int* __restrict__ amax,
-                                                        float* __restrict__ dsum) {
+// SPLIT (dhv_ray_sum_split_kernel): each row is hi + lo (the lo record `lo` bytes above), added in fp32 before the running sum
+template <bool SPLIT>
+__device__ __forceinline__ void dhv_ray_sum_body(const uint8_t* __restrict__ grad, uint32_t rec_grad, uint32_t lo, long long N, int S,
+                                                 int rays_per_cta, int nst_plan, const unsigned int* __restrict__ amax, float* __restrict__ dsum) {
   const long long n = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (n >= N) return;
   const int c = (threadIdx.x & 31) * 4;
@@ -617,22 +730,41 @@ __global__ void __launch_bounds__(256) dhv_ray_sum_kernel(const uint8_t* __restr
   const uint8_t* rec = grad + (size_t)cta * nst_plan * 2 * rec_grad;      // the CTA's tiles: local row lr is in tile lr >> 7
   float s[4] = {0.f, 0.f, 0.f, 0.f};
   for (int k0 = 0; k0 < S; k0 += DSUM_BATCH) {
-    uint2 v[DSUM_BATCH];
+    uint2 v[DSUM_BATCH], vl[SPLIT ? DSUM_BATCH : 1];
 #pragma unroll
     for (int k = 0; k < DSUM_BATCH; ++k) {
       const int lr = lr0 + k0 + k;
       v[k] = (k0 + k < S) ? *reinterpret_cast<const uint2*>(rec + (size_t)(lr >> 7) * rec_grad + img_off(lr & 127, c, 128)) : make_uint2(0u, 0u);
+      if constexpr (SPLIT)
+        vl[k] = (k0 + k < S) ? *reinterpret_cast<const uint2*>(rec + (size_t)(lr >> 7) * rec_grad + lo + img_off(lr & 127, c, 128)) : make_uint2(0u, 0u);
     }
 #pragma unroll
     for (int k = 0; k < DSUM_BATCH; ++k) {
       if (k0 + k < S) {
         const __half2 h01 = *reinterpret_cast<const __half2*>(&v[k].x), h23 = *reinterpret_cast<const __half2*>(&v[k].y);
+        if constexpr (SPLIT) {
+          const __half2 l01 = *reinterpret_cast<const __half2*>(&vl[k].x), l23 = *reinterpret_cast<const __half2*>(&vl[k].y);
+          s[0] += __low2float(h01) + __low2float(l01); s[1] += __high2float(h01) + __high2float(l01);
+          s[2] += __low2float(h23) + __low2float(l23); s[3] += __high2float(h23) + __high2float(l23);
+        } else {
         s[0] += __low2float(h01); s[1] += __high2float(h01); s[2] += __low2float(h23); s[3] += __high2float(h23);
+        }
       }
     }
   }
   const float inv = 1.0f / loss_scale_from_absmax(__uint_as_float(*amax));
   *reinterpret_cast<float4*>(dsum + n * 128 + c) = make_float4(s[0] * inv, s[1] * inv, s[2] * inv, s[3] * inv);
+}
+__global__ void __launch_bounds__(256) dhv_ray_sum_kernel(const uint8_t* __restrict__ grad, uint32_t rec_grad, long long N, int S,
+                                                        int rays_per_cta, int nst_plan, const unsigned int* __restrict__ amax,
+                                                        float* __restrict__ dsum) {
+  dhv_ray_sum_body<false>(grad, rec_grad, 0u, N, S, rays_per_cta, nst_plan, amax, dsum);
+}
+// precision TC_SPLIT: rec_grad = the stride of the hi + lo gradient records, lo = the lo record's offset
+__global__ void __launch_bounds__(256) dhv_ray_sum_split_kernel(const uint8_t* __restrict__ grad, uint32_t rec_grad, uint32_t lo, long long N, int S,
+                                                              int rays_per_cta, int nst_plan, const unsigned int* __restrict__ amax,
+                                                              float* __restrict__ dsum) {
+  dhv_ray_sum_body<true>(grad, rec_grad, lo, N, S, rays_per_cta, nst_plan, amax, dsum);
 }
 
 // Block (e, b) sums over the rays [b R, (b + 1) R): part[b][c][e] = sum dsum[ray][c] * gamma(viewdir_ray)[e] for e < ICV (the view

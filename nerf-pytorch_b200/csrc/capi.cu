@@ -174,11 +174,12 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
   memset(&sv, 0, sizeof(sv));
   if (save) {
     NB_CHECK_ARG(save->act && save->mask, "training-mode save buffers are NULL");
-    NB_CHECK_ARG(save->act_bytes >= (size_t)plan.n_tiles * rec_act_bytes(net->D) && save->mask_bytes >= (size_t)plan.n_tiles * rec_mask_bytes(net->D),
-                 "training-mode save buffers too small (see nerf_b200_train_record_bytes)");
+    const size_t rec_act = (precision == NERF_B200_PREC_TC_SPLIT ? 2 : 1) * (size_t)rec_act_bytes(net->D);   // split: hi + lo records
+    NB_CHECK_ARG(save->act_bytes >= (size_t)plan.n_tiles * rec_act && save->mask_bytes >= (size_t)plan.n_tiles * rec_mask_bytes(net->D),
+                 "training-mode save buffers too small (see nerf_b200_train_record_bytes%s)", precision == NERF_B200_PREC_TC_SPLIT ? "_split" : "");
     NB_CHECK_ARG((reinterpret_cast<uintptr_t>(save->act) & 15) == 0 && (reinterpret_cast<uintptr_t>(save->mask) & 15) == 0, "save buffers must be 16-byte aligned");
     sv.act = static_cast<uint8_t*>(save->act); sv.mask = static_cast<uint8_t*>(save->mask);
-    sv.nst_plan = plan.nst; sv.rec_act = rec_act_bytes(net->D); sv.rec_mask = rec_mask_bytes(net->D);
+    sv.nst_plan = plan.nst; sv.rec_act = (uint32_t)rec_act; sv.rec_mask = rec_mask_bytes(net->D);
   }
   if (net->use_viewdirs && vb_pre != nullptr) {
     p.vb = vb_pre;                                     // the per-ray view-bias table was prepared by ray_setup_kernel
@@ -193,7 +194,7 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
     p.vb = vb;
   }
   const bool split = precision == NERF_B200_PREC_TC_SPLIT;
-  const void* kernel = split ? (const void*)march_split_kernel : !save ? (const void*)march_wg_kernel<false> : (const void*)march_wg_kernel<true>;
+  const void* kernel = split ? (save ? (const void*)march_split_train_kernel : (const void*)march_split_kernel) : !save ? (const void*)march_wg_kernel<false> : (const void*)march_wg_kernel<true>;
   if (int rc = smem_optin_once(kernel, FWD_ALLOC)) return rc;
   TimedLaunch* tl = timing_begin(0, 2.0 * net_macs_per_row(*net) * (double)(N * (long long)S), st);
 #ifdef NERF_B200_PHASE_PROBE
@@ -203,9 +204,11 @@ static int launch_march(const float* rays, int ray_stride, const float* z_vals, 
   }
 #endif
   if (split) {
-    march_split_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, reinterpret_cast<const float*>(pk + PL.off_wscale));
+    const float* wscale = reinterpret_cast<const float*>(pk + PL.off_wscale);
+    if (save) march_split_train_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, sv, wscale);
+    else march_split_kernel<<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, wscale);
     timing_end(tl, st);
-    NB_LAUNCH_OK("march_split_kernel");
+    NB_LAUNCH_OK(save ? "march_split_train_kernel" : "march_split_kernel");
     return 0;
   }
   if (save) march_wg_kernel<true><<<plan.grid, TC_THREADS, FWD_ALLOC, st>>>(p, sv);
@@ -374,6 +377,44 @@ int nerf_b200_pack_weights_split(const NerfNetParams* net, void* packed, size_t 
   pack_chunks_split_kernel<<<dim3(8, job.job.n), 256, 0, st>>>(job, scale, dst);
   NB_LAUNCH_OK("pack_chunks_split_kernel");
   return pack_tables(*net, PL, dst, st);
+}
+
+size_t nerf_b200_packed_bytes_split_train(const NerfNetParams* net) {
+  if (!net || check_tc_net(net)) return 0;
+  return make_pack_layout_split_train(*net).total;
+}
+
+// the split training image (fused_tc.cuh: make_pack_layout_split_train): the split image, then the backward's transposed chunks
+// as hi | lo stages of the weights under their layer's scale (the dgrad chain undoes it in its epilogue)
+int nerf_b200_pack_weights_split_train(const NerfNetParams* net, void* packed, size_t packed_bytes, void* stream) {
+  if (int rc = check_tc_net(net)) return rc;
+  const PackLayout PL = make_pack_layout_split_train(*net);
+  NB_CHECK_ARG(packed && packed_bytes >= PL.total, "packed buffer too small (%zu < %zu)", packed_bytes, PL.total);
+  if (int rc = nerf_b200_pack_weights_split(net, packed, packed_bytes, stream)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* dst = static_cast<uint8_t*>(packed);
+  const int IC = net->input_ch, W = net->W, D = net->D;
+  PackSplitJob bj;
+  memset(&bj, 0, sizeof(bj));
+  unsigned boff = (unsigned)PL.off_bwd;
+  auto addT = [&](const float* src, int ld, int col0, int k0, int layer) {
+    bj.layer[bj.job.n] = (unsigned char)layer;
+    PackChunk& c = bj.job.c[bj.job.n++];
+    c.src = src + col0; c.sn = 1; c.sk = ld; c.k0 = k0; c.kvalid = 32; c.nrows = 256; c.dst_off = boff;
+    boff += 2u * 256u * 64u;
+  };
+  if (net->use_viewdirs) {
+    for (int c = 0; c < 4; ++c) addT(net->views_w, W + net->input_ch_views, 0, 32 * c, D + 1);
+    for (int c = 0; c < 8; ++c) addT(net->feature_w, W, 0, 32 * c, D);
+  }
+  for (int l = D - 1; l >= 1; --l) {
+    const bool sk = (net->skip >= 0 && l == net->skip + 1);
+    for (int c = 0; c < 8; ++c) addT(net->pts_w[l], sk ? W + IC : W, sk ? IC : 0, 32 * c, l);
+  }
+  NB_CHECK_ARG(bj.job.n == bwd_stream_chunks(D, net->use_viewdirs) && boff == PL.off_bwd + PL.bwd_bytes, "internal: split backward chunk table mismatch");
+  pack_chunks_split_kernel<<<dim3(8, bj.job.n), 256, 0, st>>>(bj, reinterpret_cast<const float*>(dst + PL.off_wscale), dst);
+  NB_LAUNCH_OK("pack_chunks_split_kernel (backward stream)");
+  return 0;
 }
 
 int nerf_b200_run_network(const float* pts, const float* viewdirs, int64_t N, int S, const NerfNetParams* net,
@@ -739,6 +780,21 @@ int nerf_b200_march_train(const float* rays, const float* z_vals, const float* n
   return march_impl(rays, z_vals, noise, N, S, net, packed, cfg, out, workspace, workspace_bytes, save, stream);
 }
 
+// precision TC_SPLIT in training mode (march_split_train_kernel): the split records for nerf_b200_march_bwd_split
+int nerf_b200_march_train_split(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                                const void* packed, const NerfRenderCfg* cfg, const NerfPassOut* out, void* workspace,
+                                size_t workspace_bytes, const NerfTrainSave* save, void* stream) {
+  NB_CHECK_ARG(save != nullptr && out && out->raw, "training mode needs the save buffers and out->raw (the compositing adjoint reads raw)");
+  NB_CHECK_ARG(cfg && cfg->precision == NERF_B200_PREC_TC_SPLIT, "the split training forward needs precision TC_SPLIT");
+  return march_impl(rays, z_vals, noise, N, S, net, packed, cfg, out, workspace, workspace_bytes, save, stream);
+}
+
+int nerf_b200_train_record_bytes_split(int64_t N, int S, const NerfNetParams* net, size_t* act_bytes, size_t* mask_bytes) {
+  if (int rc = nerf_b200_train_record_bytes(N, S, net, act_bytes, mask_bytes)) return rc;
+  if (act_bytes) *act_bytes *= 2;
+  return 0;
+}
+
 int nerf_b200_train_record_bytes(int64_t N, int S, const NerfNetParams* net, size_t* act_bytes, size_t* mask_bytes) {
   if (int rc = check_tc_net(net)) return rc;
   NB_CHECK_ARG(N >= 0 && S >= 1, "bad N / S");
@@ -856,6 +912,19 @@ int nerf_b200_render_rays_fwd_train(const float* rays, int64_t N, const NerfRend
                                     size_t workspace_bytes, const NerfTrainSave* save_coarse, const NerfTrainSave* save_fine, void* stream) {
   NB_CHECK_ARG(cfg && cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
   NB_CHECK_ARG(cfg && cfg->precision == NERF_B200_PREC_TC_FP16, "training-mode records belong to the tensor-core path");
+  NB_CHECK_ARG(save_coarse && coarse && coarse->raw, "training mode needs save_coarse and coarse->raw");
+  NB_CHECK_ARG(cfg->N_importance == 0 || (save_fine && fine && fine->raw), "training mode needs save_fine and fine->raw");
+  return render_rays_fwd_impl(rays, N, cfg, net_coarse, packed_coarse, net_fine, packed_fine, t_vals, u_det, t_rand, u_rand, noise0, noise1,
+                              z_coarse, coarse, z_fine, z_std, fine, workspace, workspace_bytes, save_coarse, save_fine, stream);
+}
+
+int nerf_b200_render_rays_fwd_train_split(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfNetParams* net_coarse,
+                                          const void* packed_coarse, const NerfNetParams* net_fine, const void* packed_fine,
+                                          const float* t_vals, const float* u_det, const float* t_rand, const float* u_rand,
+                                          const float* noise0, const float* noise1, float* z_coarse, const NerfPassOut* coarse,
+                                          float* z_fine, float* z_std, const NerfPassOut* fine, void* workspace,
+                                          size_t workspace_bytes, const NerfTrainSave* save_coarse, const NerfTrainSave* save_fine, void* stream) {
+  NB_CHECK_ARG(cfg && cfg->precision == NERF_B200_PREC_TC_SPLIT, "the split training forward needs precision TC_SPLIT");
   NB_CHECK_ARG(save_coarse && coarse && coarse->raw, "training mode needs save_coarse and coarse->raw");
   NB_CHECK_ARG(cfg->N_importance == 0 || (save_fine && fine && fine->raw), "training mode needs save_fine and fine->raw");
   return render_rays_fwd_impl(rays, N, cfg, net_coarse, packed_coarse, net_fine, packed_fine, t_vals, u_det, t_rand, u_rand, noise0, noise1,
@@ -1111,7 +1180,8 @@ BwdTcJobs make_bwd_jobs(const NerfNetParams& n, const NerfNetGrads* g, int sms) 
   return J;
 }
 
-BwdTcLayout make_bwd_layout(long long N, int S, const NerfNetParams& n, const TilePlan& plan, long long part_floats) {
+// split: the gradient records are the split backward's hi + lo pairs
+BwdTcLayout make_bwd_layout(long long N, int S, const NerfNetParams& n, const TilePlan& plan, long long part_floats, bool split = false) {
   BwdTcLayout L;
   auto up = [](size_t x) { return (x + 1023) & ~(size_t)1023; };
   size_t o = 0;
@@ -1121,16 +1191,16 @@ BwdTcLayout make_bwd_layout(long long N, int S, const NerfNetParams& n, const Ti
   L.off_dsum = o;    o = up(o + (size_t)N * 128 * 4);
   L.off_gv = o;      o = up(o + (size_t)(128 * 256 + 128) * 4);      // G = d_hv^T h_{D-1} (reduced) and this pass's db_v
   L.off_partial = o; o = up(o + (size_t)part_floats * 4);
-  L.off_grad = o;    o = up(o + (size_t)plan.n_tiles * rec_grad_bytes(n.D));
+  L.off_grad = o;    o = up(o + (size_t)plan.n_tiles * rec_grad_bytes(n.D) * (split ? 2 : 1));
   L.total = o; L.part_floats = part_floats;
   return L;
 }
 }  // namespace
 
-static size_t bwd_pass_bytes(int64_t N, int S, const NerfNetParams* net) {
+static size_t bwd_pass_bytes(int64_t N, int S, const NerfNetParams* net, bool split = false) {
   const int sms = num_sms();
   const TilePlan plan = make_tile_plan(N, S, sms);
-  return make_bwd_layout(N, S, *net, plan, (long long)sms * 256 * 256).total + 1024;
+  return make_bwd_layout(N, S, *net, plan, (long long)sms * 256 * 256, split).total + 1024;
 }
 
 size_t nerf_b200_march_bwd_tc_workspace_bytes(int64_t N, int S, const NerfNetParams* net) {
@@ -1141,17 +1211,22 @@ size_t nerf_b200_march_bwd_tc_workspace_bytes(int64_t N, int S, const NerfNetPar
 // introspection for tests and tools: where nerf_b200_march_bwd_tc keeps its intermediates inside the (1 KB-aligned)
 // workspace and how the tiles are laid out.  out[0..11] = off_d_raw, off_grad_records, rec_act_bytes, rec_mask_bytes,
 // rec_grad_bytes, grid, rays_per_cta, nst, n_tiles, off_amax, off_dsum, off_partial
-int nerf_b200_march_bwd_tc_layout(int64_t N, int S, const NerfNetParams* net, int64_t* out) {
+static int bwd_layout(int64_t N, int S, const NerfNetParams* net, int64_t* out, bool split) {
   if (int rc = check_tc_net(net)) return rc;
   NB_CHECK_ARG(out && N > 0 && S > 0, "bad arguments");
   const int sms = num_sms();
   const TilePlan plan = make_tile_plan(N, S, sms);
-  const BwdTcLayout LY = make_bwd_layout(N, S, *net, plan, (long long)sms * 256 * 256);
-  out[0] = (int64_t)LY.off_draw; out[1] = (int64_t)LY.off_grad; out[2] = rec_act_bytes(net->D); out[3] = rec_mask_bytes(net->D);
-  out[4] = rec_grad_bytes(net->D); out[5] = plan.grid; out[6] = plan.rays_per_cta; out[7] = plan.nst; out[8] = plan.n_tiles;
+  const BwdTcLayout LY = make_bwd_layout(N, S, *net, plan, (long long)sms * 256 * 256, split);
+  const int64_t m = split ? 2 : 1;
+  out[0] = (int64_t)LY.off_draw; out[1] = (int64_t)LY.off_grad; out[2] = m * rec_act_bytes(net->D); out[3] = rec_mask_bytes(net->D);
+  out[4] = m * rec_grad_bytes(net->D); out[5] = plan.grid; out[6] = plan.rays_per_cta; out[7] = plan.nst; out[8] = plan.n_tiles;
   out[9] = (int64_t)LY.off_amax; out[10] = (int64_t)LY.off_dsum; out[11] = (int64_t)LY.off_partial;
   return 0;
 }
+
+int nerf_b200_march_bwd_tc_layout(int64_t N, int S, const NerfNetParams* net, int64_t* out) { return bwd_layout(N, S, net, out, false); }
+// the same for the split backward: out[2] and out[4] are the strides of the hi + lo record pairs (the lo record follows the hi one)
+int nerf_b200_march_bwd_split_layout(int64_t N, int S, const NerfNetParams* net, int64_t* out) { return bwd_layout(N, S, net, out, true); }
 
 namespace {
 // One pass of the tensor-core backward, in its phases: prologue (loss scale, compositing adjoint, seed tiles), dgrad chain,
@@ -1162,11 +1237,14 @@ struct BwdTcPass {
   DeviceState* ds; TilePlan plan; BwdTcLayout LY; PackLayout PL; BwdTcJobs J;
   unsigned int* amax; float *d_raw, *encv, *dsum, *gv, *dbv, *partial; uint8_t* grec; const uint8_t *act, *mask;
   int seed_grid; long long seed_off, views_rays;      // seed kernels: blocks, partial rows from `seed_off`; rays per views block
+  bool split;                                         // the split backward (precision TC_SPLIT, split records and image)
+  uint32_t ract, rgrad;                               // per-tile strides of the activation and gradient records
 
   // the refusals of a pass, before anything is launched
   int check() const {
     NB_CHECK_ARG(rays && z && net && packed && cfg && raw && save && grads, "NULL pointer");
-    NB_CHECK_ARG(cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
+    if (split) NB_CHECK_ARG(cfg->precision == NERF_B200_PREC_TC_SPLIT, "the split backward needs precision TC_SPLIT");
+    else NB_CHECK_ARG(cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
     NB_CHECK_ARG(!seeds_none(seeds), "no output gradient given for a backward pass (g_rgb / every NerfOutGrads member is NULL)");
     if (int rc = check_tc_net(net)) return rc;
     NB_CHECK_ARG(net->use_viewdirs || net->output_ch >= 4, "output_linear needs output_ch >= 4 (got %d)", net->output_ch);
@@ -1185,12 +1263,14 @@ struct BwdTcPass {
   int init(void* workspace, size_t workspace_bytes) {
     ds = device_state();
     plan = make_tile_plan(N, S, ds->sms);
-    LY = make_bwd_layout(N, S, *net, plan, (long long)ds->sms * 256 * 256);
+    LY = make_bwd_layout(N, S, *net, plan, (long long)ds->sms * 256 * 256, split);
+    ract = rec_act_bytes(net->D) * (split ? 2u : 1u);
+    rgrad = rec_grad_bytes(net->D) * (split ? 2u : 1u);
     uint8_t* ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~(uintptr_t)1023);
     NB_CHECK_ARG(workspace && workspace_bytes >= LY.total + (size_t)(ws - static_cast<uint8_t*>(workspace)), "march_bwd_tc workspace too small (%zu < %zu)", workspace_bytes, LY.total + 1024);
-    NB_CHECK_ARG(save->act && save->mask && save->act_bytes >= (size_t)plan.n_tiles * rec_act_bytes(net->D) && save->mask_bytes >= (size_t)plan.n_tiles * rec_mask_bytes(net->D),
+    NB_CHECK_ARG(save->act && save->mask && save->act_bytes >= (size_t)plan.n_tiles * ract && save->mask_bytes >= (size_t)plan.n_tiles * rec_mask_bytes(net->D),
                  "training-mode records missing or too small");
-    PL = make_pack_layout(*net);
+    PL = split ? make_pack_layout_split_train(*net) : make_pack_layout(*net);
     amax = reinterpret_cast<unsigned int*>(ws + LY.off_amax);
     d_raw = reinterpret_cast<float*>(ws + LY.off_draw);
     encv = reinterpret_cast<float*>(ws + LY.off_encv);
@@ -1214,7 +1294,8 @@ struct BwdTcPass {
     const long long views_floats = net->use_viewdirs ? (long long)sms * (net->input_ch_views + 1) * 128 : 0;
     NB_CHECK_ARG(J.part_floats <= upper && seed_off + seed_floats <= cap && upper + views_floats <= cap,
                  "internal: backward partials exceed the partial region");
-    NB_TRY(smem_optin_once((const void*)dgrad_wg_kernel, SM_ALLOC));
+    if (split) NB_TRY(smem_optin_once((const void*)dgrad_split_kernel, DS_ALLOC));
+    else NB_TRY(smem_optin_once((const void*)dgrad_wg_kernel, SM_ALLOC));
     NB_TRY(smem_optin_once((const void*)wgrad_wg_kernel, WG2_TOTAL));
     return 0;
   }
@@ -1237,10 +1318,11 @@ struct BwdTcPass {
       SeedOutParams so;
       so.d_raw = d_raw; so.mask = mask; so.act = act; so.grad = grec; so.out_w = net->output_w; so.amax = amax;
       so.N = N; so.S = S; so.rays_per_cta = plan.rays_per_cta; so.nst_plan = plan.nst; so.D = D;
-      so.rec_mask = rec_mask_bytes(D); so.rec_act = rec_act_bytes(D); so.rec_grad = rec_grad_bytes(D); so.n_tiles = plan.n_tiles;
+      so.rec_mask = rec_mask_bytes(D); so.rec_act = ract; so.rec_grad = rgrad; so.n_tiles = plan.n_tiles;
       so.part = partial + seed_off;
-      dA_seed_output_kernel<<<seed_grid, 256, 0, st>>>(so);
-      NB_LAUNCH_OK("dA_seed_output_kernel");
+      if (split) dA_seed_output_split_kernel<<<seed_grid, 256, 0, st>>>(so);
+      else dA_seed_output_kernel<<<seed_grid, 256, 0, st>>>(so);
+      NB_LAUNCH_OK(split ? "dA_seed_output_split_kernel" : "dA_seed_output_kernel");
       J.reduce(seed_off, SEED_OUT_PART, seed_grid, 1024, grads->output_w, 0);
       J.reduce(seed_off + 1024, SEED_OUT_PART, seed_grid, 4, grads->output_b, 0);
       return 0;
@@ -1248,10 +1330,11 @@ struct BwdTcPass {
     SeedParams sp;
     sp.d_raw = d_raw; sp.mask = mask; sp.act = act; sp.grad = grec; sp.rgb_w = net->rgb_w; sp.amax = amax;
     sp.N = N; sp.S = S; sp.rays_per_cta = plan.rays_per_cta; sp.nst_plan = plan.nst; sp.D = D;
-    sp.rec_mask = rec_mask_bytes(D); sp.rec_act = rec_act_bytes(D); sp.rec_grad = rec_grad_bytes(D); sp.n_tiles = plan.n_tiles;
+    sp.rec_mask = rec_mask_bytes(D); sp.rec_act = ract; sp.rec_grad = rgrad; sp.n_tiles = plan.n_tiles;
     sp.part = partial + seed_off;
-    dhv_seed_heads_kernel<<<seed_grid, 256, 0, st>>>(sp);
-    NB_LAUNCH_OK("dhv_seed_heads_kernel");
+    if (split) dhv_seed_heads_split_kernel<<<seed_grid, 256, 0, st>>>(sp);
+    else dhv_seed_heads_kernel<<<seed_grid, 256, 0, st>>>(sp);
+    NB_LAUNCH_OK(split ? "dhv_seed_heads_split_kernel" : "dhv_seed_heads_kernel");
     J.reduce(seed_off, SEED_HEADS_PART, seed_grid, 384, grads->rgb_w, 0);
     J.reduce(seed_off + 384, SEED_HEADS_PART, seed_grid, 3, grads->rgb_b, 0);
     return 0;
@@ -1267,42 +1350,63 @@ struct BwdTcPass {
     dp.d_raw = views ? d_raw : nullptr; dp.alpha_w = views ? net->alpha_w : nullptr;
     dp.chunks = pk + PL.off_bwd;
     dp.N = N; dp.S = S; dp.rays_per_cta = plan.rays_per_cta; dp.nst_plan = plan.nst; dp.D = D;
-    dp.rec_mask = rec_mask_bytes(D); dp.rec_grad = rec_grad_bytes(D);
+    dp.rec_mask = rec_mask_bytes(D); dp.rec_grad = rgrad;
     dp.vc0 = 0; dp.vc1 = plan.grid;                   // every CTA of the plan
     dp.first_step = bwd_first_step(net->use_viewdirs);
     // MACs per row of the steps the kernel runs: K = W/2 (step 0) + D steps of W x W, or without view directions D - 1 steps
     const double macs = views ? (double)(net->W / 2) * net->W + (double)D * net->W * net->W : (double)(D - 1) * net->W * net->W;
     TimedLaunch* tl = timing_begin(1, 2.0 * macs * (double)(N * (long long)S), st);
-    dgrad_wg_kernel<<<plan.grid, TC_THREADS, SM_ALLOC, st>>>(dp);
+    if (split) dgrad_split_kernel<<<plan.grid, TC_THREADS, DS_ALLOC, st>>>(dp, reinterpret_cast<const float*>(pk + PL.off_wscale));
+    else dgrad_wg_kernel<<<plan.grid, TC_THREADS, SM_ALLOC, st>>>(dp);
     timing_end(tl, st);
-    NB_LAUNCH_OK("dgrad_wg_kernel");
+    NB_LAUNCH_OK(split ? "dgrad_split_kernel" : "dgrad_wg_kernel");
     return 0;
   }
 
   // 4. weight gradients (layer-major) + bias gradients on all SMs, then the reduction of the per-CTA partials (and of the seed
-  // kernels' partial rows) in CTA order (adds into the gradient tensors)
+  // kernels' partial rows) in CTA order (adds into the gradient tensors).  Split: dW = dA_hi^T H_hi + dA_lo^T H_hi + dA_hi^T H_lo
+  // as three launches of the same kernel on the hi and lo records, each reduced (added into the tensors) before the next
+  // reuses the partial region; the bias sums take dA_hi then dA_lo, alpha_linear's weight H_hi then H_lo (its bias, the sum of
+  // d_sigma, once: from the first launch).
   int wgrad(cudaStream_t st) {
+    if (!split) return wgrad_launch(act, grec, 0, J.nr, true, true, st);
+    const int nd = J.n, ndb = [&] { int k = 0; for (int i = 0; i < J.n; ++i) k += J.w[i].db_off >= 0; return k; }();
+    const int na = (net->use_viewdirs && grads) ? 1 : 0;             // alpha_linear.weight's reduction (its bias's follows it)
+    NB_TRY(wgrad_launch(act, grec, 0, J.nr, true, true, st));                                               // hi, hi (+ seed heads)
+    NB_TRY(wgrad_launch(act, grec + rec_grad_split_lo(net->D), nd, nd + ndb, true, false, st));              // lo dA, hi H
+    return wgrad_launch(act + rec_split_lo(net->D), grec, nd + ndb, nd + ndb + na, false, true, st);        // hi dA, lo H
+  }
+
+  // one weight-gradient launch on the records at a / g and its reduction: the dW jobs, then J.r[r0, r1) (every reduction when
+  // r1 = J.nr); `db` / `alpha`: the launch forms the bias sums / alpha_linear's partials
+  int wgrad_launch(const uint8_t* a, const uint8_t* g, int r0, int r1, bool db, bool alpha, cudaStream_t st) {
     const int D = net->D;
     const bool views = net->use_viewdirs != 0;
     WgradParams wp;
     memset(&wp, 0, sizeof(wp));
-    wp.act = act; wp.grad = grec; wp.rec_act = rec_act_bytes(D); wp.rec_grad = rec_grad_bytes(D);
+    wp.act = a; wp.grad = g; wp.rec_act = ract; wp.rec_grad = rgrad;
     wp.N = N; wp.S = S; wp.rays_per_cta = plan.rays_per_cta; wp.nst_plan = plan.nst; wp.n_tiles = plan.n_tiles;
     wp.t0 = 0; wp.t1 = (long long)plan.grid * plan.nst * 2;   // every tile of the plan
     wp.partial = partial; wp.d_raw = d_raw; wp.njobs = J.n;
-    for (int i = 0; i < J.n; ++i) wp.jobs[i] = J.w[i];
+    for (int i = 0; i < J.n; ++i) {
+      wp.jobs[i] = J.w[i];
+      if (!db) wp.jobs[i].db_off = -1;
+      if (!alpha) wp.jobs[i].alpha_off = -1;
+    }
     // every Linear but the heads (alpha / rgb_linear and the view columns, or output_linear: other kernels form those)
     const double heads = views ? (double)net->W + 3.0 * (net->W / 2) + (double)net->input_ch_views * (net->W / 2) : (double)net->W * net->output_ch;
-    TimedLaunch* tl = timing_begin(2, 2.0 * (net_macs_per_row(*net) - heads) * (double)(N * (long long)S), st);
+    const bool first = a == act && g == grec;         // the algorithmic work is counted once per pass
+    TimedLaunch* tl = timing_begin(2, first ? 2.0 * (net_macs_per_row(*net) - heads) * (double)(N * (long long)S) : 0.0, st);
     wgrad_wg_kernel<<<J.total_ctas, WG2_THREADS, WG2_TOTAL, st>>>(wp);
     timing_end(tl, st);
-    NB_LAUNCH_OK("wgrad_wg_kernel");
+    NB_LAUNCH_OK(split ? "wgrad_wg_kernel (split record pair)" : "wgrad_wg_kernel");
     ReduceParams rp;
     memset(&rp, 0, sizeof(rp));
-    rp.partial = partial; rp.amax = amax; rp.njobs = J.nr;
     if (views) J.r[0].dst = gv;                       // job 0 reduces into the scratch block G
-    for (int i = 0; i < J.nr; ++i) rp.jobs[i] = J.r[i];
-    dim3 rg(128, J.nr);
+    rp.partial = partial; rp.amax = amax; rp.njobs = 0;
+    for (int i = 0; i < J.nr; ++i)
+      if (i < J.n || (i >= r0 && i < r1)) rp.jobs[rp.njobs++] = J.r[i];
+    dim3 rg(128, rp.njobs);
     wgrad_reduce_kernel<<<rg, 256, 0, st>>>(rp);
     NB_LAUNCH_OK("wgrad_reduce_kernel");
     return 0;
@@ -1314,8 +1418,9 @@ struct BwdTcPass {
     const int ICV = net->input_ch_views;
     encv_kernel<<<cdiv(N * ICV, 256), 256, 0, st>>>(rays + 8, cfg->ray_stride, N, ICV, encv);
     NB_LAUNCH_OK("encv_kernel");
-    dhv_ray_sum_kernel<<<cdiv(N, 8), 256, 0, st>>>(grec, rec_grad_bytes(net->D), N, S, plan.rays_per_cta, plan.nst, amax, dsum);
-    NB_LAUNCH_OK("dhv_ray_sum_kernel");
+    if (split) dhv_ray_sum_split_kernel<<<cdiv(N, 8), 256, 0, st>>>(grec, rgrad, rec_grad_split_lo(net->D), N, S, plan.rays_per_cta, plan.nst, amax, dsum);
+    else dhv_ray_sum_kernel<<<cdiv(N, 8), 256, 0, st>>>(grec, rgrad, N, S, plan.rays_per_cta, plan.nst, amax, dsum);
+    NB_LAUNCH_OK(split ? "dhv_ray_sum_split_kernel" : "dhv_ray_sum_kernel");
     const int sms = ds->sms;
     const long long voff = (long long)sms * 128 * 256;  // the upper half of the partial region: reduced already (stream order)
     dim3 vg(ICV + 1, sms);
@@ -1337,9 +1442,10 @@ struct BwdTcPass {
 
 // pass q of a render_rays backward (a zero pass, which check() refuses, when q is NULL); its seeds are `g` when given, else
 // {rgb_map = q->g_rgb}
-BwdTcPass bind_pass(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* q, const NerfOutGrads* g) {
+BwdTcPass bind_pass(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* q, const NerfOutGrads* g, bool split) {
   BwdTcPass b;
   memset(&b, 0, sizeof(b));
+  b.split = split;
   if (!q) return b;
   b.rays = rays; b.z = q->z_vals; b.noise = q->noise; b.N = N; b.S = q->S; b.net = q->net; b.packed = q->packed; b.cfg = cfg;
   b.raw = q->raw; b.save = q->save; b.seeds = g ? *g : rgb_seed(q->g_rgb); b.grads = q->grads;
@@ -1348,9 +1454,11 @@ BwdTcPass bind_pass(const float* rays, int64_t N, const NerfRenderCfg* cfg, cons
 
 int march_bwd_tc_impl(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
                       const void* packed, const NerfRenderCfg* cfg, const float* raw, const NerfTrainSave* save,
-                      const NerfOutGrads& g, const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
+                      const NerfOutGrads& g, const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream,
+                      bool split = false) {
   BwdTcPass b;
   memset(&b, 0, sizeof(b));
+  b.split = split;
   b.rays = rays; b.z = z_vals; b.noise = noise; b.N = N; b.S = S; b.net = net; b.packed = packed; b.cfg = cfg;
   b.raw = raw; b.save = save; b.seeds = g; b.grads = grads;
   NB_TRY(b.check());
@@ -1372,14 +1480,34 @@ int nerf_b200_march_bwd_tc_outs(const float* rays, const float* z_vals, const fl
   return march_bwd_tc_impl(rays, z_vals, noise, N, S, net, packed, cfg, raw, save, *g, grads, workspace, workspace_bytes, stream);
 }
 
-size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, const NerfNetParams* net_coarse, int S_fine, const NerfNetParams* net_fine) {
+// the split backward of one pass (precision TC_SPLIT): the split records of nerf_b200_march_train_split, the split training
+// image (nerf_b200_pack_weights_split_train); seeds as nerf_b200_march_bwd_tc_outs
+size_t nerf_b200_march_bwd_split_workspace_bytes(int64_t N, int S, const NerfNetParams* net) {
+  if (!net || check_tc_net(net) || N <= 0 || S <= 0) return 0;
+  return bwd_pass_bytes(N, S, net, true);
+}
+
+int nerf_b200_march_bwd_split(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                              const void* packed, const NerfRenderCfg* cfg, const float* raw, const NerfTrainSave* save,
+                              const NerfOutGrads* g, const NerfNetGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
+  NB_CHECK_ARG(g, "NULL pointer");
+  return march_bwd_tc_impl(rays, z_vals, noise, N, S, net, packed, cfg, raw, save, *g, grads, workspace, workspace_bytes, stream, true);
+}
+
+static size_t render_rays_bwd_bytes(int64_t N, int S_coarse, const NerfNetParams* net_coarse, int S_fine, const NerfNetParams* net_fine, bool split) {
   if (!net_coarse || check_tc_net(net_coarse) || N <= 0 || S_coarse <= 0) return 0;
-  size_t b = bwd_pass_bytes(N, S_coarse, net_coarse);
+  size_t b = bwd_pass_bytes(N, S_coarse, net_coarse, split);
   if (net_fine && S_fine > 0) {
     if (check_tc_net(net_fine) || net_fine->use_viewdirs != net_coarse->use_viewdirs) return 0;
-    b += bwd_pass_bytes(N, S_fine, net_fine);
+    b += bwd_pass_bytes(N, S_fine, net_fine, split);
   }
   return b;
+}
+size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, const NerfNetParams* net_coarse, int S_fine, const NerfNetParams* net_fine) {
+  return render_rays_bwd_bytes(N, S_coarse, net_coarse, S_fine, net_fine, false);
+}
+size_t nerf_b200_render_rays_bwd_split_workspace_bytes(int64_t N, int S_coarse, const NerfNetParams* net_coarse, int S_fine, const NerfNetParams* net_fine) {
+  return render_rays_bwd_bytes(N, S_coarse, net_coarse, S_fine, net_fine, true);
 }
 
 // Backward of both passes of render_rays (run_nerf.py:765-772: loss = img2mse(rgb) + img2mse(rgb0); z_samples is detached, :394,
@@ -1387,15 +1515,15 @@ size_t nerf_b200_render_rays_bwd_tc_workspace_bytes(int64_t N, int S_coarse, con
 // x 168 registers), so nothing of the other pass could run beside it.
 static int render_rays_bwd_tc_impl(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse, const NerfBwdPass* fine,
                                    const NerfOutGrads* coarse_g, const NerfOutGrads* fine_g, void* workspace, size_t workspace_bytes,
-                                   void* stream) {
-  BwdTcPass c = bind_pass(rays, N, cfg, coarse, coarse_g), f = bind_pass(rays, N, cfg, fine, fine_g);
+                                   void* stream, bool split = false) {
+  BwdTcPass c = bind_pass(rays, N, cfg, coarse, coarse_g, split), f = bind_pass(rays, N, cfg, fine, fine_g, split);
   NB_TRY(c.check());
   if (fine) NB_TRY(f.check());
   NB_CHECK_ARG(!fine || (fine->net->use_viewdirs != 0) == (coarse->net->use_viewdirs != 0),
                "coarse and fine networks must agree on use_viewdirs (they share one ray batch)");
   if (N == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t cb = bwd_pass_bytes(N, coarse->S, coarse->net);
+  const size_t cb = bwd_pass_bytes(N, coarse->S, coarse->net, split);
   NB_CHECK_ARG(workspace && workspace_bytes >= cb, "render_rays_bwd_tc workspace too small");
   NB_TRY(c.run(workspace, cb, st));
   return fine ? f.run(static_cast<uint8_t*>(workspace) + cb, workspace_bytes - cb, st) : 0;
@@ -1410,6 +1538,14 @@ int nerf_b200_render_rays_bwd_tc_outs(const float* rays, int64_t N, const NerfRe
                                       const NerfOutGrads* coarse_g, const NerfOutGrads* fine_g, void* workspace, size_t workspace_bytes,
                                       void* stream) {
   return render_rays_bwd_tc_impl(rays, N, cfg, coarse, fine, coarse_g, fine_g, workspace, workspace_bytes, stream);
+}
+
+// the split backward of both passes on one stream (graph-capturable); seeds per pass as NerfOutGrads (rgb_map alone for an rgb loss)
+int nerf_b200_render_rays_bwd_split(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfBwdPass* coarse, const NerfBwdPass* fine,
+                                    const NerfOutGrads* coarse_g, const NerfOutGrads* fine_g, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+  NB_CHECK_ARG(coarse_g && (!fine || fine_g), "NULL output gradients");
+  return render_rays_bwd_tc_impl(rays, N, cfg, coarse, fine, coarse_g, fine_g, workspace, workspace_bytes, stream, true);
 }
 
 // ---- the two ends of the optimisation step (train_step.cuh) ------------------------------------------

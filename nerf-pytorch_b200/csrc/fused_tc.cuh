@@ -123,6 +123,17 @@ static inline PackLayout make_pack_layout_split(const NerfNetParams& n) {
   return L;
 }
 
+// The split training image (the split backward): the split image above byte for byte, then, 1 KB-aligned, the backward's
+// transposed chunk stream (make_pack_layout's) with every chunk as two hi | lo ring stages of the weights scaled by their
+// layer's scale.
+static inline PackLayout make_pack_layout_split_train(const NerfNetParams& n) {
+  PackLayout L = make_pack_layout_split(n);
+  L.off_bwd = (L.total + 1023) & ~(size_t)1023;
+  L.bwd_bytes = 2 * make_pack_layout(n).bwd_bytes;
+  L.total = L.off_bwd + L.bwd_bytes;
+  return L;
+}
+
 // element (row n, k) of a chunk = src[n * sn + (k0 + k) * sk]: forward chunks read W[n][k0 + k] (sn = ld, sk = 1), the
 // backward's transposed chunks read W[k0 + k][n] (sn = 1, sk = ld)
 struct PackChunk { const float* src; int sn, sk, k0, kvalid, nrows; unsigned dst_off; };

@@ -166,16 +166,17 @@ __device__ __forceinline__ float quad_sum(float v) {
 // (xs[i], ys[j], zs[k]), k = 0 .. nz - 1 (p.S = nz), and row m = n * nz + k of the pass is sigma's C-order index.
 struct DensityGrid { const float* xs; const float* ys; const float* zs; int ny; float* sigma; };
 
-// The pass of march_wg_kernel (SPLIT false) and march_split_kernel (SPLIT true, never EMIT).  SPLIT: every MMA operand is a hi
-// and a lo fp16 image (the split map of fused_tc.cuh), each weight chunk streams as two ring stages, the weights are scaled by
-// wscale[l] (a power of two: the accumulator starts at bias * wscale[l] and is scaled back exactly after the MMAs).
+// The pass of march_wg_kernel (SPLIT false) and march_split_kernel / march_split_train_kernel (SPLIT true).  SPLIT: every MMA
+// operand is a hi and a lo fp16 image (the split map of fused_tc.cuh), each weight chunk streams as two ring stages, the weights
+// are scaled by wscale[l] (a power of two: the accumulator starts at bias * wscale[l] and is scaled back exactly after the MMAs).
+// EMIT && SPLIT: a tile's record is the hi record followed by the lo record (rec_split_lo), and every image goes out twice: the
+// hi operand and the lo operand SPLIT_LO above it.
 // DENSITY (never EMIT): the points come from the axes of `grid`, only the pts layers stream and run, and the sigma head
 // (alpha_linear, or row 3 of output_linear without view directions) goes straight out as one fp32 per row: no view layers,
 // view bias, raw rows or compositing.  The head is the same code in the same order as the other modes, so sigma is bit for bit
 // raw[..., 3] of the pts mode on the same points.
 template <bool EMIT, bool SPLIT, bool DENSITY = false>
 __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveDev sv, const float* wscale, const DensityGrid grid = {}) {
-  static_assert(!(EMIT && SPLIT), "the split forward has no training mode");
   static_assert(!(EMIT && DENSITY), "the density pass has no training mode");
   constexpr int NST = SPLIT ? SPLIT_NST : FWD_NST;
   constexpr int CPS = SPLIT ? 2 : 1;                              // ring stages per weight chunk
@@ -234,6 +235,7 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
   const uint32_t act = sb + SM_ACT + (uint32_t)w * 32768u, enc = sb + FWD_ENC + (uint32_t)w * 8192u;
   const uint32_t ring = sb + (SPLIT ? SPLIT_WRING : FWD_WRING);
   const uint64_t l2_first = EMIT ? ptx::l2_policy_evict_first() : 0ull;
+  const uint32_t rec_lo = rec_split_lo(D);                       // EMIT && SPLIT: lo record -> its tile's hi record
   auto wg_sync = [&]() { ptx::named_bar_sync(1 + w, 128); };
   // row-dependent parts of the swizzled addresses of this thread's pairs: column pair (8 j + 2 q4) of row r sits at
   // rowoff(r) + (j >> 3) * 8192 + (((j & 7) ^ (r & 7)) << 4) + 4 q4
@@ -287,7 +289,11 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
     }
     ptx::fence_proxy_async_smem();
     wg_sync();
-    if (EMIT && t == 0) { ptx::bulk_s2g_hint(arec + (uint32_t)w * 8192u, enc, 8192u, l2_first); ptx::bulk_commit(); }
+    if (EMIT && t == 0) {
+      ptx::bulk_s2g_hint(arec + (uint32_t)w * 8192u, enc, 8192u, l2_first);
+      if constexpr (SPLIT) ptx::bulk_s2g_hint(arec + rec_lo + (uint32_t)w * 8192u, enc + SPLIT_LO, 8192u, l2_first);
+      ptx::bulk_commit();
+    }
 
     float hp[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};   // head partial sums of this thread's columns, per row
     ph.stop(PH_SAMPLER);
@@ -403,6 +409,7 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
           wg_sync();
           if (EMIT && l < D && t == 0) {
             ptx::bulk_s2g_hint(arec + rec_act_h(l) + (uint32_t)w * 32768u, act, 32768u, l2_first);
+            if constexpr (SPLIT) ptx::bulk_s2g_hint(arec + rec_lo + rec_act_h(l) + (uint32_t)w * 32768u, act + SPLIT_LO, 32768u, l2_first);
             ptx::bulk_commit();
           }
         }
@@ -433,8 +440,18 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
             const int bit = 31 - (8 * (j & 3) + 2 * q4);
             m0[j >> 2] |= ((__float_as_uint(x0) >> 31) << bit) | ((__float_as_uint(x1) >> 31) << (bit - 1));
             m1[j >> 2] |= ((__float_as_uint(y0) >> 31) << bit) | ((__float_as_uint(y1) >> 31) << (bit - 1));
+            if constexpr (SPLIT) {
+              uint32_t h0, l0, h1, l1;
+              split_f16x2(fmaxf(x0, 0.f), fmaxf(x1, 0.f), h0, l0);
+              split_f16x2(fmaxf(y0, 0.f), fmaxf(y1, 0.f), h1, l1);
+              ptx::st_shared_b32(pair_addr(act, ro0, r0, j), h0);
+              ptx::st_shared_b32(pair_addr(act, ro1, r1, j), h1);
+              ptx::st_shared_b32(pair_addr(act + SPLIT_LO, ro0, r0, j), l0);
+              ptx::st_shared_b32(pair_addr(act + SPLIT_LO, ro1, r1, j), l1);
+            } else {
             ptx::st_shared_b32(pair_addr(act, ro0, r0, j), ptx::cvt_relu_f16x2(x0, x1));
             ptx::st_shared_b32(pair_addr(act, ro1, r1, j), ptx::cvt_relu_f16x2(y0, y1));
+            }
           }
           const float h00 = fmaxf(x0, 0.f), h01 = fmaxf(x1, 0.f), h10 = fmaxf(y0, 0.f), h11 = fmaxf(y1, 0.f);
 #pragma unroll
@@ -457,6 +474,7 @@ __device__ __forceinline__ void march_pass(const MarchParams p, const TrainSaveD
           wg_sync();
           if (t == 0) {
             ptx::bulk_s2g_hint(arec + rec_act_hv(D) + (uint32_t)w * 16384u, act, 16384u, l2_first);
+            if constexpr (SPLIT) ptx::bulk_s2g_hint(arec + rec_lo + rec_act_hv(D) + (uint32_t)w * 16384u, act + SPLIT_LO, 16384u, l2_first);
             ptx::bulk_commit();
           }
         }
@@ -515,6 +533,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) march_wg_kernel(const MarchPara
 // precision TC_SPLIT: fp32-class results from three fp16 MMAs per K-step (inference only; wscale: the split image's scales)
 __global__ void __launch_bounds__(TC_THREADS, 1) march_split_kernel(const MarchParams p, const float* __restrict__ wscale) {
   march_pass<false, true>(p, TrainSaveDev{}, wscale);
+}
+
+// precision TC_SPLIT in training mode: march_split_kernel's outputs, bit for bit, plus the split records (hi record, then lo
+// record, per tile; mask bits = signs of the split fp32 pre-activations) that the split backward reads
+__global__ void __launch_bounds__(TC_THREADS, 1) march_split_train_kernel(const MarchParams p, const TrainSaveDev sv, const float* __restrict__ wscale) {
+  march_pass<true, true>(p, sv, wscale);
 }
 
 // The density grid (nerf_b200_density_grid): sigma on the points of `g`, precision TC_FP16 on the fp16 image, TC_SPLIT (wscale

@@ -62,6 +62,11 @@ __host__ __device__ __forceinline__ uint32_t rec_grad_bytes(int D) { return 3276
 __host__ __device__ __forceinline__ uint32_t rec_grad_step(int j) { return 32768u + (uint32_t)j * 65536u; }         // output of dgrad step j
 __host__ __device__ __forceinline__ uint32_t rec_grad_dA(int l, int D) { return rec_grad_step(D - l); }              // pts layer l
 
+// Split records (precision TC_SPLIT, the split backward): a tile's activation record is the hi record above followed by the lo
+// record (lo = fp16(x - hi) of every image, same layout), and so is its gradient record; the mask record is unchanged.
+__host__ __device__ __forceinline__ uint32_t rec_split_lo(int D) { return rec_act_bytes(D); }                        // act: lo record
+__host__ __device__ __forceinline__ uint32_t rec_grad_split_lo(int D) { return rec_grad_bytes(D); }                 // grad: lo record
+
 // byte offset of element (row r, column col) inside a [128 x C] tile image in global memory
 __host__ __device__ __forceinline__ uint32_t img_off(int r, int col, int C) {
   return (uint32_t)((r >> 6) * (C >> 6) * 8192 + (col >> 6) * 8192 + ((r & 63) >> 3) * 1024 + (r & 7) * 128 + ((((col & 63) >> 3) ^ (r & 7)) << 4) + (col & 7) * 2);

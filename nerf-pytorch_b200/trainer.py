@@ -8,6 +8,7 @@ no autograd graph and no per-tensor optimizer:
 
     pack weights -> pack rays -> z sampling -> fused pass (coarse, training mode) -> resampling -> fused pass (fine)
     -> fused MSE + gradient seed (both terms) -> tensor-core backward of both passes into ONE flat gradient buffer
+    (precision tc_split with set_backward('tc_split'): the split training image, split records and the split backward)
     -> [one all-reduce of that buffer when data parallel] -> flat Adam with the decayed rate computed on the device
 
 captured once per ray count and replayed.  The constructor's `n_rays` is the capacity: the buffers hold that many rays and
@@ -98,8 +99,12 @@ class FusedTrainStep:
         if not isinstance(self.net_c, api.NeRF):
             raise RuntimeError("FusedTrainStep needs nerf_b200.NeRF networks (with or without view directions)")
         self.use_viewdirs = bool(self.net_c.use_viewdirs)
-        if api.get_precision() != "tc_fp16":
-            raise RuntimeError("FusedTrainStep runs the tensor-core path (set_precision('tc_fp16'))")
+        # tc_split trains here only with its tensor-core backward; every other combination keeps the tc_fp16 requirement
+        self.split = api.get_precision() == "tc_split" and api.get_backward() == "tc_split"
+        if api.get_precision() != "tc_fp16" and not self.split:
+            raise RuntimeError("FusedTrainStep runs the tensor-core path (set_precision('tc_fp16'), or set_precision('tc_split') with "
+                               "set_backward('tc_split'))")
+        self._sfx = "_split" if self.split else ""     # the library entries of the split path
         self.dev = self.net_c._check_device()
         self.H, self.W, self.K, self.N = int(H), int(W), K, int(n_rays)
         self.Sc, self.Ni = int(kw["N_samples"]), int(kw.get("N_importance", 0))
@@ -160,9 +165,14 @@ class FusedTrainStep:
         self._out_f = NerfPassOut(api._ptr(o["rgb"]), api._ptr(o["disp"]), api._ptr(o["acc"]), C.c_void_p(0), C.c_void_p(0), api._ptr(o["raw"]))
         self._np_c, self._np_f = self.net_c.net_params(), (self.net_f.net_params() if self.Ni > 0 else None)
         lib = self.lib
-        self._pk_c = torch.empty(lib.nerf_b200_packed_bytes(C.byref(self._np_c)), dtype=torch.uint8, device=self.dev)
+        self._pack_fn = getattr(lib, "nerf_b200_pack_weights" + ("_split_train" if self.split else ""))
+        packed_bytes = getattr(lib, "nerf_b200_packed_bytes" + ("_split_train" if self.split else ""))
+        self._pk_c = torch.empty(packed_bytes(C.byref(self._np_c)), dtype=torch.uint8, device=self.dev)
         self._pk_f = self._pk_c if (self.Ni == 0 or self.net_f is self.net_c) else \
-            torch.empty(lib.nerf_b200_packed_bytes(C.byref(self._np_f)), dtype=torch.uint8, device=self.dev)
+            torch.empty(packed_bytes(C.byref(self._np_f)), dtype=torch.uint8, device=self.dev)
+        # the split backward takes its seeds as NerfOutGrads (dL/drgb_map of each pass)
+        self._og_c = _lib.NerfOutGrads(rgb_map=api._ptr(o["g_rgb0"]))
+        self._og_f = _lib.NerfOutGrads(rgb_map=api._ptr(o["g_rgb"]))
         # every buffer above has the rays as its leading dimension, so an n-ray step (n <= N) runs on their first n rows, which
         # start at the same pointers; the records and workspaces follow the tile plan of n (see _size_buffers)
         self._sized = {}
@@ -194,10 +204,11 @@ class FusedTrainStep:
         with api._on(self.rays):
             for tag, S, np_ in (("c", self.Sc, self._np_c), ("f", Sf, self._np_f))[:1 + fine]:
                 ab, mb = C.c_size_t(0), C.c_size_t(0)
-                check(lib.nerf_b200_train_record_bytes(n, S, C.byref(np_), C.byref(ab), C.byref(mb)), "train_record_bytes")
+                check(getattr(lib, "nerf_b200_train_record_bytes" + self._sfx)(n, S, C.byref(np_), C.byref(ab), C.byref(mb)),
+                      "train_record_bytes" + self._sfx)
                 b["act_" + tag], b["mask_" + tag] = buf("act_" + tag, ab.value), buf("mask_" + tag, mb.value)
             b["ws"] = buf("ws", lib.nerf_b200_march_workspace_bytes(n, Sf))
-            bw = lib.nerf_b200_render_rays_bwd_tc_workspace_bytes(n, self.Sc, C.byref(self._np_c), Sf if fine else 0,
+            bw = getattr(lib, "nerf_b200_render_rays_bwd_" + ("split" if self.split else "tc") + "_workspace_bytes")(n, self.Sc, C.byref(self._np_c), Sf if fine else 0,
                                                                   C.byref(self._np_f) if fine else None)
             b["bws"] = buf("bws", bw + 1024)
         if cap is not None and all(b[k] is cap[k] for k in b):
@@ -253,9 +264,9 @@ class FusedTrainStep:
         b = self._sized[n]
         st = api._stream(self.rays)
         with api._on(self.rays):
-            check(lib.nerf_b200_pack_weights(C.byref(self._np_c), api._ptr(self._pk_c), self._pk_c.numel(), st), "pack_weights")
+            check(self._pack_fn(C.byref(self._np_c), api._ptr(self._pk_c), self._pk_c.numel(), st), "pack_weights")
             if self._pk_f is not self._pk_c:
-                check(lib.nerf_b200_pack_weights(C.byref(self._np_f), api._ptr(self._pk_f), self._pk_f.numel(), st), "pack_weights")
+                check(self._pack_fn(C.byref(self._np_f), api._ptr(self._pk_f), self._pk_f.numel(), st), "pack_weights")
             # the draws of an n-ray step fill the first n rows only: the generator advances as in a step built for n rays
             if self.t_rand is not None:                                 # (the reference's draw order)
                 self.t_rand[:n].uniform_()                              # run_nerf.py:371
@@ -266,13 +277,13 @@ class FusedTrainStep:
             if self.noise1 is not None:
                 self.noise1[:n].normal_().mul_(self.noise_std)
             fine = self.Ni > 0
-            check(lib.nerf_b200_render_rays_fwd_train(
+            check(getattr(lib, "nerf_b200_render_rays_fwd_train" + self._sfx)(
                 api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(self._np_c), api._ptr(self._pk_c),
                 C.byref(self._np_f) if fine else None, api._ptr(self._pk_f) if fine else None,
                 api._ptr(self.t_vals), api._ptr(self.u_det), api._ptr(self.t_rand), api._ptr(self.u_rand), api._ptr(self.noise0), api._ptr(self.noise1),
                 api._ptr(self.z_c), C.byref(self._out_c), api._ptr(self.z_f) if fine else None, api._ptr(self.z_std) if fine else None,
                 C.byref(self._out_f) if fine else None, api._ptr(b["ws"]), b["ws"].numel(),
-                C.byref(b["sv_c"]), C.byref(b["sv_f"]) if fine else None, st), "render_rays_fwd_train")
+                C.byref(b["sv_c"]), C.byref(b["sv_f"]) if fine else None, st), "render_rays_fwd_train" + self._sfx)
             # loss = img2mse(rgb, target) + img2mse(rgb0, target)  (run_nerf.py:764-772), means over the n rays, and its gradient seeds
             self.state[0:1].zero_()
             self.flat_g.zero_()
@@ -282,6 +293,12 @@ class FusedTrainStep:
                 check(lib.nerf_b200_mse_seed(api._ptr(o["rgb"]), api._ptr(self.target), n, gscale, api._ptr(o["g_rgb"]), api._ptr(self.state), st), "mse_seed")
             check(lib.nerf_b200_mse_seed(api._ptr(o["rgb0"]), api._ptr(self.target), n, gscale, api._ptr(o["g_rgb0"]), api._ptr(self.state), st), "mse_seed")
             # backward of both passes into the flat gradient buffer (one call)
+            if self.split:
+                check(lib.nerf_b200_render_rays_bwd_split(api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(b["bp_c"]),
+                                                          C.byref(b["bp_f"]) if fine else None, C.byref(self._og_c),
+                                                          C.byref(self._og_f) if fine else None, api._ptr(b["bws"]), b["bws"].numel(), st),
+                      "render_rays_bwd_split")
+                return
             check(lib.nerf_b200_render_rays_bwd_tc(api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(b["bp_c"]),
                                                    C.byref(b["bp_f"]) if fine else None, api._ptr(b["bws"]), b["bws"].numel(), st), "render_rays_bwd_tc")
 
