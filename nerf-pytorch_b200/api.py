@@ -16,6 +16,7 @@ from __future__ import annotations
 import ctypes as C
 import numbers
 import os
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -89,6 +90,12 @@ def _on(t: torch.Tensor):
 
 def _ptr(t):
     return C.c_void_p(0 if t is None else t.data_ptr())
+
+
+def _call(lib, name, *args):
+    """Call the library entry `name` and raise its error under the name without the nerf_b200_ prefix.  Callers spell `name`
+    out in full, so that a search for an entry point finds them."""
+    check(getattr(lib, name)(*args), name[len("nerf_b200_"):])
 
 
 def _f32c(t: torch.Tensor, what: str) -> torch.Tensor:
@@ -272,19 +279,19 @@ class NeRF(nn.Module):
         """fp16 UMMA-swizzled weight streams (forward chunks + the transposed chunks of the backward), re-packed
         whenever a parameter changed in place (optimizer.step bumps Parameter._version; load_state_dict / .to()
         change data_ptr) or invalidate_pack() was called."""
-        return self._packed_image("_pack", "")
+        return self._packed_image("_pack", "nerf_b200_packed_bytes", "nerf_b200_pack_weights")
 
     def packed_split(self):
         """The split image of precision tc_split (hi | lo fp16 halves of the scaled forward weights), cached apart from
         packed() and re-packed on the same conditions."""
-        return self._packed_image("_pack_split", "_split")
+        return self._packed_image("_pack_split", "nerf_b200_packed_bytes_split", "nerf_b200_pack_weights_split")
 
     def packed_split_train(self):
         """The split training image of set_backward('tc_split'): packed_split()'s bytes followed by the backward's transposed
         chunks as hi | lo halves, cached apart from the other images and re-packed on the same conditions."""
-        return self._packed_image("_pack_split_train", "_split_train")
+        return self._packed_image("_pack_split_train", "nerf_b200_packed_bytes_split_train", "nerf_b200_pack_weights_split_train")
 
-    def _packed_image(self, attr, kind):
+    def _packed_image(self, attr, size_fn, pack_fn):
         dev = self._check_device()
         key = (getattr(self, "_pack_epoch", 0),) + tuple((q.data_ptr(), q._version) for _, _, _, q in self._named_params())
         cached = getattr(self, attr, None)
@@ -292,13 +299,13 @@ class NeRF(nn.Module):
             return cached[1]
         lib = _lib.load()
         n = self.net_params()
-        nbytes = getattr(lib, "nerf_b200_packed_bytes" + kind)(C.byref(n))
+        nbytes = getattr(lib, size_fn)(C.byref(n))
         if nbytes == 0:
             raise RuntimeError("nerf_b200: " + lib.nerf_b200_last_error().decode())
         buf = cached[1] if (cached is not None and cached[1].numel() == nbytes and cached[1].device == dev) \
             else torch.empty(nbytes, dtype=torch.uint8, device=dev)
         with _on(buf):
-            check(getattr(lib, "nerf_b200_pack_weights" + kind)(C.byref(n), _ptr(buf), nbytes, _stream(buf)), "pack_weights" + kind)
+            _call(lib, pack_fn, C.byref(n), _ptr(buf), nbytes, _stream(buf))
         setattr(self, attr, (key, buf))
         return buf
 
@@ -500,14 +507,76 @@ def _cfg_struct(cfgd, ray_stride):
     return cfg
 
 
-def _train_save(lib, N, S, net_params, dev, split=False):
-    """Allocate the per-tile records of one training-mode pass (csrc/train_common.cuh; split: hi + lo records) ->
-    (NerfTrainSave, tensors)."""
+class _TcTrain(NamedTuple):
+    """One tensor-core training path: what differs between the fp16 and the split path.  `image` is the NeRF method giving the
+    packed image the path reads, `packed_bytes` / `pack_weights` size and pack it into a buffer of the caller's (FusedTrainStep).
+    The backward of one pass (`march_bwd*`) or of both passes in one call (`bwd*`) takes NerfOutGrads seeds; the `_rgb` entries
+    take dL/drgb_map alone (in NerfBwdPass.g_rgb for `bwd_rgb`) and are None where the path has no such entry."""
+    image: object
+    packed_bytes: str
+    pack_weights: str
+    record_bytes: str
+    fwd: str
+    march_bwd_rgb: str | None
+    march_bwd: str
+    march_bwd_ws: str
+    bwd_rgb: str | None
+    bwd: str
+    bwd_ws: str
+
+
+_TC_FP16 = _TcTrain(image=NeRF.packed, packed_bytes="nerf_b200_packed_bytes", pack_weights="nerf_b200_pack_weights",
+                    record_bytes="nerf_b200_train_record_bytes", fwd="nerf_b200_render_rays_fwd_train",
+                    march_bwd_rgb="nerf_b200_march_bwd_tc", march_bwd="nerf_b200_march_bwd_tc_outs",
+                    march_bwd_ws="nerf_b200_march_bwd_tc_workspace_bytes", bwd_rgb="nerf_b200_render_rays_bwd_tc",
+                    bwd="nerf_b200_render_rays_bwd_tc_outs", bwd_ws="nerf_b200_render_rays_bwd_tc_workspace_bytes")
+_TC_SPLIT = _TcTrain(image=NeRF.packed_split_train, packed_bytes="nerf_b200_packed_bytes_split_train",
+                     pack_weights="nerf_b200_pack_weights_split_train", record_bytes="nerf_b200_train_record_bytes_split",
+                     fwd="nerf_b200_render_rays_fwd_train_split", march_bwd_rgb=None, march_bwd="nerf_b200_march_bwd_split",
+                     march_bwd_ws="nerf_b200_march_bwd_split_workspace_bytes", bwd_rgb=None, bwd="nerf_b200_render_rays_bwd_split",
+                     bwd_ws="nerf_b200_render_rays_bwd_split_workspace_bytes")
+
+
+def _train_path(precision, backward, want_grad, net_c=None, net_f=None, fused=False):
+    """The backward a call takes, from get_precision(), get_backward(), whether it needs gradients and its coarse and fine
+    networks (net_f None: no fine pass) -> None (no gradient needed), "exact" (the fp32 recompute backward) or the
+    tensor-core path whose training forward leaves the records its backward reads (_TC_FP16, _TC_SPLIT).  Raises the refusals.
+
+    A drop-in call (render, render_rays) trains on fp16 records under tc_fp16 with set_backward('tc'), but takes the exact
+    backward when its networks disagree on use_viewdirs; set_backward('tc_split') trains on split records under tc_split only.
+    FusedTrainStep (fused=True) always trains on records: under tc_fp16 on the fp16 path whatever set_backward says, under
+    tc_split with set_backward('tc_split'), and with networks that agree on use_viewdirs (they share the ray batch)."""
+    if not want_grad:
+        return None
+    fp16 = precision == "tc_fp16" and (backward == "tc" or fused)
+    split = precision == "tc_split" and backward == "tc_split"
+    if fused and not (fp16 or split):
+        raise RuntimeError("FusedTrainStep runs the tensor-core path (set_precision('tc_fp16'), or set_precision('tc_split') with "
+                           "set_backward('tc_split'))")
+    if backward == "tc_split" and not split and not fused:
+        raise RuntimeError(f"set_backward('tc_split') needs precision tc_split (precision is {precision}): "
+                           "call set_precision('tc_split') or set_backward('tc')")
+    if net_f is not None and bool(net_f.use_viewdirs) != bool(net_c.use_viewdirs):
+        if fused:
+            raise RuntimeError("FusedTrainStep: coarse and fine networks must agree on use_viewdirs (they share the ray batch)")
+        if split:
+            raise RuntimeError("set_backward('tc_split') needs the coarse and fine networks to agree on use_viewdirs")
+        return "exact"
+    return _TC_FP16 if fp16 else _TC_SPLIT if split else "exact"
+
+
+def _record_bytes(lib, path, N, S, net_params):
+    """(activation bytes, mask bytes) of the per-tile records one training-mode pass of `path` leaves (csrc/train_common.cuh)."""
     ab, mb = C.c_size_t(0), C.c_size_t(0)
-    sfx = "_split" if split else ""
-    check(getattr(lib, "nerf_b200_train_record_bytes" + sfx)(N, S, C.byref(net_params), C.byref(ab), C.byref(mb)), "train_record_bytes" + sfx)
-    act = torch.empty(ab.value, dtype=torch.uint8, device=dev)
-    mask = torch.empty(mb.value, dtype=torch.uint8, device=dev)
+    _call(lib, path.record_bytes, N, S, C.byref(net_params), C.byref(ab), C.byref(mb))
+    return ab.value, mb.value
+
+
+def _train_save(lib, N, S, net_params, dev, path=_TC_FP16):
+    """Allocate the records of one training-mode pass of `path` -> (NerfTrainSave, act, mask)."""
+    ab, mb = _record_bytes(lib, path, N, S, net_params)
+    act = torch.empty(ab, dtype=torch.uint8, device=dev)
+    mask = torch.empty(mb, dtype=torch.uint8, device=dev)
     return _records_save(act, mask), act, mask
 
 
@@ -516,9 +585,10 @@ def _records_save(act, mask):
     return NerfTrainSave(_ptr(act), act.numel(), _ptr(mask), mask.numel())
 
 
-def _pass_structs(net, gbuf, rec, train_tc):
-    """NerfNetParams, NerfNetGrads and, for the tensor-core backward, NerfTrainSave of one backward pass (rec: raw, act, mask)."""
-    return net.net_params(), net.grad_struct(gbuf), (_records_save(rec[1], rec[2]) if train_tc else None)
+def _bwd_pass(z, noise, S, net_params, packed, raw, save, g_rgb, grads):
+    """NerfBwdPass of one tensor-core backward pass (it keeps the structs it points to alive)."""
+    return _lib.NerfBwdPass(_ptr(z), _ptr(noise), S, C.pointer(net_params), _ptr(packed), _ptr(raw), C.pointer(save), _ptr(g_rgb),
+                            C.pointer(grads))
 
 
 def _workspace(nbytes, dev):
@@ -561,53 +631,44 @@ def _flush_deferred_pack():
 
 
 class _RenderRays(torch.autograd.Function):
-    """Forward: nerf_b200_render_rays_fwd (coarse z -> fused pass -> resample -> fused pass); when a parameter needs a
-    gradient and the tensor-core backward is selected, the training-mode variant that also leaves the per-tile
-    activation records.  Backward: per pass nerf_b200_march_bwd_tc (wgmma dgrad chain + layer-major wgrad from
-    those records) or, in exact mode, nerf_b200_march_bwd (fp32 recompute + GEMM backprop).  Every output but z_std
-    carries a gradient, as in the reference: a loss on rgb_map / rgb0 alone (run_nerf.py:765-772) takes those entry
-    points, a loss that also reads disp, acc, disp0, acc0 or raw takes their _outs variants (NerfOutGrads seeds per
-    pass).  z_samples is detached in the reference (:394) so nothing flows through the resampling."""
+    """Forward: nerf_b200_render_rays_fwd (coarse z -> fused pass -> resample -> fused pass); on a tensor-core training path
+    (_train_path) that path's training-mode variant, which also leaves the per-tile activation records.  Backward: per pass
+    the path's dgrad chain + layer-major wgrad from those records, or on the exact path nerf_b200_march_bwd (fp32 recompute +
+    GEMM backprop).  Every output but z_std carries a gradient, as in the reference: a loss on rgb_map / rgb0 alone
+    (run_nerf.py:765-772) takes the rgb-only entry points where the path has them, a loss that also reads disp, acc, disp0,
+    acc0 or raw takes their _outs variants (NerfOutGrads seeds per pass).  z_samples is detached in the reference (:394) so
+    nothing flows through the resampling."""
 
     @staticmethod
-    def forward(ctx, ray_batch, cfgd, net_c, net_f, t_rand, u_rand, noise0, noise1, *params):
+    def forward(ctx, ray_batch, cfgd, path, net_c, net_f, t_rand, u_rand, noise0, noise1, *params):
         lib = _lib.load()
         dev = ray_batch.device
         N = ray_batch.shape[0]
         Sc, Ni = cfgd["N_samples"], cfgd["N_importance"]
         Sf = Sc + Ni
         cfg = _cfg_struct(cfgd, ray_batch.shape[1])
-        tc = cfg.precision == PREC_TC_FP16          # tc_split runs like fp32 here: no training-mode records, raw kept
+        records = isinstance(path, _TcTrain)
         pc, pf = net_c.net_params(), (net_f.net_params() if net_f is not None else None)
         pk_c = _packed_for(net_c, cfg.precision)
         pk_f = _packed_for(net_f, cfg.precision) if net_f is not None else None
+        if records:                                 # the training forward reads its path's image
+            pk_c, pk_f = path.image(net_c), (path.image(net_f) if net_f is not None else None)
         f32 = dict(device=dev, dtype=torch.float32)
         t_vals = _linspace01(Sc, dev)                                             # run_nerf.py:357
         u_det = _linspace01(Ni, dev) if Ni > 0 else None                          # run_nerf_helpers.py:205
         z_c = torch.empty((N, Sc), **f32)
         o = {k: torch.empty(s, **f32) for k, s in (("rgb0", (N, 3)), ("disp0", (N,)), ("acc0", (N,)), ("w0", (N, Sc)))}
         retraw, fine = cfgd["retraw"], Ni > 0
-        # cfgd["want_grad"]: grad mode was on at the call AND a parameter requires a gradient (inside Function.forward grad mode is
-        # always off, and ctx.needs_input_grad stays True under torch.no_grad()): only then the training-mode kernel runs
-        # (the tensor-core backward needs both nets alike with or without view directions: they share the ray batch)
-        train_tc = bool(tc and cfgd["want_grad"] and get_backward() == "tc" and
-                        (net_f is None or bool(net_f.use_viewdirs) == bool(net_c.use_viewdirs)))
-        # set_backward('tc_split') under tc_split: the split training forward and the split backward (render_rays refused the
-        # mode under the other precisions before any launch)
-        train_split = bool(cfg.precision == PREC_TC_SPLIT and cfgd["want_grad"] and get_backward() == "tc_split")
-        if train_split and net_f is not None and bool(net_f.use_viewdirs) != bool(net_c.use_viewdirs):
-            raise RuntimeError("set_backward('tc_split') needs the coarse and fine networks to agree on use_viewdirs")
-        if train_split:
-            pk_c = net_c.packed_split_train()
-            pk_f = net_f.packed_split_train() if net_f is not None else None
-        raw_c = torch.empty((N, Sc, 4), **f32) if ((retraw and not fine) or not tc or train_tc) else None
+        # raw is kept outside tc_fp16 (tc_split runs like fp32 here unless it trains on records) and for the records' backward
+        keep_raw = cfg.precision != PREC_TC_FP16 or records
+        raw_c = torch.empty((N, Sc, 4), **f32) if ((retraw and not fine) or keep_raw) else None
         out_c = NerfPassOut(_ptr(o["rgb0"]), _ptr(o["disp0"]), _ptr(o["acc0"]), C.c_void_p(0), _ptr(o["w0"]), _ptr(raw_c))
         z_f = z_std = raw_f = None
         out_f = None
         if fine:
             z_f, z_std = torch.empty((N, Sf), **f32), torch.empty((N,), **f32)
             o.update(rgb=torch.empty((N, 3), **f32), disp=torch.empty((N,), **f32), acc=torch.empty((N,), **f32))
-            raw_f = torch.empty((N, Sf, 4), **f32) if (retraw or not tc or train_tc) else None
+            raw_f = torch.empty((N, Sf, 4), **f32) if (retraw or keep_raw) else None
             out_f = NerfPassOut(_ptr(o["rgb"]), _ptr(o["disp"]), _ptr(o["acc"]), C.c_void_p(0), C.c_void_p(0), _ptr(raw_f))
         ws_bytes = lib.nerf_b200_march_workspace_bytes(N, Sf)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
@@ -619,25 +680,22 @@ class _RenderRays(torch.autograd.Function):
         # render() may have left the construction of this very batch to the prologue launch (_DEFERRED_PACK): take it over here
         gen = _take_deferred_pack(ray_batch)
         with _on(ray_batch):
-            if gen is not None and (train_tc or train_split):  # the training-mode entry builds nothing: one extra launch now
-                _launch_pack(lib, gen, ray_batch)
-                gen = None
-            if train_tc or train_split:
-                sv_c, act_c, mask_c = _train_save(lib, N, Sc, pc, dev, train_split)
+            if records:
+                if gen is not None:                 # the training-mode entry builds nothing: one extra launch now
+                    _launch_pack(lib, gen, ray_batch)
+                sv_c, act_c, mask_c = _train_save(lib, N, Sc, pc, dev, path)
                 saved_rec = (raw_c, act_c, mask_c)
                 sv_f = None
                 if fine:
-                    sv_f, act_f, mask_f = _train_save(lib, N, Sf, pf if pf is not None else pc, dev, train_split)
+                    sv_f, act_f, mask_f = _train_save(lib, N, Sf, pf if pf is not None else pc, dev, path)
                     saved_rec += (raw_f, act_f, mask_f)
-                sfx = "_split" if train_split else ""
-                check(getattr(lib, "nerf_b200_render_rays_fwd_train" + sfx)(*common, C.byref(sv_c), C.byref(sv_f) if sv_f is not None else None,
-                                                                            _stream(ray_batch)), "render_rays_fwd_train" + sfx)
+                _call(lib, path.fwd, *common, C.byref(sv_c), C.byref(sv_f) if sv_f is not None else None, _stream(ray_batch))
             elif gen is not None:
                 check(lib.nerf_b200_render_fwd(C.byref(gen[0]), *common, _stream(ray_batch)), "render_fwd")
             else:
                 check(lib.nerf_b200_render_rays_fwd(*common, _stream(ray_batch)), "render_rays_fwd")
         if ctx is not None:
-            ctx.cfgd, ctx.nets, ctx.train_tc, ctx.train_split = cfgd, (net_c, net_f), train_tc, train_split
+            ctx.cfgd, ctx.path, ctx.nets = cfgd, path, (net_c, net_f)
             ctx.save_for_backward(ray_batch, z_c, z_f if fine else torch.empty(0, device=dev),
                                   noise0 if noise0 is not None else torch.empty(0, device=dev),
                                   noise1 if noise1 is not None else torch.empty(0, device=dev), *saved_rec)
@@ -669,10 +727,9 @@ class _RenderRays(torch.autograd.Function):
             s_coarse = dict(rgb_map=g[3], disp_map=g[4], acc_map=g[5])
         else:
             s_fine, s_coarse = {}, dict(rgb_map=g[0], disp_map=g[1], acc_map=g[2], raw=g[3])
-        rgb_only = not any(v is not None for s in (s_fine, s_coarse) for k, v in s.items() if k != "rgb_map")
-
-        if ctx.train_split:                             # the split backward takes NerfOutGrads only; a pass without one is skipped
-            rgb_only = False
+        # the split path has no rgb-only entries: its seeds are NerfOutGrads, and a pass without one is skipped
+        rgb_only = (ctx.path == "exact" or ctx.path.bwd_rgb is not None) and \
+            not any(v is not None for s in (s_fine, s_coarse) for k, v in s.items() if k != "rgb_map")
 
         def seed(s):
             if not rgb_only:
@@ -686,17 +743,17 @@ class _RenderRays(torch.autograd.Function):
 
     @staticmethod
     def _passes(ctx, z_c, z_f, noise0, noise1, rec, seed_f, seed_c):
-        """[(seed, z, noise, net, grad buffers, records)] of the coarse and (with fine samples) the fine pass, and the parameter
-        gradients autograd receives."""
+        """[(seed, z, noise or None, net, grad buffers, records)] of the coarse and (with fine samples) the fine pass, and the
+        parameter gradients autograd receives."""
         net_c, net_f = ctx.nets
         fine = ctx.cfgd["N_importance"] > 0
         grads_c = _grad_buffers(net_c)
         same_net = fine and (net_f is None)
         grads_f = grads_c if same_net else (_grad_buffers(net_f) if fine else None)
-        passes = [(seed_c, z_c, noise0, net_c, grads_c, rec[0:3])]
+        passes = [(seed_c, z_c, noise0 if noise0.numel() else None, net_c, grads_c, rec[0:3])]
         if fine:
-            passes.append((seed_f, z_f, noise1, net_c if same_net else net_f, grads_f, rec[3:6]))
-        out = [None] * 8
+            passes.append((seed_f, z_f, noise1 if noise1.numel() else None, net_c if same_net else net_f, grads_f, rec[3:6]))
+        out = [None] * 9
         out += [grads_c[k] for _, _, k, _ in net_c._named_params()]
         if net_f is not None:
             out += [grads_f[k] for _, _, k, _ in net_f._named_params()]
@@ -705,88 +762,39 @@ class _RenderRays(torch.autograd.Function):
     @staticmethod
     def _backward(ctx, lib, ray_batch, z_c, z_f, noise0, noise1, rec, cfg, seed_f, seed_c, rgb_only):
         """The backward of the passes with a seed (None: the pass does not run).  rgb_only: each seed is dL/drgb_map and the
-        rgb-only entry points run (nerf_b200_render_rays_bwd_tc / march_bwd_tc / march_bwd); otherwise each seed is a
-        (NerfOutGrads, tensors) pair from _out_grads and their _outs variants run."""
-        N = ray_batch.shape[0]
-        sfx = "" if rgb_only else "_outs"
+        rgb-only entry points run; otherwise each seed is a (NerfOutGrads, tensors) pair from _out_grads and the NerfOutGrads
+        entry points run.  A tensor-core path runs both passes in one call (one after the other on the stream) when both
+        have a seed, else the pass that has one; the exact path runs each pass that has one."""
+        N, path = ray_batch.shape[0], ctx.path
 
         def seed_arg(seed):
             return _ptr(seed) if rgb_only else C.byref(seed[0])
         passes, out = _RenderRays._passes(ctx, z_c, z_f, noise0, noise1, rec, seed_f, seed_c)
-        if ctx.train_split:
-            return _RenderRays._backward_split(lib, ray_batch, cfg, passes, out)
+        passes = [p for p in passes if p[0] is not None]
         with _on(ray_batch):
-            if ctx.train_tc and seed_f is not None and seed_c is not None:
-                # both passes in one call: one after the other on the stream (capi.cu: render_rays_bwd_tc_impl)
-                keep, bp = [], []
-                for seed, z, noise, net, gbuf, rc in passes:
-                    n, gs, sv = _pass_structs(net, gbuf, rc, True)
-                    keep += [n, gs, sv]
-                    bp.append(_lib.NerfBwdPass(_ptr(z), _ptr(noise if noise.numel() else None), z.shape[1], C.pointer(n), _ptr(net.packed()),
-                                               _ptr(rc[0]), C.pointer(sv), _ptr(seed if rgb_only else None), C.pointer(gs)))
-                ws_bytes = lib.nerf_b200_render_rays_bwd_tc_workspace_bytes(N, bp[0].S, bp[0].net, bp[1].S, bp[1].net)
-                ws = _workspace(ws_bytes, ray_batch.device)
-                seeds = () if rgb_only else (C.byref(seed_c[0]), C.byref(seed_f[0]))
-                check(getattr(lib, "nerf_b200_render_rays_bwd_tc" + sfx)(_ptr(ray_batch), N, C.byref(cfg), C.byref(bp[0]), C.byref(bp[1]),
-                                                                         *seeds, _ptr(ws), ws_bytes, _stream(ray_batch)),
-                      "render_rays_bwd_tc" + sfx)
-                return out
-            for seed, z, noise, net, gbuf, rc in passes:
-                if seed is None:
-                    continue
-                S = z.shape[1]
-                n, gs, sv = _pass_structs(net, gbuf, rc, ctx.train_tc)
-                nz = _ptr(noise if noise.numel() else None)
-                if ctx.train_tc:
-                    ws_bytes = lib.nerf_b200_march_bwd_tc_workspace_bytes(N, S, C.byref(n))
-                    ws = _workspace(ws_bytes, z.device)
-                    check(getattr(lib, "nerf_b200_march_bwd_tc" + sfx)(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(net.packed()),
-                                                                       C.byref(cfg), _ptr(rc[0]), C.byref(sv), seed_arg(seed), C.byref(gs),
-                                                                       _ptr(ws), ws_bytes, _stream(z)), "march_bwd_tc" + sfx)
-                else:
+            if path == "exact":
+                for seed, z, noise, net, gbuf, _ in passes:
+                    n, gs, S = net.net_params(), net.grad_struct(gbuf), z.shape[1]
                     ws_bytes = lib.nerf_b200_march_bwd_workspace_bytes(N, S, C.byref(n))
                     ws = _workspace(ws_bytes, z.device)
-                    check(getattr(lib, "nerf_b200_march_bwd" + sfx)(_ptr(ray_batch), _ptr(z), nz, N, S, C.byref(n), _ptr(None), C.byref(cfg),
-                                                                    seed_arg(seed), C.byref(gs), _ptr(ws), ws_bytes, _stream(z)),
-                          "march_bwd" + sfx)
-        return out
-
-
-    @staticmethod
-    def _backward_split(lib, ray_batch, cfg, passes, out):
-        """The split backward (set_backward('tc_split')): both passes in one nerf_b200_render_rays_bwd_split call when both have
-        a seed, else each pass that has one through nerf_b200_march_bwd_split."""
-        N = ray_batch.shape[0]
-        keep, bp, seeds = [], [], []
-        for seed, z, noise, net, gbuf, rc in passes:
-            if seed is None:
-                continue
-            n, gs, sv = _pass_structs(net, gbuf, rc, True)
-            keep += [n, gs, sv, seed]
-            seeds.append(seed)
-            bp.append(_lib.NerfBwdPass(_ptr(z), _ptr(noise if noise.numel() else None), z.shape[1], C.pointer(n),
-                                       _ptr(net.packed_split_train()), _ptr(rc[0]), C.pointer(sv), _ptr(None), C.pointer(gs)))
-        with _on(ray_batch):
+                    _call(lib, "nerf_b200_march_bwd" if rgb_only else "nerf_b200_march_bwd_outs", _ptr(ray_batch), _ptr(z), _ptr(noise),
+                          N, S, C.byref(n), _ptr(None), C.byref(cfg), seed_arg(seed), C.byref(gs), _ptr(ws), ws_bytes, _stream(z))
+                return out
+            bp = [_bwd_pass(z, noise, z.shape[1], net.net_params(), path.image(net), rc[0], _records_save(rc[1], rc[2]),
+                            seed if rgb_only else None, net.grad_struct(gbuf)) for seed, z, noise, net, gbuf, rc in passes]
             if len(bp) == 2:
-                ws_bytes = lib.nerf_b200_render_rays_bwd_split_workspace_bytes(N, bp[0].S, bp[0].net, bp[1].S, bp[1].net)
+                ws_bytes = getattr(lib, path.bwd_ws)(N, bp[0].S, bp[0].net, bp[1].S, bp[1].net)
                 ws = _workspace(ws_bytes, ray_batch.device)
-                check(lib.nerf_b200_render_rays_bwd_split(_ptr(ray_batch), N, C.byref(cfg), C.byref(bp[0]), C.byref(bp[1]),
-                                                          C.byref(seeds[0][0]), C.byref(seeds[1][0]), _ptr(ws), ws_bytes,
-                                                          _stream(ray_batch)), "render_rays_bwd_split")
-            for q, seed in zip(bp if len(bp) == 1 else [], seeds):
-                ws_bytes = lib.nerf_b200_march_bwd_split_workspace_bytes(N, q.S, q.net)
+                seeds = () if rgb_only else (C.byref(seed_c[0]), C.byref(seed_f[0]))
+                _call(lib, path.bwd_rgb if rgb_only else path.bwd, _ptr(ray_batch), N, C.byref(cfg), C.byref(bp[0]), C.byref(bp[1]),
+                      *seeds, _ptr(ws), ws_bytes, _stream(ray_batch))
+            elif bp:
+                (q,), seed = bp, passes[0][0]
+                ws_bytes = getattr(lib, path.march_bwd_ws)(N, q.S, q.net)
                 ws = _workspace(ws_bytes, ray_batch.device)
-                check(lib.nerf_b200_march_bwd_split(_ptr(ray_batch), q.z_vals, q.noise, N, q.S, q.net, q.packed, C.byref(cfg), q.raw,
-                                                    q.save, C.byref(seed[0]), q.grads, _ptr(ws), ws_bytes, _stream(ray_batch)),
-                      "march_bwd_split")
+                _call(lib, path.march_bwd_rgb if rgb_only else path.march_bwd, _ptr(ray_batch), q.z_vals, q.noise, N, q.S, q.net, q.packed,
+                      C.byref(cfg), q.raw, q.save, seed_arg(seed), q.grads, _ptr(ws), ws_bytes, _stream(ray_batch))
         return out
-
-
-def _check_split_backward(want_grad):
-    """set_backward('tc_split') trains only in precision tc_split: refuse a call that needs gradients in any other."""
-    if want_grad and get_backward() == "tc_split" and get_precision() != "tc_split":
-        raise RuntimeError(f"set_backward('tc_split') needs precision tc_split (precision is {get_precision()}): "
-                           "call set_precision('tc_split') or set_backward('tc')")
 
 
 def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False, lindisp=False, perturb=0.,
@@ -833,13 +841,14 @@ def render_rays(ray_batch, network_fn, network_query_fn, N_samples, retraw=False
                 lindisp=bool(lindisp), perturb=float(perturb), white_bkgd=bool(white_bkgd), retraw=bool(retraw))
     net_f = network_fine if N_importance > 0 else None          # the reference ignores network_fine without fine samples
     params = [q for _, _, _, q in network_fn._named_params()] + ([q for _, _, _, q in net_f._named_params()] if net_f is not None else [])
-    cfgd["want_grad"] = bool(torch.is_grad_enabled() and any(p.requires_grad for p in params))
-    _check_split_backward(cfgd["want_grad"])
-    if cfgd["want_grad"]:
-        outs = _RenderRays.apply(ray_batch, cfgd, network_fn, net_f, t_rand, u_rand, noise0, noise1, *params)
+    # gradients are needed when grad mode is on AND a parameter requires one (inside Function.forward grad mode is always off,
+    # and ctx.needs_input_grad stays True under torch.no_grad())
+    path = _train_path(get_precision(), get_backward(), torch.is_grad_enabled() and any(p.requires_grad for p in params), network_fn, net_f)
+    if path is not None:
+        outs = _RenderRays.apply(ray_batch, cfgd, path, network_fn, net_f, t_rand, u_rand, noise0, noise1, *params)
     else:                                                        # inference: no autograd node to build (saves ~50 us of host time per call)
         with torch.no_grad():
-            outs = _RenderRays.forward(None, ray_batch, cfgd, network_fn, net_f, t_rand, u_rand, noise0, noise1)
+            outs = _RenderRays.forward(None, ray_batch, cfgd, None, network_fn, net_f, t_rand, u_rand, noise0, noise1)
     if N_importance > 0:
         rgb, disp, acc, rgb0, disp0, acc0, z_std, raw = outs
         ret = {"rgb_map": rgb, "disp_map": disp, "acc_map": acc}
@@ -898,11 +907,14 @@ def render(H, W, K, chunk=1024 * 32, rays=None, c2w=None, ndc=True, near=0., far
     every mode, `c2w_staticcam` (rays from one camera, view directions from another, :104-107) included; per-ray
     near/far arrays are written into their two columns afterwards."""
     lib = _lib.load()
-    grad_nets = [n for n in (kwargs.get("network_fn"), kwargs.get("network_fine")) if isinstance(n, nn.Module)]
-    _check_split_backward(torch.is_grad_enabled() and any(p.requires_grad for n in grad_nets for p in n.parameters()))
+    net_c, net_f = kwargs.get("network_fn"), kwargs.get("network_fine")
+    want = torch.is_grad_enabled() and any(p.requires_grad for n in (net_c, net_f) if isinstance(n, nn.Module) for p in n.parameters())
+    net_f = net_f if kwargs.get("N_importance", 0) > 0 else None
+    # refuse what cannot train before the batch is built; networks that are not NeRF modules are render_rays' to refuse
+    nets = (net_c, net_f) if isinstance(net_c, NeRF) and (net_f is None or isinstance(net_f, NeRF)) else ()
+    _train_path(get_precision(), get_backward(), want, *nets)
     if get_precision() == "fp32":                  # refuse a net the exact path cannot run before the batch is built
-        nets = [kwargs.get("network_fn")] + ([kwargs.get("network_fine")] if kwargs.get("N_importance", 0) > 0 else [])
-        for net in nets:
+        for net in (net_c, net_f):
             if isinstance(net, NeRF) and lib.nerf_b200_march_bwd_workspace_bytes(1, 1, C.byref(net.net_params())) == 0:
                 raise RuntimeError("nerf_b200: " + lib.nerf_b200_last_error().decode())
     ndc = int(bool(ndc))

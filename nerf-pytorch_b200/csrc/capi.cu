@@ -129,7 +129,8 @@ static bool is_tc(int precision) { return precision == NERF_B200_PREC_TC_FP16 ||
 static PackLayout pack_layout_for(const NerfNetParams& net, int precision) {
   return precision == NERF_B200_PREC_TC_SPLIT ? make_pack_layout_split(net) : make_pack_layout(net);
 }
-#define NB_SPLIT_TRAIN_MSG "precision TC_SPLIT has no training-mode records: it trains through the exact backward (nerf_b200_march_bwd)"
+#define NB_SPLIT_TRAIN_MSG "precision TC_SPLIT trains through the _split entry points (split records, nerf_b200_march_bwd_split) " \
+                           "or through the exact backward (nerf_b200_march_bwd)"
 
 // The network half of a fused tensor-core pass over N rays of S samples (march, run_network, density_grid): validates it,
 // fills MarchParams' network fields from the packed image of `precision` and plans the persistent grid (whole rays per CTA,
@@ -772,21 +773,27 @@ int nerf_b200_march(const float* rays, const float* z_vals, const float* noise, 
   return march_impl(rays, z_vals, noise, N, S, net, packed, cfg, out, workspace, workspace_bytes, nullptr, stream);
 }
 
-int nerf_b200_march_train(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
-                          const void* packed, const NerfRenderCfg* cfg, const NerfPassOut* out, void* workspace,
-                          size_t workspace_bytes, const NerfTrainSave* save, void* stream) {
+// training mode of one pass: it also leaves the per-tile records of the tensor-core backward (split: the hi + lo records of
+// march_split_train_kernel for nerf_b200_march_bwd_split); `split` picks the precision the entry point takes
+static int march_train_impl(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                            const void* packed, const NerfRenderCfg* cfg, const NerfPassOut* out, void* workspace,
+                            size_t workspace_bytes, const NerfTrainSave* save, void* stream, bool split) {
   NB_CHECK_ARG(save != nullptr && out && out->raw, "training mode needs the save buffers and out->raw (the compositing adjoint reads raw)");
-  NB_CHECK_ARG(!cfg || cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
+  if (split) NB_CHECK_ARG(cfg && cfg->precision == NERF_B200_PREC_TC_SPLIT, "the split training forward needs precision TC_SPLIT");
+  else NB_CHECK_ARG(!cfg || cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
   return march_impl(rays, z_vals, noise, N, S, net, packed, cfg, out, workspace, workspace_bytes, save, stream);
 }
 
-// precision TC_SPLIT in training mode (march_split_train_kernel): the split records for nerf_b200_march_bwd_split
+int nerf_b200_march_train(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
+                          const void* packed, const NerfRenderCfg* cfg, const NerfPassOut* out, void* workspace,
+                          size_t workspace_bytes, const NerfTrainSave* save, void* stream) {
+  return march_train_impl(rays, z_vals, noise, N, S, net, packed, cfg, out, workspace, workspace_bytes, save, stream, false);
+}
+
 int nerf_b200_march_train_split(const float* rays, const float* z_vals, const float* noise, int64_t N, int S, const NerfNetParams* net,
                                 const void* packed, const NerfRenderCfg* cfg, const NerfPassOut* out, void* workspace,
                                 size_t workspace_bytes, const NerfTrainSave* save, void* stream) {
-  NB_CHECK_ARG(save != nullptr && out && out->raw, "training mode needs the save buffers and out->raw (the compositing adjoint reads raw)");
-  NB_CHECK_ARG(cfg && cfg->precision == NERF_B200_PREC_TC_SPLIT, "the split training forward needs precision TC_SPLIT");
-  return march_impl(rays, z_vals, noise, N, S, net, packed, cfg, out, workspace, workspace_bytes, save, stream);
+  return march_train_impl(rays, z_vals, noise, N, S, net, packed, cfg, out, workspace, workspace_bytes, save, stream, true);
 }
 
 int nerf_b200_train_record_bytes_split(int64_t N, int S, const NerfNetParams* net, size_t* act_bytes, size_t* mask_bytes) {
@@ -903,17 +910,27 @@ int nerf_b200_render_fwd(const NerfRayGen* gen, float* rays, int64_t N, const Ne
 }
 
 // the same call in training mode: both passes also leave their per-tile records (activation images + ReLU masks) for
-// nerf_b200_march_bwd_tc, and must write raw (coarse->raw, fine->raw)
+// the tensor-core backward, and must write raw (coarse->raw, fine->raw).  The refusals of both training entries; `split`
+// picks the precision the entry takes.
+static int check_fwd_train(const NerfRenderCfg* cfg, const NerfPassOut* coarse, const NerfPassOut* fine,
+                           const NerfTrainSave* save_coarse, const NerfTrainSave* save_fine, bool split) {
+  if (split) NB_CHECK_ARG(cfg && cfg->precision == NERF_B200_PREC_TC_SPLIT, "the split training forward needs precision TC_SPLIT");
+  else {
+    NB_CHECK_ARG(cfg && cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
+    NB_CHECK_ARG(cfg->precision == NERF_B200_PREC_TC_FP16, "training-mode records belong to the tensor-core path");
+  }
+  NB_CHECK_ARG(save_coarse && coarse && coarse->raw, "training mode needs save_coarse and coarse->raw");
+  NB_CHECK_ARG(cfg->N_importance == 0 || (save_fine && fine && fine->raw), "training mode needs save_fine and fine->raw");
+  return 0;
+}
+
 int nerf_b200_render_rays_fwd_train(const float* rays, int64_t N, const NerfRenderCfg* cfg, const NerfNetParams* net_coarse,
                                     const void* packed_coarse, const NerfNetParams* net_fine, const void* packed_fine,
                                     const float* t_vals, const float* u_det, const float* t_rand, const float* u_rand,
                                     const float* noise0, const float* noise1, float* z_coarse, const NerfPassOut* coarse,
                                     float* z_fine, float* z_std, const NerfPassOut* fine, void* workspace,
                                     size_t workspace_bytes, const NerfTrainSave* save_coarse, const NerfTrainSave* save_fine, void* stream) {
-  NB_CHECK_ARG(cfg && cfg->precision != NERF_B200_PREC_TC_SPLIT, NB_SPLIT_TRAIN_MSG);
-  NB_CHECK_ARG(cfg && cfg->precision == NERF_B200_PREC_TC_FP16, "training-mode records belong to the tensor-core path");
-  NB_CHECK_ARG(save_coarse && coarse && coarse->raw, "training mode needs save_coarse and coarse->raw");
-  NB_CHECK_ARG(cfg->N_importance == 0 || (save_fine && fine && fine->raw), "training mode needs save_fine and fine->raw");
+  if (int rc = check_fwd_train(cfg, coarse, fine, save_coarse, save_fine, false)) return rc;
   return render_rays_fwd_impl(rays, N, cfg, net_coarse, packed_coarse, net_fine, packed_fine, t_vals, u_det, t_rand, u_rand, noise0, noise1,
                               z_coarse, coarse, z_fine, z_std, fine, workspace, workspace_bytes, save_coarse, save_fine, stream);
 }
@@ -924,9 +941,7 @@ int nerf_b200_render_rays_fwd_train_split(const float* rays, int64_t N, const Ne
                                           const float* noise0, const float* noise1, float* z_coarse, const NerfPassOut* coarse,
                                           float* z_fine, float* z_std, const NerfPassOut* fine, void* workspace,
                                           size_t workspace_bytes, const NerfTrainSave* save_coarse, const NerfTrainSave* save_fine, void* stream) {
-  NB_CHECK_ARG(cfg && cfg->precision == NERF_B200_PREC_TC_SPLIT, "the split training forward needs precision TC_SPLIT");
-  NB_CHECK_ARG(save_coarse && coarse && coarse->raw, "training mode needs save_coarse and coarse->raw");
-  NB_CHECK_ARG(cfg->N_importance == 0 || (save_fine && fine && fine->raw), "training mode needs save_fine and fine->raw");
+  if (int rc = check_fwd_train(cfg, coarse, fine, save_coarse, save_fine, true)) return rc;
   return render_rays_fwd_impl(rays, N, cfg, net_coarse, packed_coarse, net_fine, packed_fine, t_vals, u_det, t_rand, u_rand, noise0, noise1,
                               z_coarse, coarse, z_fine, z_std, fine, workspace, workspace_bytes, save_coarse, save_fine, stream);
 }

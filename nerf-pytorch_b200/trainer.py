@@ -8,7 +8,7 @@ no autograd graph and no per-tensor optimizer:
 
     pack weights -> pack rays -> z sampling -> fused pass (coarse, training mode) -> resampling -> fused pass (fine)
     -> fused MSE + gradient seed (both terms) -> tensor-core backward of both passes into ONE flat gradient buffer
-    (precision tc_split with set_backward('tc_split'): the split training image, split records and the split backward)
+    (the fp16 path, or under precision tc_split with set_backward('tc_split') the split one: api._train_path)
     -> [one all-reduce of that buffer when data parallel] -> flat Adam with the decayed rate computed on the device
 
 captured once per ray count and replayed.  The constructor's `n_rays` is the capacity: the buffers hold that many rays and
@@ -99,24 +99,18 @@ class FusedTrainStep:
         if not isinstance(self.net_c, api.NeRF):
             raise RuntimeError("FusedTrainStep needs nerf_b200.NeRF networks (with or without view directions)")
         self.use_viewdirs = bool(self.net_c.use_viewdirs)
-        # tc_split trains here only with its tensor-core backward; every other combination keeps the tc_fp16 requirement
-        self.split = api.get_precision() == "tc_split" and api.get_backward() == "tc_split"
-        if api.get_precision() != "tc_fp16" and not self.split:
-            raise RuntimeError("FusedTrainStep runs the tensor-core path (set_precision('tc_fp16'), or set_precision('tc_split') with "
-                               "set_backward('tc_split'))")
-        self._sfx = "_split" if self.split else ""     # the library entries of the split path
-        self.dev = self.net_c._check_device()
-        self.H, self.W, self.K, self.N = int(H), int(W), K, int(n_rays)
         self.Sc, self.Ni = int(kw["N_samples"]), int(kw.get("N_importance", 0))
         if self.Ni > 0 and self.net_f is None:
             self.net_f = self.net_c
-        if self.Ni > 0 and bool(self.net_f.use_viewdirs) != self.use_viewdirs:
-            raise RuntimeError("FusedTrainStep: coarse and fine networks must agree on use_viewdirs (they share the ray batch)")
+        self.path = api._train_path(api.get_precision(), api.get_backward(), True, self.net_c, self.net_f if self.Ni > 0 else None,
+                                    fused=True)
+        self.dev = self.net_c._check_device()
+        self.H, self.W, self.K, self.N = int(H), int(W), K, int(n_rays)
         self.ray_stride = 11 if self.use_viewdirs else 8
         q = kw.get("network_query_fn")
         self.cfgd = dict(N_samples=self.Sc, N_importance=self.Ni, multires=int(getattr(q, "multires", 10)),
                          multires_views=int(getattr(q, "multires_views", 4)), lindisp=bool(kw.get("lindisp", False)),
-                         perturb=float(kw.get("perturb", 0.)), white_bkgd=bool(kw.get("white_bkgd", False)), retraw=True, want_grad=True)
+                         perturb=float(kw.get("perturb", 0.)), white_bkgd=bool(kw.get("white_bkgd", False)), retraw=True)
         self.noise_std = float(kw.get("raw_noise_std", 0.))
         self.ndc, self.near, self.far = int(bool(kw.get("ndc", True))), float(kw.get("near", 0.)), float(kw.get("far", 1.))
         self.lr0, self.decay_rate, self.decay_steps = float(lrate), 0.1, float(lrate_decay) * 1000.0
@@ -165,12 +159,12 @@ class FusedTrainStep:
         self._out_f = NerfPassOut(api._ptr(o["rgb"]), api._ptr(o["disp"]), api._ptr(o["acc"]), C.c_void_p(0), C.c_void_p(0), api._ptr(o["raw"]))
         self._np_c, self._np_f = self.net_c.net_params(), (self.net_f.net_params() if self.Ni > 0 else None)
         lib = self.lib
-        self._pack_fn = getattr(lib, "nerf_b200_pack_weights" + ("_split_train" if self.split else ""))
-        packed_bytes = getattr(lib, "nerf_b200_packed_bytes" + ("_split_train" if self.split else ""))
+        self._pack_fn = getattr(lib, self.path.pack_weights)
+        packed_bytes = getattr(lib, self.path.packed_bytes)
         self._pk_c = torch.empty(packed_bytes(C.byref(self._np_c)), dtype=torch.uint8, device=self.dev)
         self._pk_f = self._pk_c if (self.Ni == 0 or self.net_f is self.net_c) else \
             torch.empty(packed_bytes(C.byref(self._np_f)), dtype=torch.uint8, device=self.dev)
-        # the split backward takes its seeds as NerfOutGrads (dL/drgb_map of each pass)
+        # the seeds of a path without an rgb-only backward (split): NerfOutGrads of dL/drgb_map of each pass
         self._og_c = _lib.NerfOutGrads(rgb_map=api._ptr(o["g_rgb0"]))
         self._og_f = _lib.NerfOutGrads(rgb_map=api._ptr(o["g_rgb"]))
         # every buffer above has the rays as its leading dimension, so an n-ray step (n <= N) runs on their first n rows, which
@@ -203,25 +197,20 @@ class FusedTrainStep:
         b = {}
         with api._on(self.rays):
             for tag, S, np_ in (("c", self.Sc, self._np_c), ("f", Sf, self._np_f))[:1 + fine]:
-                ab, mb = C.c_size_t(0), C.c_size_t(0)
-                check(getattr(lib, "nerf_b200_train_record_bytes" + self._sfx)(n, S, C.byref(np_), C.byref(ab), C.byref(mb)),
-                      "train_record_bytes" + self._sfx)
-                b["act_" + tag], b["mask_" + tag] = buf("act_" + tag, ab.value), buf("mask_" + tag, mb.value)
+                ab, mb = api._record_bytes(lib, self.path, n, S, np_)
+                b["act_" + tag], b["mask_" + tag] = buf("act_" + tag, ab), buf("mask_" + tag, mb)
             b["ws"] = buf("ws", lib.nerf_b200_march_workspace_bytes(n, Sf))
-            bw = getattr(lib, "nerf_b200_render_rays_bwd_" + ("split" if self.split else "tc") + "_workspace_bytes")(n, self.Sc, C.byref(self._np_c), Sf if fine else 0,
-                                                                  C.byref(self._np_f) if fine else None)
+            bw = getattr(lib, self.path.bwd_ws)(n, self.Sc, C.byref(self._np_c), Sf if fine else 0, C.byref(self._np_f) if fine else None)
             b["bws"] = buf("bws", bw + 1024)
         if cap is not None and all(b[k] is cap[k] for k in b):
             return cap
         o = self.out
         b["sv_c"] = api._records_save(b["act_c"], b["mask_c"])
-        b["bp_c"] = _lib.NerfBwdPass(api._ptr(self.z_c), api._ptr(self.noise0), self.Sc, C.pointer(self._np_c), api._ptr(self._pk_c),
-                                     api._ptr(o["raw0"]), C.pointer(b["sv_c"]), api._ptr(o["g_rgb0"]), C.pointer(self._gs[0]))
+        b["bp_c"] = api._bwd_pass(self.z_c, self.noise0, self.Sc, self._np_c, self._pk_c, o["raw0"], b["sv_c"], o["g_rgb0"], self._gs[0])
         b["sv_f"] = b["bp_f"] = None
         if fine:
             b["sv_f"] = api._records_save(b["act_f"], b["mask_f"])
-            b["bp_f"] = _lib.NerfBwdPass(api._ptr(self.z_f), api._ptr(self.noise1), Sf, C.pointer(self._np_f), api._ptr(self._pk_f),
-                                         api._ptr(o["raw"]), C.pointer(b["sv_f"]), api._ptr(o["g_rgb"]), C.pointer(self._gs[-1]))
+            b["bp_f"] = api._bwd_pass(self.z_f, self.noise1, Sf, self._np_f, self._pk_f, o["raw"], b["sv_f"], o["g_rgb"], self._gs[-1])
         return b
 
     def _capture(self, n, pool=None, keep_rng=False):
@@ -277,13 +266,12 @@ class FusedTrainStep:
             if self.noise1 is not None:
                 self.noise1[:n].normal_().mul_(self.noise_std)
             fine = self.Ni > 0
-            check(getattr(lib, "nerf_b200_render_rays_fwd_train" + self._sfx)(
-                api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(self._np_c), api._ptr(self._pk_c),
-                C.byref(self._np_f) if fine else None, api._ptr(self._pk_f) if fine else None,
-                api._ptr(self.t_vals), api._ptr(self.u_det), api._ptr(self.t_rand), api._ptr(self.u_rand), api._ptr(self.noise0), api._ptr(self.noise1),
-                api._ptr(self.z_c), C.byref(self._out_c), api._ptr(self.z_f) if fine else None, api._ptr(self.z_std) if fine else None,
-                C.byref(self._out_f) if fine else None, api._ptr(b["ws"]), b["ws"].numel(),
-                C.byref(b["sv_c"]), C.byref(b["sv_f"]) if fine else None, st), "render_rays_fwd_train" + self._sfx)
+            api._call(lib, self.path.fwd, api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(self._np_c), api._ptr(self._pk_c),
+                      C.byref(self._np_f) if fine else None, api._ptr(self._pk_f) if fine else None,
+                      api._ptr(self.t_vals), api._ptr(self.u_det), api._ptr(self.t_rand), api._ptr(self.u_rand), api._ptr(self.noise0),
+                      api._ptr(self.noise1), api._ptr(self.z_c), C.byref(self._out_c), api._ptr(self.z_f) if fine else None,
+                      api._ptr(self.z_std) if fine else None, C.byref(self._out_f) if fine else None, api._ptr(b["ws"]), b["ws"].numel(),
+                      C.byref(b["sv_c"]), C.byref(b["sv_f"]) if fine else None, st)
             # loss = img2mse(rgb, target) + img2mse(rgb0, target)  (run_nerf.py:764-772), means over the n rays, and its gradient seeds
             self.state[0:1].zero_()
             self.flat_g.zero_()
@@ -292,15 +280,11 @@ class FusedTrainStep:
             if fine:
                 check(lib.nerf_b200_mse_seed(api._ptr(o["rgb"]), api._ptr(self.target), n, gscale, api._ptr(o["g_rgb"]), api._ptr(self.state), st), "mse_seed")
             check(lib.nerf_b200_mse_seed(api._ptr(o["rgb0"]), api._ptr(self.target), n, gscale, api._ptr(o["g_rgb0"]), api._ptr(self.state), st), "mse_seed")
-            # backward of both passes into the flat gradient buffer (one call)
-            if self.split:
-                check(lib.nerf_b200_render_rays_bwd_split(api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(b["bp_c"]),
-                                                          C.byref(b["bp_f"]) if fine else None, C.byref(self._og_c),
-                                                          C.byref(self._og_f) if fine else None, api._ptr(b["bws"]), b["bws"].numel(), st),
-                      "render_rays_bwd_split")
-                return
-            check(lib.nerf_b200_render_rays_bwd_tc(api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(b["bp_c"]),
-                                                   C.byref(b["bp_f"]) if fine else None, api._ptr(b["bws"]), b["bws"].numel(), st), "render_rays_bwd_tc")
+            # backward of both passes into the flat gradient buffer (one call): the seeds in NerfBwdPass.g_rgb where the path has an
+            # rgb-only backward, else as NerfOutGrads
+            seeds = () if self.path.bwd_rgb else (C.byref(self._og_c), C.byref(self._og_f) if fine else None)
+            api._call(lib, self.path.bwd_rgb or self.path.bwd, api._ptr(self.packed_rays), n, C.byref(cfg), C.byref(b["bp_c"]),
+                      C.byref(b["bp_f"]) if fine else None, *seeds, api._ptr(b["bws"]), b["bws"].numel(), st)
 
     def _adam(self):
         with api._on(self.rays):
