@@ -131,6 +131,17 @@ int nerf_b200_marching_cubes_emit(const float* sigma, const float* xs, const flo
                                   int nx, int ny, int nz, float iso, float* verts, int64_t max_verts,
                                   int32_t* faces, int64_t max_faces, void* workspace, size_t workspace_bytes,
                                   void* stream);
+/* The density and its gradient at P arbitrary points pts [P,3] (vertex normals: n = -grad / |grad|):  */
+/* sigma [P] = raw[..., 3] of nerf_b200_run_network in FP32 (pre-ReLU, no noise), grad [P,3] =        */
+/* dsigma/dx.  Always the exact fp32 path, whatever the precision: the exact forward with saved       */
+/* activations, then its backward chain seeded with the density head.  Any net the exact path        */
+/* serves; L = multires (0 for i_embed = -1).  Points go in slabs of 16384, so the workspace is at    */
+/* most 512 + 16384 * (2 input_ch + D W + 2 W + 4) * 4 bytes for any P; it must start on a 16-byte    */
+/* boundary.  No atomics: the same bits on every run.  Refusals (NULL pointers, P < 0, a small       */
+/* workspace, a net the exact path refuses) come before any launch; P = 0 does nothing.              */
+size_t nerf_b200_density_gradient_workspace_bytes(int64_t P, const NerfNetParams* net);
+int nerf_b200_density_gradient(const float* pts, int64_t P, const NerfNetParams* net, int L,
+                               float* sigma, float* grad, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- raw2outputs (run_nerf.py:262-305) and its adjoint (SURVEY App. E) ------------------------ */
 /* raw [N,S,4], z_vals [N,S], rays_d row pointer with stride `d_stride` floats, noise [N,S]|NULL.  */

@@ -87,6 +87,8 @@ SIGNATURES = {
     "nerf_b200_marching_cubes_count": (C.c_int, [c_fp, C.c_int, C.c_int, C.c_int, C.c_float, c_fp, c_fp, C.c_size_t, c_fp]),
     "nerf_b200_marching_cubes_emit": (C.c_int, [c_fp, c_fp, c_fp, c_fp, C.c_int, C.c_int, C.c_int, C.c_float, c_fp, C.c_int64,
                                                 c_fp, C.c_int64, c_fp, C.c_size_t, c_fp]),
+    "nerf_b200_density_gradient_workspace_bytes": (C.c_size_t, [C.c_int64, C.POINTER(NerfNetParams)]),
+    "nerf_b200_density_gradient": (C.c_int, [c_fp, C.c_int64, C.POINTER(NerfNetParams), C.c_int, c_fp, c_fp, c_fp, C.c_size_t, c_fp]),
     "nerf_b200_raw2outputs": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, c_fp, C.c_int64, C.c_int, C.c_int,
                                         C.POINTER(NerfPassOut), c_fp]),
     "nerf_b200_raw2outputs_bwd": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, c_fp, C.c_int64, C.c_int, C.c_int, c_fp, c_fp, c_fp]),

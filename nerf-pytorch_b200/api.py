@@ -31,7 +31,7 @@ __all__ = ["NeRF", "Embedder", "get_embedder", "sample_pdf", "raw2outputs", "run
            "batchify_rays", "render_rays", "render", "create_nerf",
            "img2mse", "mse2psnr", "to8b", "set_precision", "get_precision", "set_backward", "get_backward",
            "launch_count", "DEBUG", "GraphedRender", "render_to8b", "DeviceRayBatcher", "density_grid", "marching_cubes",
-           "extract_mesh", "save_ply"]
+           "extract_mesh", "save_ply", "density_gradient", "vertex_attributes"]
 
 DEBUG = False
 _PRECISION = {"mode": PREC_TC_FP16}
@@ -1293,16 +1293,82 @@ def extract_mesh(network_fn, network_query_fn, xs, ys, zs, iso):
     return marching_cubes(density_grid(network_fn, network_query_fn, xs, ys, zs), xs, ys, zs, iso)
 
 
-def save_ply(path, verts, faces):
-    """Write a triangle mesh (verts [V, 3], faces [F, 3]; tensors or arrays) as binary little-endian PLY."""
-    v = np.ascontiguousarray(verts.detach().cpu().numpy() if torch.is_tensor(verts) else verts, dtype="<f4").reshape(-1, 3)
-    f = np.asarray(faces.detach().cpu().numpy() if torch.is_tensor(faces) else faces).reshape(-1, 3)
+@torch.no_grad()
+def density_gradient(network_fn, network_query_fn, pts):
+    """(sigma [...], grad [..., 3]) of `network_fn` at pts [..., 3] (float32, on pts' device): sigma = run_network(pts)[..., 3] in
+    fp32, the pre-ReLU density without noise, and grad = dsigma/dx through the network and the positional encoding.  Always the
+    exact fp32 path, whatever set_precision says, so the same bits in every precision and on every run; any net the exact path
+    serves.  `multires` is read from `network_query_fn` as density_grid reads it."""
+    if not isinstance(network_fn, NeRF):
+        raise RuntimeError("nerf_b200.density_gradient: network must be a nerf_b200.NeRF")
+    pts = _f32c(pts, "pts")
+    if pts.shape[-1] != 3:
+        raise RuntimeError(f"nerf_b200.density_gradient: pts must be [..., 3] (got shape {tuple(pts.shape)})")
+    mr = getattr(network_query_fn, "multires", None)
+    if mr is None:
+        mr = (network_fn.input_ch - 3) // 6
+    P = pts.numel() // 3
+    sigma = torch.empty(pts.shape[:-1], device=pts.device, dtype=torch.float32)
+    grad = torch.empty(pts.shape, device=pts.device, dtype=torch.float32)
+    if P == 0:
+        return sigma, grad
+    lib = _lib.load()
+    n = network_fn.net_params()
+    ws_bytes = lib.nerf_b200_density_gradient_workspace_bytes(P, C.byref(n))
+    ws = _workspace(ws_bytes, pts.device)
+    with _on(pts):
+        _call(lib, "nerf_b200_density_gradient", _ptr(pts), P, C.byref(n), int(mr), _ptr(sigma), _ptr(grad), _ptr(ws), ws_bytes,
+              _stream(pts))
+    return sigma, grad
+
+
+@torch.no_grad()
+def vertex_attributes(network_fn, network_query_fn, verts):
+    """(normals [V, 3], colors [V, 3]) of the mesh vertices verts [V, 3], for save_ply.  normals = -grad / |grad| of
+    density_gradient (toward decreasing density, as marching_cubes winds its faces), 0 where |grad| is 0 or not finite.  colors
+    = sigmoid(run_network(verts, viewdirs = -normals)[..., :3]) in the current set_precision: the view head looking at the
+    surface head-on from outside; a vertex without a normal is seen along a zero view direction (as density_grid's points are),
+    and a net without view directions takes none.  Usually network_fn = render_kwargs_test['network_fine']."""
+    verts = _f32c(verts, "verts")
+    if verts.dim() != 2 or verts.shape[1] != 3:
+        raise RuntimeError(f"nerf_b200.vertex_attributes: verts must be [V, 3] (got shape {tuple(verts.shape)})")
+    _, grad = density_gradient(network_fn, network_query_fn, verts)
+    norm = grad.norm(dim=-1, keepdim=True)
+    ok = torch.isfinite(norm) & (norm > 0)
+    zero = torch.zeros_like(grad)
+    look = torch.where(ok, grad / norm, zero)                         # the viewing ray's direction, -normal
+    normals = torch.where(ok, -look, zero)
+    raw = network_query_fn(verts[:, None], look if network_fn.use_viewdirs else None, network_fn)
+    return normals, torch.sigmoid(raw[:, 0, :3])
+
+
+def save_ply(path, verts, faces, normals=None, colors=None):
+    """Write a triangle mesh (verts [V, 3], faces [F, 3]; tensors or arrays) as binary little-endian PLY, with optional
+    per-vertex normals [V, 3] (float properties nx ny nz) and colors [V, 3] in [0, 1] (uchar red green blue, converted as
+    to8b converts images)."""
+    def host(a):
+        return a.detach().cpu().numpy() if torch.is_tensor(a) else np.asarray(a)
+    v = np.ascontiguousarray(host(verts), dtype="<f4").reshape(-1, 3)
+    f = host(faces).reshape(-1, 3)
+    fields, props = [("p", "<f4", (3,))], "property float x\nproperty float y\nproperty float z\n"
+    if normals is not None:
+        fields.append(("n", "<f4", (3,)))
+        props += "property float nx\nproperty float ny\nproperty float nz\n"
+    if colors is not None:
+        fields.append(("c", "u1", (3,)))
+        props += "property uchar red\nproperty uchar green\nproperty uchar blue\n"
+    vrec = np.empty(len(v), dtype=fields)
+    vrec["p"] = v
+    if normals is not None:
+        vrec["n"] = host(normals).reshape(-1, 3)
+    if colors is not None:
+        vrec["c"] = to8b(host(colors).astype(np.float32).reshape(-1, 3))
     rec = np.empty(len(f), dtype=[("n", "u1"), ("idx", "<i4", (3,))])
     rec["n"] = 3
     rec["idx"] = f
-    header = (f"ply\nformat binary_little_endian 1.0\nelement vertex {len(v)}\nproperty float x\nproperty float y\n"
-              f"property float z\nelement face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
+    header = (f"ply\nformat binary_little_endian 1.0\nelement vertex {len(v)}\n{props}"
+              f"element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
     with open(path, "wb") as fh:
         fh.write(header.encode("ascii"))
-        fh.write(v.tobytes())
+        fh.write(vrec.tobytes())
         fh.write(rec.tobytes())

@@ -128,6 +128,38 @@ __global__ void sum_partials_kernel(const float* __restrict__ part, int nparts, 
   dst[(size_t)(idx / cols) * ld + idx % cols] += s;
 }
 
+// ---- the density gradient dsigma/dx at arbitrary points (nerf_b200_density_gradient) ----
+// The chain is the exact backward's (gemm_nn, the ReLU mask); these two kernels are its first and last step.
+
+// dA[m, c] = (h[m, c] > 0) * w_sigma[c]: dsigma / d(pre-activation of the last pts layer), w_sigma the density head's row
+__global__ void __launch_bounds__(256) sigma_seed_kernel(const float* __restrict__ h, const float* __restrict__ w_sigma, long long M,
+                                                         int W, float* __restrict__ dA) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M * W) return;
+  dA[i] = h[i] > 0.0f ? w_sigma[i % W] : 0.0f;
+}
+
+// grad[m, j] = dsigma/dx_j from d_enc [M, IC] = dsigma/d(encoding) through the encoding's Jacobian (run_nerf_helpers.py:36-45,
+// columns x, then sin and cos of 2^k x per octave k < L, 3 wide each): d_enc[x_j] + sum_k 2^k (cos(a) d_enc[sin_kj] -
+// sin(a) d_enc[cos_kj]), a = 2^k x_j formed as mlp_simt_kernel forms it.  Octaves are added in order: the same bits every run.
+__global__ void __launch_bounds__(256) enc_jacobian_kernel(const float* __restrict__ d_enc, int IC, int L, const float* __restrict__ pts,
+                                                           long long M, float* __restrict__ grad) {
+  const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  const float* d = d_enc + m * IC;
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const float x = pts[m * 3 + j];
+    float g = d[j];
+    for (int k = 0; k < L; ++k) {
+      const float s = exp2f((float)k), a = __fmul_rn(x, s);
+      const float t = __fmaf_rn(cosf(a), d[3 + 6 * k + j], -__fmul_rn(sinf(a), d[6 + 6 * k + j]));
+      g = __fmaf_rn(s, t, g);
+    }
+    grad[m * 3 + j] = g;
+  }
+}
+
 // activations saved by the exact forward (row-major fp32), all optional
 struct SimtSave {
   float* enc;    // [M, IC]

@@ -985,12 +985,13 @@ static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, i
   NB_LAUNCH_OK("sgemm_tn_kernel");
   return part ? sum_partials(part, nslab, K1, N, C, ldc, st) : 0;
 }
+// colsum NULL: the ReLU mask alone, no partials (scratch may be NULL)
 static int mask_colsum(float* d, int ldd, const float* h, int ldh, long long M, int C, float* colsum, float* scratch,
                        long long scratch_floats, cudaStream_t st) {
   const int rpb = 256;
   const int nblk = cdiv(M, rpb);
-  float* part = nblk > 1 ? scratch : nullptr;
-  NB_CHECK_ARG(nblk == 1 || (long long)nblk * C <= scratch_floats, "internal: column-sum partials do not fit the scratch buffer");
+  float* part = (nblk > 1 && colsum) ? scratch : nullptr;
+  NB_CHECK_ARG(!colsum || nblk == 1 || (long long)nblk * C <= scratch_floats, "internal: column-sum partials do not fit the scratch buffer");
   dim3 grid(nblk, cdiv(C, 64));
   relu_mask_colsum_kernel<<<grid, 64, 0, st>>>(d, ldd, h, ldh, M, C, colsum, rpb, part);
   NB_LAUNCH_OK("relu_mask_colsum_kernel");
@@ -1096,6 +1097,74 @@ int nerf_b200_march_bwd_outs(const float* rays, const float* z_vals, const float
   (void)packed;
   NB_CHECK_ARG(g, "NULL pointer");
   return march_bwd_impl(rays, z_vals, noise, N, S, net, cfg, *g, grads, workspace, workspace_bytes, stream);
+}
+
+// ---- the density gradient at arbitrary points (exact path) ----------------------------------------
+// Slabs of up to GRAD_SLAB points: mlp_simt_kernel in save mode (enc, h; raw for sigma) with one zero view direction, the seed
+// dA_{D-1}, then march_bwd_impl's chain through pts_linears[D-1..1] (gemm_nn, ReLU mask), d_enc = dA_{s+1} W_{s+1}[:, :IC] +
+// dA_0 W_0, and the encoding's Jacobian.  Workspace: 256 B (the zero view direction) | enc [slab, IC] | h [D][slab, W] |
+// raw [slab, 4] | dA ping/pong 2 x [slab, W] | d_enc [slab, IC], each buffer on a 16-byte boundary (round4), 256 spare bytes.
+static const long long GRAD_SLAB = 1ll << 14;
+static const int GRAD_BUFFERS = 6;
+static_assert(GRAD_BUFFERS * 3 * sizeof(float) <= 256, "the workspace's spare bytes must cover the 16-byte rounding");
+
+size_t nerf_b200_density_gradient_workspace_bytes(int64_t P, const NerfNetParams* net) {
+  if (P < 0 || check_exact_net(net)) return 0;
+  const long long slab = P < GRAD_SLAB ? P : GRAD_SLAB;
+  const size_t per_row = 2 * (size_t)net->input_ch + (size_t)net->D * net->W + 2 * (size_t)net->W + 4;
+  return 256 + (size_t)slab * per_row * 4 + 256;
+}
+
+int nerf_b200_density_gradient(const float* pts, int64_t P, const NerfNetParams* net, int L, float* sigma, float* grad,
+                               void* workspace, size_t workspace_bytes, void* stream) {
+  NB_CHECK_ARG(pts && net && sigma && grad && workspace, "NULL pointer");
+  NB_CHECK_ARG(P >= 0, "P must be >= 0 (got %lld)", (long long)P);
+  if (int rc = check_exact_net(net)) return rc;
+  NB_CHECK_ARG(L >= 0 && 3 + 6 * L == net->input_ch, "multires %d does not match input_ch %d", L, net->input_ch);
+  const size_t need = nerf_b200_density_gradient_workspace_bytes(P, net);
+  NB_CHECK_ARG(workspace_bytes >= need, "workspace too small: need %zu bytes", need);
+  NB_CHECK_ARG(((uintptr_t)workspace & 15) == 0, "workspace must start on a 16-byte boundary");
+  if (P == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int W = net->W, IC = net->input_ch, D = net->D;
+  const long long slab = P < GRAD_SLAB ? P : GRAD_SLAB;
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  const float* zero_dir = reinterpret_cast<const float*>(ws);
+  float* p = reinterpret_cast<float*>(ws + 256);
+  SimtSave sv;
+  memset(&sv, 0, sizeof(sv));
+  sv.enc = p;            p += round4(slab * IC);
+  sv.h = p;              p += round4((long long)D * slab * W);
+  float* raw = p;        p += round4(slab * 4);
+  float* dA0 = p;        p += round4(slab * W);
+  float* dA1 = p;        p += round4(slab * W);
+  float* d_enc = p;
+  const float* w_sigma = net->use_viewdirs ? net->alpha_w : net->output_w + 3 * (size_t)W;
+  NB_CUDA(cudaMemsetAsync(ws, 0, 256, st));
+  for (long long m0 = 0; m0 < P; m0 += slab) {
+    const long long M = P - m0 < slab ? P - m0 : slab;
+    const float* x = pts + m0 * 3;
+    NB_TRY(launch_mlp_simt(x, zero_dir, 0, M, 1, *net, L, 0, raw, sv, st));
+    raw_sigma_kernel<<<cdiv(M, 256), 256, 0, st>>>(raw, M, sigma + m0);
+    NB_LAUNCH_OK("raw_sigma_kernel");
+    sigma_seed_kernel<<<cdiv(M * W, 256), 256, 0, st>>>(sv.h + (size_t)(D - 1) * M * W, w_sigma, M, W, dA0);
+    NB_LAUNCH_OK("sigma_seed_kernel");
+    // pts_linears, last to first; the skip layer's input is cat([input_pts, h]): its first IC columns go to d_enc
+    float* dcur = dA0;
+    float* dnext = dA1;
+    for (int l = D - 1; l >= 1; --l) {
+      const bool after_skip = l - 1 == net->skip;
+      const int Kl = after_skip ? W + IC : W, off = after_skip ? IC : 0;
+      if (after_skip) NB_TRY(gemm_nn(dcur, W, net->pts_w[l], Kl, d_enc, IC, M, IC, W, 0, st));
+      NB_TRY(gemm_nn(dcur, W, net->pts_w[l] + off, Kl, dnext, W, M, W, W, 0, st));
+      NB_TRY(mask_colsum(dnext, W, sv.h + (size_t)(l - 1) * M * W, W, M, W, nullptr, nullptr, 0, st));
+      float* t = dcur; dcur = dnext; dnext = t;
+    }
+    NB_TRY(gemm_nn(dcur, W, net->pts_w[0], IC, d_enc, IC, M, IC, W, net->skip >= 0 ? 1 : 0, st));
+    enc_jacobian_kernel<<<cdiv(M, 256), 256, 0, st>>>(d_enc, IC, L, x, M, grad + m0 * 3);
+    NB_LAUNCH_OK("enc_jacobian_kernel");
+  }
+  return 0;
 }
 
 // ---- tensor-core backward of one pass (bwd_wg.cuh) ------------------------------------------------
